@@ -3,8 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's engine (CUDA kernels through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU implementation of the same path
-                                                             # (the pinned CPU restatement, oracle/; /root/reference does
-                                                             #  not exist on the GPU box)
+                                                             # (its pinned CPU restatement in oracle/)
 
 One "step" is one iteration of `p_sample_loop` over one batch of 64 motions: one denoiser pass (8-layer MDM
 transformer over 64 x 197 tokens) + the posterior/noise update -- everything the reference does in one loop
@@ -82,8 +81,9 @@ def measured_peaks(timed_region_s: float):
         key = "bf16_tflops" if burst or "bf16_tflops_sustained" not in p else "bf16_tflops_sustained"
         return {"bf16_tflops": p[key], "hbm_gbs": p.get("hbm_gbs"),
                 "source": f"MEASURED_PEAKS.json {key} (cuBLAS bf16; timed region {timed_region_s:.2f} s -> {'burst' if key == 'bf16_tflops' else 'sustained'})"}
-    return {"bf16_tflops": 1650.0 if burst else 1400.0, "hbm_gbs": 6650.0,
-            "source": f"fallback of B200_PROFILING.md ({'burst' if burst else 'sustained'})"}
+    # NVIDIA's H100 SXM data sheet (dense BF16, 700 W card): an upper bound, not a rate this card was measured to reach
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0,
+            "source": f"H100 SXM data sheet, dense BF16 at 700 W ({'burst' if burst else 'sustained'} region: same figure)"}
 
 
 class NvmlSampler:
@@ -163,7 +163,7 @@ class NvmlSampler:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -465,7 +465,7 @@ def run_engine(args):
     barrier()
     w0 = time.time()
     e0.record()
-    loop(args.steps)
+    final = loop(args.steps)
     e1.record()
     barrier()
     clocks.window("timed", w0, time.time())
@@ -476,6 +476,8 @@ def run_engine(args):
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
     ms = float(tms.item())
     value = world * args.steps / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"sample": gathered if world > 1 else final})
 
     # ---- end to end through the C ABI with HOST buffers: x_T from pinned memory in, samples out ----
     x_host = torch.randn(B, D, 1, L).pin_memory()
@@ -522,14 +524,7 @@ def run_engine(args):
     dom_ms = by_kind[dom][0] / by_kind[dom][1]
     achieved = KERNEL_FLOPS[dom](B) / (dom_ms * 1e-3) / 1e12
     split = 3 if precision == C.capi.PRECISION_BF16X3 else 1
-    traffic, traffic_src = None, None
-    try:  # DRAM bytes of the dominant kernel from the committed `ncu --set full` capture (per launch, like `achieved`)
-        with open(os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")) as f:
-            tr = json.load(f)
-        if tr.get("kernel") == dom:
-            traffic, traffic_src = tr["dram_bytes_read"] + tr["dram_bytes_write"], tr["source"]
-    except (OSError, ValueError, KeyError):
-        pass
+    traffic, traffic_src = None, "not measured"
     kname = "linear_chain_kernel (out-proj + FFN1 + FFN2 + next QKV of one encoder layer)" if dom.startswith("chain") else f"linear2_kernel ({dom})"
     roofline = {"bound": "tensor", "kernel": f"{kname}, {by_kind[dom][1]} launches/step", "achieved": achieved,
                 "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["bf16_tflops"], "traffic": traffic,
@@ -562,13 +557,23 @@ def run_engine(args):
             "data": "synthetic (random-init weights, engine Philox noise)",
             "config": {"workload": WORKLOAD,
                        "global_batch": world * B, "parallelism": f"batch-sharded x{world}, one NCCL all-gather of finished samples",
-                       "l2": "per-step working set (weights 70 MB as bf16 hi+lo, activations ~0.4 GB) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (weights 70 MB as bf16 hi+lo, activations ~0.4 GB) exceeds the 50 MB L2; no explicit flush",
                        "cuda_graph": f"one captured {len(prof) + 1}-kernel step graph, replayed per step, step index on the device"},
             "clocks": clocks.summary(), "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "cpu_baseline": cpu,
             "configs": configs, "library_baseline": library}
     emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write what the timed path returned in its last step as out_dir/<name>.npy (float32), so that two builds run with
+    the same arguments (same seeds, hence the same inputs) can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def main():
@@ -579,6 +584,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "bf16"])
     ap.add_argument("--skip-configs", action="store_true", help="only configs[1]: skip the configs block and the eager-PyTorch baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the samples of the last timed step as DIR/sample.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

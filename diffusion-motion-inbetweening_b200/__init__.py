@@ -1,4 +1,4 @@
-"""condmdi_b200: B200-native sampling engine for CondMDI (setarehc/diffusion-motion-inbetweening).
+"""condmdi_b200: H100-native sampling engine for CondMDI (setarehc/diffusion-motion-inbetweening).
 
 The directory name follows the repository convention (`diffusion-motion-inbetweening_b200/`); it is imported
 as `condmdi_b200` through the shim package next to it.

@@ -1,4 +1,4 @@
-"""Build libcondmdi_b200.so (sm_100a) in-tree with nvcc.
+"""Build libcondmdi_b200.so (sm_90a, H100) in-tree with nvcc.
 
 The library is the product: every kernel of the sampling path plus the C ABI of include/condmdi_b200.h.
 It is compiled here (nvcc cross-compiles without a GPU) and travels to the GPU box with the tree.
@@ -18,7 +18,7 @@ BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcondmdi_b200.so")
 SOURCES = ["gemm2.cu", "gemm_chain.cu", "attention.cu", "elementwise.cu", "unet_kernels.cu", "backward.cu", "attention_bwd_tc.cu", "attention_bwd_simt_test.cu", "tma_host.cu", "capi_test.cu", "engine.cu"]
 HEADERS = ["common.cuh", "kernels.h", "gemm_epilogue.cuh", "engine_unet.inc", os.path.join("..", "..", "include", "condmdi_b200.h")]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 

@@ -2,7 +2,7 @@
 //
 // The engine never launches it (the sampling path uses attention_bwd_tc.cu); it is the INDEPENDENT implementation
 // `cmdi_test_attention_bwd` (capi_test.cu, CMDI_TEST_ATTN_BWD_SIMT=1) runs so that tests/test_gpu_kernels.py can hold the
-// tcgen05 kernel against a second, structurally different device implementation as well as against torch autograd.
+// wgmma kernel against a second, structurally different device implementation as well as against torch autograd.
 #include "common.cuh"
 #include "kernels.h"
 

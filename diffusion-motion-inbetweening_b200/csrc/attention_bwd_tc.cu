@@ -1,27 +1,24 @@
-// Backward of the attention core on tcgen05 tensor cores (reconstruction guidance only: the denoiser's input-VJP,
+// Backward of the attention core on wgmma tensor cores (reconstruction guidance only: the denoiser's input-VJP,
 // gaussian_diffusion.py:411-416 runs autograd through nn.MultiheadAttention here).
 //
 //   S = Q K^T / sqrt(128)   P = softmax_rows(S)   O = P V
 //   dV = P^T dO    dP = dO V^T    delta_i = sum_j P_ij dP_ij    dS = P o (dP - delta) / sqrt(128)
 //   dQ = dS K      dK = dS^T Q
 //
-// Two launches of one kernel, each CTA owning a 128-row tile of one (sequence, head):
-//   mode 0 (rows = queries): X = Q_t K^T, Y = dO_t V^T; row statistics (max, sum, delta) by the two threads of a
-//           row; dS -> TMEM (bf16 hi/lo, aliasing Y); dQ_t = dS K (A from TMEM, K MN-major from the tile that served
-//           X).  Writes lse2_i = max*c + log2(sum) and delta_i per query row for mode 1.
+// Two launches of one kernel, each CTA owning a 128-row tile of one (sequence, head), 64 rows per warpgroup:
+//   mode 0 (rows = queries): X = Q_t K^T, Y = dO_t V^T; row statistics (max, sum, delta) by the four threads of a row (a
+//           quad of the wgmma fragment); dS in registers -> bf16 hi/lo A fragments; dQ_t = dS K (K MN-major from the tile
+//           that served X).  Writes lse2_i = max*c + log2(sum) and delta_i per query row for mode 1.
 //   mode 1 (rows = keys):    X = K_t Q^T = S^T, Y = V_t dO^T = dP^T; P^T = exp2(c X - lse2_i) and dS^T with the
 //           per-column statistics of mode 0; dV_t = P^T dO in two 64-column halves, dK_t = dS^T Q.
-// Every product uses the bf16 hi/lo operand split (3 MMAs), fp32 accumulation in TMEM.
+// Every product uses the bf16 hi/lo operand split (3 MMAs), fp32 accumulation in registers.
 //
-// Shared memory (225 KB, one CTA per SM):
-//   R_A  64 KB: the 128-row tile operand of X (hi, lo), then of Y, then the store staging
+// Shared memory (220 KB, one CTA per SM):
+//   R_A  64 KB: the 128-row tile operand of X (hi, lo), then of Y
 //   R_B 104 KB: the 208-row operand of X (hi, lo); stays resident as the MN-major B operand of dQ / dK
 //   R_C  52 KB: the 208-row operand of Y, streamed one 64-column block (hi + lo) at a time; in mode 1 the
 //               same blocks are streamed a second time as the MN-major B operand of dV
-// TMEM: X [0,208) (P^T hi/lo alias it in mode 1; the dQ / dK accumulator reuses [0,128) afterwards),
-//       Y [208,416) (dS hi/lo alias it), dV half accumulator [416,480).
 #include "common.cuh"
-#include "gemm_epilogue.cuh"
 #include "kernels.h"
 
 namespace cmdi {
@@ -31,183 +28,92 @@ namespace {
 constexpr int kHeadDim = 128;
 constexpr int kTile = 128;
 constexpr int kPad = kAttnKeyPad;             // 208 = 13 * 16
+constexpr int kKeyBlocks = kPad / 16;
 constexpr int kTBlk = kTile * 128;            // 16384: 64 head-dim columns of a 128-row tile
 constexpr int kFBlk = kPad * 128;             // 26624: 64 head-dim columns of a 208-row operand
 constexpr int kOffAHi = 0, kOffALo = 2 * kTBlk;
 constexpr int kOffBHi = 4 * kTBlk, kOffBLo = kOffBHi + 2 * kFBlk;
 constexpr int kOffCHi = kOffBLo + 2 * kFBlk, kOffCLo = kOffCHi + kFBlk;
 constexpr int kSmemTiles = kOffCLo + kFBlk;   // 225280
-constexpr int kNumEwWarps = 8;
-constexpr int kThreads = 64 + kNumEwWarps * 32;
-constexpr uint32_t kColX = 0, kColXHi = 0, kColXLo = 104, kColY = 208, kColYHi = 208, kColYLo = 312, kColC0 = 416;
-constexpr uint32_t kTmemCols = 512;
-constexpr int kChunks0 = 7, kChunks1 = 6;     // 16-column chunks per half-row thread
+constexpr int kThreads = 256;
 
 struct __align__(8) BwdBarriers {
-  uint64_t x_full[2], a2_full, c_full, x_done, y_done[2], p_full, o1_done[2], c0_free, out_done;
-  uint32_t tmem_base;
-  uint32_t pad;
-  float red_a[2][128];
-  float red_b[2][128];
+  uint64_t x_full, a2_full, c_full;
   float col_lse[kPad];
   float col_delta[kPad];
 };
 
-__device__ __forceinline__ void named_barrier(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+// bf16 hi / lo A fragments (m64k16, see common.cuh) of key block t from an accumulator-layout row fragment v
+__device__ __forceinline__ void to_frags(const float (&v)[kPad / 2], uint32_t (&hi)[kKeyBlocks][4], uint32_t (&lo)[kKeyBlocks][4]) {
+#pragma unroll
+  for (int t = 0; t < kKeyBlocks; ++t)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int i = 8 * t + 4 * (q >> 1) + 2 * (q & 1);
+      split_bf16x2(v[i], v[i + 1], hi[t][q], lo[t][q]);
+    }
 }
 
-// write this thread's NCHUNKS*16 values as bf16 hi/lo pairs into TMEM (chunk c -> 8 packed columns)
-template <int CHUNK0, int NCHUNKS>
-__device__ __forceinline__ void store_split(uint32_t trow, uint32_t col_hi, uint32_t col_lo, bool split, const float* s) {
+// D (+)= A[64 x 208] B^T with the A operand of this warpgroup at a_off (+ k-block kb) and B at b_off, three bf16 terms
+__device__ __forceinline__ void mma_x(float (&d)[kPad / 2], uint32_t sbase, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                      int kb0, int kb1, uint32_t a_blk, uint32_t b_blk, bool split, bool first) {
+  const int nterms = split ? 3 : 1;
 #pragma unroll
-  for (int c = 0; c < NCHUNKS; ++c) {
-    uint32_t ph[8], pl[8];
+  for (int term = 0; term < 3; ++term) {
+    if (term >= nterms) break;
+    const uint32_t ao = (split && term == 0) ? a_lo : a_hi;
+    const uint32_t bo = (split && term == 1) ? b_lo : b_hi;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      const uint64_t da = make_desc_kmajor_sw128(sbase + ao + kb * a_blk);
+      const uint64_t db = make_desc_kmajor_sw128(sbase + bo + kb * b_blk);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) split_bf16x2(s[c * 16 + j * 2], s[c * 16 + j * 2 + 1], ph[j], pl[j]);
-    tmem_st8(trow + col_hi + (CHUNK0 + c) * 8, ph);
-    if (split) tmem_st8(trow + col_lo + (CHUNK0 + c) * 8, pl);
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n208k16_ss(d, desc_advance(da, kk * 32), desc_advance(db, kk * 32), (first && term == 0 && kb == kb0 && kk == 0) ? 0u : 1u);
+    }
   }
 }
 
-template <int CHUNK0, int NCHUNKS>
-__device__ __forceinline__ void elementwise_half(const AttnBwdParams& p, int mode, uint32_t trow, BwdBarriers* bars, int half,
-                                                 int row, bool row_valid, long long stat_index, bool split) {
-  const int S = p.seq_len;
-  const float c_exp = 0.08838834764831845f * 1.4426950408889634f;  // log2(e) / sqrt(128)
-  const float c_scale = 0.08838834764831845f;
-  float s[NCHUNKS * 16];
-  // ---- X -> registers ----
-  mbar_wait(&bars->x_done, 0);
-  tc_fence_after();
-  {
-    uint32_t v[NCHUNKS][16];
+// D = A[64 x 208 keys] (registers, hi / lo) * B[208 x N] (MN-major in shared memory), three bf16 terms
+template <int N>
+__device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&ah)[kKeyBlocks][4], const uint32_t (&al)[kKeyBlocks][4],
+                                       uint32_t b_hi, uint32_t b_lo, bool split) {
+  const uint64_t dh = make_desc_mnmajor_sw128(b_hi, kFBlk);
+  const uint64_t dl = make_desc_mnmajor_sw128(b_lo, kFBlk);
+  wgmma_fence_operands(d);
+  wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < NCHUNKS; ++c) tmem_ld16(trow + kColX + (CHUNK0 + c) * 16, v[c]);
-    tmem_ld_wait();
-#pragma unroll
-    for (int c = 0; c < NCHUNKS; ++c)
-#pragma unroll
-      for (int j = 0; j < 16; ++j) s[c * 16 + j] = __uint_as_float(v[c][j]);
+  for (int t = 0; t < kKeyBlocks; ++t) {
+    if constexpr (N == 128) {
+      if (split) wgmma_m64n128k16_rs_tb(d, al[t], desc_advance(dh, t * 2048), t ? 1u : 0u);
+      wgmma_m64n128k16_rs_tb(d, ah[t], desc_advance(dh, t * 2048), (split || t) ? 1u : 0u);
+      if (split) wgmma_m64n128k16_rs_tb(d, ah[t], desc_advance(dl, t * 2048), 1u);
+    } else {
+      if (split) wgmma_m64n64k16_rs_tb(d, al[t], desc_advance(dh, t * 2048), t ? 1u : 0u);
+      wgmma_m64n64k16_rs_tb(d, ah[t], desc_advance(dh, t * 2048), (split || t) ? 1u : 0u);
+      if (split) wgmma_m64n64k16_rs_tb(d, ah[t], desc_advance(dl, t * 2048), 1u);
+    }
   }
-  float inv = 1.f, delta = 0.f;
-  if (mode == 0) {
-    // row softmax: the two threads of a row exchange max and sum
-    float mx = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < NCHUNKS * 16; ++i) {
-      if (CHUNK0 * 16 + i >= S) s[i] = -INFINITY;  // padded keys
-      mx = fmaxf(mx, s[i]);
-    }
-    bars->red_a[half][row] = mx;
-    named_barrier(1, kNumEwWarps * 32);
-    mx = fmaxf(bars->red_a[0][row], bars->red_a[1][row]);
-    const float mc = mx * c_exp;
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < NCHUNKS * 16; ++i) {
-      s[i] = fast_exp2(fmaf(s[i], c_exp, -mc));
-      sum += s[i];
-    }
-    // ---- Y: delta = sum_j P_ij dP_ij ----
-    mbar_wait(&bars->y_done[1], 0);
-    tc_fence_after();
-    float dsum = 0.f;
-#pragma unroll
-    for (int c = 0; c < NCHUNKS; ++c) {
-      uint32_t v[16];
-      tmem_ld16(trow + kColY + (CHUNK0 + c) * 16, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j) dsum = fmaf(s[c * 16 + j], __uint_as_float(v[j]), dsum);
-    }
-    bars->red_b[half][row] = sum;
-    named_barrier(1, kNumEwWarps * 32);          // (also: every thread is past its reads of red_a)
-    const float l = bars->red_b[0][row] + bars->red_b[1][row];
-    inv = 1.0f / l;
-    bars->red_a[half][row] = dsum;
-    named_barrier(1, kNumEwWarps * 32);
-    delta = (bars->red_a[0][row] + bars->red_a[1][row]) * inv;
-    if (half == 0 && row_valid) {
-      p.stats[stat_index] = make_float2(mc + log2f(l), delta);
-    }
-    // ---- dS = P (dP - delta) / sqrt(d), in place of P ----
-#pragma unroll
-    for (int c = 0; c < NCHUNKS; ++c) {
-      uint32_t v[16];
-      tmem_ld16(trow + kColY + (CHUNK0 + c) * 16, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        s[c * 16 + j] = s[c * 16 + j] * inv * (__uint_as_float(v[j]) - delta) * c_scale;
-    }
-    tc_fence_before();
-    named_barrier(1, kNumEwWarps * 32);          // every Y value has been read: dS may overwrite the Y columns
-    tc_fence_after();
-    store_split<CHUNK0, NCHUNKS>(trow, kColYHi, kColYLo, split, s);
-  } else {
-    // column statistics of mode 0 (lse2 = +inf for padded queries -> P = 0)
-#pragma unroll
-    for (int i = 0; i < NCHUNKS * 16; ++i) s[i] = fast_exp2(fmaf(s[i], c_exp, -bars->col_lse[CHUNK0 * 16 + i]));
-    tc_fence_before();
-    named_barrier(1, kNumEwWarps * 32);          // every X value has been read: P^T may overwrite the X columns
-    tc_fence_after();
-    store_split<CHUNK0, NCHUNKS>(trow, kColXHi, kColXLo, split, s);
-    mbar_wait(&bars->y_done[1], 0);
-    tc_fence_after();
-#pragma unroll
-    for (int c = 0; c < NCHUNKS; ++c) {
-      uint32_t v[16];
-      tmem_ld16(trow + kColY + (CHUNK0 + c) * 16, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        s[c * 16 + j] = s[c * 16 + j] * (__uint_as_float(v[j]) - bars->col_delta[(CHUNK0 + c) * 16 + j]) * c_scale;
-    }
-    tc_fence_before();
-    named_barrier(1, kNumEwWarps * 32);
-    tc_fence_after();
-    store_split<CHUNK0, NCHUNKS>(trow, kColYHi, kColYLo, split, s);
-  }
-  tmem_st_wait();
-  tc_fence_before();
-  mbar_arrive(&bars->p_full);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_operands(d);
 }
 
-// drain a 32-row x 64-column fp32 accumulator block of this warp to the bf16 planes
-__device__ __forceinline__ void drain_block(const AttnBwdParams& p, const CUtensorMap* map_o_hi, const CUtensorMap* map_o_lo,
-                                            uint32_t taddr, uint32_t stage, int lane, int tile_row0, int lane_group, int row0,
-                                            int out_col) {
-  uint32_t v0[32], v1[32];
-  tmem_ld32(taddr, v0);
-  tmem_ld32(taddr + 32, v1);
-  tmem_ld_wait();
-  uint32_t hw[32], lw[32];
+// rows r0 = 16 w + lane / 4 and r0 + 8 of the warpgroup's 64: fp32 accumulator columns -> bf16 hi / lo planes
+template <int N>
+__device__ __forceinline__ void store_rows(const AttnBwdParams& p, const float (&d)[N / 2], int tile_row0, int row0, int out_col, int lane) {
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    split_bf16x2(__uint_as_float(v0[2 * j]), __uint_as_float(v0[2 * j + 1]), hw[j], lw[j]);
-    split_bf16x2(__uint_as_float(v1[2 * j]), __uint_as_float(v1[2 * j + 1]), hw[16 + j], lw[16 + j]);
-  }
-  const int S = p.seq_len;
-  const int group_row0 = tile_row0 + lane_group * 32;
-  if (group_row0 + 32 <= S) {
-    store_block_tma(stage, lane, hw, map_o_hi, out_col, row0 + group_row0);
-    store_block_tma(stage, lane, lw, map_o_lo, out_col, row0 + group_row0);
-    if (lane == 0) tma_store_wait_read();
-  } else if (group_row0 < S) {
-    RowSlots rows;
-    rows.ok = 0;
+  for (int g = 0; g < 2; ++g) {
+    const int r = tile_row0 + 8 * g;
+    if (r >= p.seq_len) continue;
+    const size_t off = (size_t)(row0 + r) * p.ld_dqkv + out_col + 2 * (lane & 3);
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const int q = group_row0 + r * 4 + (lane >> 3);
-      rows.row[r] = (q < S) ? (row0 + q) : 0;
-      if (q < S) rows.ok |= 1u << r;
+    for (int j = 0; j < N / 8; ++j) {
+      uint32_t hw, lw;
+      split_bf16x2(d[4 * j + 2 * g], d[4 * j + 2 * g + 1], hw, lw);
+      *reinterpret_cast<uint32_t*>(p.dqkv_hi + off + 8 * j) = hw;
+      *reinterpret_cast<uint32_t*>(p.dqkv_lo + off + 8 * j) = lw;
     }
-    const long long pitch = (long long)p.ld_dqkv * 2;
-    store_block_coalesced(stage, lane, hw, reinterpret_cast<char*>(p.dqkv_hi + out_col), rows, pitch, 8, 1, 0);
-    store_block_coalesced(stage, lane, lw, reinterpret_cast<char*>(p.dqkv_lo + out_col), rows, pitch, 8, 1, 0);
   }
-  __syncwarp();
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -215,14 +121,14 @@ attention_bwd_tc_kernel(const __grid_constant__ CUtensorMap qkv_t_hi, const __gr
                         const __grid_constant__ CUtensorMap qkv_f_hi, const __grid_constant__ CUtensorMap qkv_f_lo,
                         const __grid_constant__ CUtensorMap do_t_hi, const __grid_constant__ CUtensorMap do_t_lo,
                         const __grid_constant__ CUtensorMap do_f_hi, const __grid_constant__ CUtensorMap do_f_lo,
-                        const __grid_constant__ CUtensorMap out_hi, const __grid_constant__ CUtensorMap out_lo,
                         const AttnBwdParams p, const int mode) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   BwdBarriers* bars = reinterpret_cast<BwdBarriers*>(smem + kSmemTiles);
+  const uint32_t sbase = smem_u32(smem);
 
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp_idx >> 2, w = warp_idx & 3;
   const int tile = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
   const int S = p.seq_len, H = p.num_heads;
   const bool split = (p.nsplit == 3);
@@ -230,239 +136,168 @@ attention_bwd_tc_kernel(const __grid_constant__ CUtensorMap qkv_t_hi, const __gr
   const int q_col = head * kHeadDim, k_col = H * kHeadDim + head * kHeadDim, v_col = 2 * H * kHeadDim + head * kHeadDim;
   const int do_col = head * kHeadDim;
   // mode 0: A1 = Q tile, B1 = K, A2 = dO tile, B2 = V.   mode 1: A1 = K tile, B1 = Q, A2 = V tile, B2 = dO.
-  const CUtensorMap* a1_hi = &qkv_t_hi;
-  const CUtensorMap* a1_lo = &qkv_t_lo;
-  const CUtensorMap* b1_hi = &qkv_f_hi;
-  const CUtensorMap* b1_lo = &qkv_f_lo;
   const CUtensorMap* a2_hi = mode == 0 ? &do_t_hi : &qkv_t_hi;
   const CUtensorMap* a2_lo = mode == 0 ? &do_t_lo : &qkv_t_lo;
   const CUtensorMap* b2_hi = mode == 0 ? &qkv_f_hi : &do_f_hi;
   const CUtensorMap* b2_lo = mode == 0 ? &qkv_f_lo : &do_f_lo;
   const int a1_col = mode == 0 ? q_col : k_col, b1_col = mode == 0 ? k_col : q_col;
   const int a2_col = mode == 0 ? do_col : v_col, b2_col = mode == 0 ? v_col : do_col;
+  const uint32_t planes = split ? 2 : 1;
+  auto load_c = [&](int blk) {  // one 64-column block (hi + lo) of the 208-row Y operand
+    mbar_arrive_expect_tx(&bars->c_full, planes * kFBlk);
+    tma_load_2d(smem + kOffCHi, b2_hi, &bars->c_full, b2_col + blk * 64, row0);
+    if (split) tma_load_2d(smem + kOffCLo, b2_lo, &bars->c_full, b2_col + blk * 64, row0);
+  };
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&qkv_t_hi);
     tma_prefetch_desc(&qkv_f_hi);
-    mbar_init(&bars->x_full[0], 1);
-    mbar_init(&bars->x_full[1], 1);
+    mbar_init(&bars->x_full, 1);
     mbar_init(&bars->a2_full, 1);
     mbar_init(&bars->c_full, 1);
-    mbar_init(&bars->x_done, 1);
-    mbar_init(&bars->y_done[0], 1);
-    mbar_init(&bars->y_done[1], 1);
-    mbar_init(&bars->p_full, kNumEwWarps * 32);
-    mbar_init(&bars->o1_done[0], 1);
-    mbar_init(&bars->o1_done[1], 1);
-    mbar_init(&bars->c0_free, 4);
-    mbar_init(&bars->out_done, 1);
     fence_barrier_init();
+    mbar_arrive_expect_tx(&bars->x_full, planes * 2 * (kTBlk + kFBlk));
+    for (int j = 0; j < 2; ++j) {
+      tma_load_2d(smem + kOffAHi + j * kTBlk, &qkv_t_hi, &bars->x_full, a1_col + j * 64, row0 + tile * kTile);
+      tma_load_2d(smem + kOffBHi + j * kFBlk, &qkv_f_hi, &bars->x_full, b1_col + j * 64, row0);
+      if (split) {
+        tma_load_2d(smem + kOffALo + j * kTBlk, &qkv_t_lo, &bars->x_full, a1_col + j * 64, row0 + tile * kTile);
+        tma_load_2d(smem + kOffBLo + j * kFBlk, &qkv_f_lo, &bars->x_full, b1_col + j * 64, row0);
+      }
+    }
+    load_c(0);
   }
-  if (warp_idx == 1) {
-    tmem_alloc(&bars->tmem_base, kTmemCols);
-    tmem_relinquish();
-  }
-  if (mode == 1 && warp_idx >= 2) {
-    // per-query statistics written by the mode-0 launch
-    for (int i = threadIdx.x - 64; i < kPad; i += kNumEwWarps * 32) {
+  if (mode == 1) {
+    // per-query statistics written by the mode-0 launch (lse2 = +inf for padded queries -> P = 0)
+    for (int i = threadIdx.x; i < kPad; i += kThreads) {
       float2 st = make_float2(INFINITY, 0.f);
       if (i < S) st = p.stats[(long long)(row0 + i) * H + head];
       bars->col_lse[i] = st.x;
       bars->col_delta[i] = st.y;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
-  const uint32_t planes = split ? 2 : 1;
 
-  if (warp_idx == 0) {
-    if (lane == 0) {
-      auto load_c = [&](int blk) {  // one 64-column block (hi + lo) of the 208-row Y operand
-        mbar_arrive_expect_tx(&bars->c_full, planes * kFBlk);
-        tma_load_2d(smem + kOffCHi, b2_hi, &bars->c_full, b2_col + blk * 64, row0);
-        if (split) tma_load_2d(smem + kOffCLo, b2_lo, &bars->c_full, b2_col + blk * 64, row0);
-      };
-      for (int j = 0; j < 2; ++j) {
-        mbar_arrive_expect_tx(&bars->x_full[j], planes * (kTBlk + kFBlk));
-        tma_load_2d(smem + kOffAHi + j * kTBlk, a1_hi, &bars->x_full[j], a1_col + j * 64, row0 + tile * kTile);
-        tma_load_2d(smem + kOffBHi + j * kFBlk, b1_hi, &bars->x_full[j], b1_col + j * 64, row0);
-        if (split) {
-          tma_load_2d(smem + kOffALo + j * kTBlk, a1_lo, &bars->x_full[j], a1_col + j * 64, row0 + tile * kTile);
-          tma_load_2d(smem + kOffBLo + j * kFBlk, b1_lo, &bars->x_full[j], b1_col + j * 64, row0);
-        }
-      }
-      load_c(0);
-      // the operands of the later phases can only land once their shared-memory regions drain; pull them into L2 now
-      for (int j = 0; j < 2; ++j) {
-        tma_prefetch_2d(a2_hi, a2_col + j * 64, row0 + tile * kTile);
-        if (split) tma_prefetch_2d(a2_lo, a2_col + j * 64, row0 + tile * kTile);
-      }
-      tma_prefetch_2d(b2_hi, b2_col + 64, row0);
-      if (split) tma_prefetch_2d(b2_lo, b2_col + 64, row0);
-      mbar_wait(&bars->x_done, 0);   // the X MMAs no longer read R_A
-      mbar_arrive_expect_tx(&bars->a2_full, planes * 2 * kTBlk);
-      for (int j = 0; j < 2; ++j) {
-        tma_load_2d(smem + kOffAHi + j * kTBlk, a2_hi, &bars->a2_full, a2_col + j * 64, row0 + tile * kTile);
-        if (split) tma_load_2d(smem + kOffALo + j * kTBlk, a2_lo, &bars->a2_full, a2_col + j * 64, row0 + tile * kTile);
-      }
-      mbar_wait(&bars->y_done[0], 0);
-      load_c(1);
-      if (mode == 1) {
-        mbar_wait(&bars->y_done[1], 0);
-        load_c(0);
-        mbar_wait(&bars->o1_done[0], 0);
-        load_c(1);
-      }
+  const float c_exp = 0.08838834764831845f * 1.4426950408889634f;  // log2(e) / sqrt(128)
+  const float c_scale = 0.08838834764831845f;
+  const uint32_t a_wg = wg * 64 * 128;  // this warpgroup's rows of the tile operand
+  const int cq = 2 * (lane & 3);
+  const int tile_row0 = tile * kTile + wg * 64 + 16 * w + (lane >> 2);  // rows tile_row0 and tile_row0 + 8
+
+  // ---------------- X = A1 B1^T ----------------
+  float x[kPad / 2];
+  mbar_wait(&bars->x_full, 0);
+  wgmma_fence_operands(x);
+  wgmma_fence();
+  mma_x(x, sbase, kOffAHi + a_wg, kOffALo + a_wg, kOffBHi, kOffBLo, 0, 2, kTBlk, kFBlk, split, true);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_operands(x);
+  __syncthreads();  // R_A is free: the Y tile operand replaces it
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&bars->a2_full, planes * 2 * kTBlk);
+    for (int j = 0; j < 2; ++j) {
+      tma_load_2d(smem + kOffAHi + j * kTBlk, a2_hi, &bars->a2_full, a2_col + j * 64, row0 + tile * kTile);
+      if (split) tma_load_2d(smem + kOffALo + j * kTBlk, a2_lo, &bars->a2_full, a2_col + j * 64, row0 + tile * kTile);
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      const uint32_t sbase = smem_u32(smem);
-      constexpr uint32_t idesc_x = make_idesc_bf16(kTile, kPad, 0);
-      constexpr uint32_t idesc_o = make_idesc_bf16(kTile, kHeadDim, 1);
-      constexpr uint32_t idesc_h = make_idesc_bf16(kTile, 64, 1);
-      const int nterms = split ? 3 : 1;
-      // ---------------- X = A1 B1^T ----------------
-      uint32_t accum = 0;
-      for (int j = 0; j < 2; ++j) {
-        mbar_wait(&bars->x_full[j], 0);
-        tc_fence_after();
-        for (int term = 0; term < nterms; ++term) {
-          const uint32_t ao = (split && term == 0) ? kOffALo : kOffAHi;
-          const uint32_t bo = (split && term == 1) ? kOffBLo : kOffBHi;
-          const uint64_t da = make_desc_kmajor_sw128(sbase + ao + j * kTBlk);
-          const uint64_t db = make_desc_kmajor_sw128(sbase + bo + j * kFBlk);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_ss(tmem_base + kColX, desc_advance(da, kk * 32), desc_advance(db, kk * 32), idesc_x, accum);
-            accum = 1;
-          }
-        }
-      }
-      umma_commit(&bars->x_done);
-      // ---------------- Y = A2 B2^T, one 64-column block of the contraction at a time ----------------
-      mbar_wait(&bars->a2_full, 0);
-      accum = 0;
-      for (int kb = 0; kb < 2; ++kb) {
-        mbar_wait(&bars->c_full, kb & 1);
-        tc_fence_after();
-        for (int term = 0; term < nterms; ++term) {
-          const uint32_t ao = (split && term == 0) ? kOffALo : kOffAHi;
-          const uint32_t bo = (split && term == 1) ? kOffCLo : kOffCHi;
-          const uint64_t da = make_desc_kmajor_sw128(sbase + ao + kb * kTBlk);
-          const uint64_t db = make_desc_kmajor_sw128(sbase + bo);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_ss(tmem_base + kColY, desc_advance(da, kk * 32), desc_advance(db, kk * 32), idesc_x, accum);
-            accum = 1;
-          }
-        }
-        umma_commit(&bars->y_done[kb]);
-      }
-      // ---------------- products with the elementwise results as the A operand (from TMEM) ----------------
-      mbar_wait(&bars->p_full, 0);
-      tc_fence_after();
-      if (mode == 1) {
-        // dV_t = P^T dO, 64 head-dim columns at a time (R_C holds that block of dO as an MN-major B operand)
-        for (int nb = 0; nb < 2; ++nb) {
-          mbar_wait(&bars->c_full, nb & 1);  // third and fourth completion of c_full
-          if (nb == 1) mbar_wait(&bars->c0_free, 0);
-          tc_fence_after();
-          const uint64_t dh = make_desc_mnmajor_sw128(sbase + kOffCHi, kFBlk);
-          const uint64_t dl = make_desc_mnmajor_sw128(sbase + kOffCLo, kFBlk);
-          accum = 0;
-          if (split) {
-#pragma unroll 1
-            for (int ks = 0; ks < kPad / 16; ++ks) {
-              umma_ts(tmem_base + kColC0, tmem_base + kColXLo + ks * 8, desc_advance(dh, ks * 2048), idesc_h, accum);
-              accum = 1;
-            }
-          }
-#pragma unroll 1
-          for (int ks = 0; ks < kPad / 16; ++ks) {
-            umma_ts(tmem_base + kColC0, tmem_base + kColXHi + ks * 8, desc_advance(dh, ks * 2048), idesc_h, accum);
-            accum = 1;
-          }
-          if (split) {
-#pragma unroll 1
-            for (int ks = 0; ks < kPad / 16; ++ks)
-              umma_ts(tmem_base + kColC0, tmem_base + kColXHi + ks * 8, desc_advance(dl, ks * 2048), idesc_h, 1u);
-          }
-          umma_commit(&bars->o1_done[nb]);
-        }
-      }
-      // dQ_t = dS K (mode 0) / dK_t = dS^T Q (mode 1): B = the resident R_B operand, MN-major; accumulator in X[0,128)
-      {
-        const uint64_t dh = make_desc_mnmajor_sw128(sbase + kOffBHi, kFBlk);
-        const uint64_t dl = make_desc_mnmajor_sw128(sbase + kOffBLo, kFBlk);
-        accum = 0;
-        if (split) {
-#pragma unroll 1
-          for (int ks = 0; ks < kPad / 16; ++ks) {
-            umma_ts(tmem_base + kColX, tmem_base + kColYLo + ks * 8, desc_advance(dh, ks * 2048), idesc_o, accum);
-            accum = 1;
-          }
-        }
-#pragma unroll 1
-        for (int ks = 0; ks < kPad / 16; ++ks) {
-          umma_ts(tmem_base + kColX, tmem_base + kColYHi + ks * 8, desc_advance(dh, ks * 2048), idesc_o, accum);
-          accum = 1;
-        }
-        if (split) {
-#pragma unroll 1
-          for (int ks = 0; ks < kPad / 16; ++ks)
-            umma_ts(tmem_base + kColX, tmem_base + kColYHi + ks * 8, desc_advance(dl, ks * 2048), idesc_o, 1u);
-        }
-        umma_commit(&bars->out_done);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int ew = warp_idx - 2;
-    const int lane_group = warp_idx & 3;
-    const int half = ew >> 2;
-    const int row = lane_group * 32 + lane;
-    const uint32_t trow = tmem_base + ((uint32_t)(lane_group * 32) << 16);
-    const int tile_row = tile * kTile + row;
-    const bool row_valid = tile_row < S;
-    const long long stat_index = (long long)(row0 + tile_row) * H + head;
-    if (half == 0) {
-      elementwise_half<0, kChunks0>(p, mode, trow, bars, 0, row, row_valid, stat_index, split);
-    } else {
-      elementwise_half<kChunks0, kChunks1>(p, mode, trow, bars, 1, row, row_valid, stat_index, split);
-    }
-    // ---------------- outputs ----------------
-    // y_done[1] has completed (waited above): R_A is free and becomes the store-staging area (8 x 4 KB)
-    const uint32_t stage = smem_u32(smem + kOffAHi + ew * kEpiStageBytes);
-    if (mode == 1) {
-      // dV half `half` is drained by the four warps of that half (32 rows x 64 columns each)
-      mbar_wait(&bars->o1_done[half], 0);
-      tc_fence_after();
-      drain_block(p, &out_hi, &out_lo, trow + kColC0, stage, lane, tile * kTile, lane_group, row0, v_col + half * 64);
-      if (half == 0) {
-        tc_fence_before();
-        if (lane == 0) mbar_arrive(&bars->c0_free);
-      }
-    }
-    mbar_wait(&bars->out_done, 0);
-    tc_fence_after();
-    drain_block(p, &out_hi, &out_lo, trow + kColX + half * 64, stage, lane, tile * kTile, lane_group, row0,
-                (mode == 0 ? q_col : k_col) + half * 64);
-    if (lane == 0) tma_store_wait_all();
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  // ---------------- probabilities (unnormalised in mode 0) ----------------
+  float mc0 = 0.f, mc1 = 0.f, sum0 = 0.f, sum1 = 0.f;
+  if (mode == 0) {
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < kPad / 8; ++j) {
+      if (8 * j + cq >= S) { x[4 * j] = -INFINITY; x[4 * j + 2] = -INFINITY; }  // padded keys
+      if (8 * j + cq + 1 >= S) { x[4 * j + 1] = -INFINITY; x[4 * j + 3] = -INFINITY; }
+      mx0 = fmaxf(mx0, fmaxf(x[4 * j], x[4 * j + 1]));
+      mx1 = fmaxf(mx1, fmaxf(x[4 * j + 2], x[4 * j + 3]));
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
+    }
+    mc0 = mx0 * c_exp; mc1 = mx1 * c_exp;
+#pragma unroll
+    for (int i = 0; i < kPad / 2; ++i) {
+      x[i] = fast_exp2(fmaf(x[i], c_exp, -((i & 2) ? mc1 : mc0)));
+      if (i & 2) sum1 += x[i]; else sum0 += x[i];
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+      sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < kPad / 2; ++i) x[i] = fast_exp2(fmaf(x[i], c_exp, -bars->col_lse[8 * (i >> 2) + cq + (i & 1)]));
+  }
+
+  // ---------------- Y = A2 B2^T, one 64-column block of the contraction at a time ----------------
+  float y[kPad / 2];
+  mbar_wait(&bars->a2_full, 0);
+  for (int kb = 0; kb < 2; ++kb) {
+    mbar_wait(&bars->c_full, kb & 1);
+    wgmma_fence_operands(y);
+    wgmma_fence();
+    mma_x(y, sbase, kOffAHi + a_wg, kOffALo + a_wg, kOffCHi, kOffCLo, kb, kb + 1, kTBlk, 0, split, kb == 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(y);
+    __syncthreads();  // R_C is free
+    if (threadIdx.x == 0 && (kb == 0 || mode == 1)) load_c(kb ^ 1);  // mode 1: dO block 0 again, for dV
+  }
+
+  uint32_t ah[kKeyBlocks][4], al[kKeyBlocks][4];
+  if (mode == 0) {
+    // delta = sum_j P_ij dP_ij, dS = P (dP - delta) / sqrt(d)
+    float d0 = 0.f, d1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < kPad / 2; ++i) {
+      if (i & 2) d1 = fmaf(x[i], y[i], d1); else d0 = fmaf(x[i], y[i], d0);
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      d0 += __shfl_xor_sync(0xffffffffu, d0, o);
+      d1 += __shfl_xor_sync(0xffffffffu, d1, o);
+    }
+    const float inv0 = 1.0f / sum0, inv1 = 1.0f / sum1;
+    const float delta0 = d0 * inv0, delta1 = d1 * inv1;
+    if ((lane & 3) == 0) {
+      if (tile_row0 < S) p.stats[(long long)(row0 + tile_row0) * H + head] = make_float2(mc0 + log2f(sum0), delta0);
+      if (tile_row0 + 8 < S) p.stats[(long long)(row0 + tile_row0 + 8) * H + head] = make_float2(mc1 + log2f(sum1), delta1);
+    }
+#pragma unroll
+    for (int i = 0; i < kPad / 2; ++i) y[i] = x[i] * ((i & 2) ? inv1 : inv0) * (y[i] - ((i & 2) ? delta1 : delta0)) * c_scale;
+    to_frags(y, ah, al);
+    // dQ_t = dS K: B = the resident R_B operand, MN-major
+    float acc[kHeadDim / 2];
+    mma_rs<kHeadDim>(acc, ah, al, sbase + kOffBHi, sbase + kOffBLo, split);
+    store_rows<kHeadDim>(p, acc, tile_row0, row0, q_col, lane);
+  } else {
+    // dS^T = P^T (dP^T - delta_i) / sqrt(d)
+#pragma unroll
+    for (int i = 0; i < kPad / 2; ++i) y[i] = x[i] * (y[i] - bars->col_delta[8 * (i >> 2) + cq + (i & 1)]) * c_scale;
+    to_frags(x, ah, al);
+    // dV_t = P^T dO, 64 head-dim columns at a time (R_C holds that block of dO as an MN-major B operand)
+    for (int nb = 0; nb < 2; ++nb) {
+      mbar_wait(&bars->c_full, nb & 1);  // third and fourth completion of c_full
+      float acc[32];
+      mma_rs<64>(acc, ah, al, sbase + kOffCHi, sbase + kOffCLo, split);
+      __syncthreads();
+      if (threadIdx.x == 0 && nb == 0) load_c(1);
+      store_rows<64>(p, acc, tile_row0, row0, v_col + nb * 64, lane);
+    }
+    to_frags(y, ah, al);
+    // dK_t = dS^T Q: B = the resident R_B operand, MN-major
+    float acc[kHeadDim / 2];
+    mma_rs<kHeadDim>(acc, ah, al, sbase + kOffBHi, sbase + kOffBLo, split);
+    store_rows<kHeadDim>(p, acc, tile_row0, row0, k_col, lane);
   }
 }
 
 }  // namespace
-
 
 cudaError_t configure_attention_bwd_tc_kernel() {
   return cudaFuncSetAttribute(attention_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -478,7 +313,7 @@ cudaError_t launch_attention_bwd_tc(const AttnBwdTcMaps& m, const AttnBwdParams&
   dim3 grid((p.seq_len + kTile - 1) / kTile, p.num_heads, p.num_seqs);
   for (int mode = 0; mode < 2; ++mode) {
     attention_bwd_tc_kernel<<<grid, kThreads, smem, stream>>>(*m.qkv_t_hi, *m.qkv_t_lo, *m.qkv_f_hi, *m.qkv_f_lo, *m.do_t_hi,
-                                                               *m.do_t_lo, *m.do_f_hi, *m.do_f_lo, *m.out_hi, *m.out_lo, p, mode);
+                                                               *m.do_t_lo, *m.do_f_hi, *m.do_f_lo, p, mode);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }

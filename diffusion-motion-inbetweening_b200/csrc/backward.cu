@@ -2,7 +2,7 @@
 //   g = d/dz sum((x_obs - x0_hat(z))^2 * M) -- a backward pass through ClassifierFreeSampleModel(MDM) w.r.t. its input).
 //
 // Only dX is needed (no weight gradients).  The matrix products of the backward pass (dX = dY W for every linear)
-// run on the same tcgen05 linear kernels as the forward pass, against transposed weight planes; this file holds
+// run on the same wgmma linear kernels as the forward pass, against transposed weight planes; this file holds
 // the rest:
 //   guidance_seed_kernel   dL/dx0_hat = -2 (x_obs - x0_hat) * M, split over the CFG cond / uncond outputs
 //   layernorm512_bwd       dX of LayerNorm from the stashed pre-norm input
@@ -154,7 +154,7 @@ __global__ void __launch_bounds__(256) transpose_split_kernel(const float* __res
 cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t stream) {
   const size_t n = (size_t)p.B * p.L * p.D_pad;
   size_t grid = (n + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   guidance_seed_kernel<<<(unsigned)grid, 256, 0, stream>>>(p);
   return cudaGetLastError();
 }

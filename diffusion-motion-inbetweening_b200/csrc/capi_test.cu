@@ -42,7 +42,7 @@ struct DevBuf {
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 int num_sms_of_current_device() {
-  int dev = 0, n = 148;
+  int dev = 0, n = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
   return n;

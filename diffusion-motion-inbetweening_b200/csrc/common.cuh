@@ -1,9 +1,8 @@
-// Device-side primitives for the sm_100a kernels of the CondMDI sampling engine.
+// Device-side primitives for the sm_90a kernels of the CondMDI sampling engine.
 //
-// Everything here is a thin wrapper over one PTX instruction: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences) and the
-// shared-memory + instruction descriptors the 5th-gen tensor cores consume.
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptors" tables.
+// Everything here is a thin wrapper over one PTX instruction: mbarrier, TMA (cp.async.bulk.tensor), wgmma
+// (warpgroup MMA: fence / issue / commit / wait) and the shared-memory matrix descriptors the Hopper tensor cores
+// consume.  Descriptor bit layouts follow the PTX ISA "matrix descriptor format" table for wgmma.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -155,34 +154,16 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 // ... and have completed their global writes
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
-// ----------------------------------------------------------------------------------------------
-// Whole warp executes. ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: descriptors
+// wgmma: shared-memory matrix descriptors
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
+// 64-bit descriptor:
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (sm_100)
-//   [49,52) base offset = 0 (tiles are 1024 B aligned)   [61,64) swizzle: 2 = 128 B
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset = 0 (tiles are 1024 B aligned)   [62,64) swizzle: 1 = 128 B
 //
 // K-major operand, 128 B swizzle (tile written by a TMA box of 64 bf16 x rows):
-//   row r at byte r*128, 16 B chunks XOR-swizzled by (r & 7); 8-row atoms 1024 B apart -> SBO = 1024.
+//   row r at byte r*128, 16 B chunks XOR-swizzled by (r & 7); 8-row groups SBO bytes apart (1024 for dense rows).
 //   LBO is unused for swizzled K-major layouts (set to 1 like CUTLASS does).
 // MN-major operand, 128 B swizzle (TMA box of 64 contiguous MN-elements x K rows):
 //   K index k at byte k*128 inside a 64-wide MN group -> SBO = 1024 (8 K-rows),
@@ -192,12 +173,18 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
 __device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) {
   return make_smem_desc(smem_addr, 16, 1024);
+}
+// A 128-row K-major tile read as two m64 operands whose 8-row groups interleave: operand h (start + h * 1024) covers
+// rows {16 g + 8 h + i : g < 8, i < 8}.  Warp w of the consuming warpgroup then holds accumulator rows 32 w .. 32 w + 31
+// of the tile (fragment rows 16 w + i -> 32 w + 8 h + i, 16 w + 8 + i -> 32 w + 16 + 8 h + i): the same rows a warp
+// owns in the epilogue's row-per-thread layout (see acc_rows_to_lanes).
+__device__ __forceinline__ uint64_t make_desc_kmajor_sw128_interleaved(uint32_t smem_addr) {
+  return make_smem_desc(smem_addr, 16, 2048);
 }
 __device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t mn_group_stride_bytes) {
   return make_smem_desc(smem_addr, mn_group_stride_bytes, 1024);
@@ -205,97 +192,151 @@ __device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr, 
 // advance a descriptor's start address by `bytes` (must keep the result inside the 14-bit field)
 __device__ __forceinline__ uint64_t desc_advance(uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); }
 
-// Instruction descriptor for kind::f16 with BF16 operands and FP32 accumulation.
-//   [4,6) c_format = 1 (F32)   [7,10) a_format = 1 (BF16)   [10,13) b_format = 1 (BF16)
-//   [15] a_major (0 = K)   [16] b_major (0 = K, 1 = MN)   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
 // ----------------------------------------------------------------------------------------------
-// tcgen05: MMA issue / commit (single thread)
+// wgmma: issue / commit / wait (warpgroup-collective)
 // ----------------------------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Accumulator fragment of an m64nN tile, thread t of the warpgroup (warp w = t / 32, lane l):
+//   d[4 j + 0, 1] = (row 16 w + l / 4,     columns 8 j + 2 (l % 4) + {0, 1})
+//   d[4 j + 2, 3] = (row 16 w + 8 + l / 4, the same columns)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem]   (A: lane = row, each 32-bit column holds two consecutive K elements)
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all tcgen05 ops previously issued by this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// register budget of a warpgroup role (setmaxnreg: producer warps give registers to the MMA / epilogue warpgroups)
+template <int N>
+__device__ __forceinline__ void warpgroup_reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void warpgroup_reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+__device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers (warp-collective; warp w touches lanes 32*(w%4) .. +31)
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive 32-bit columns: thread i gets row (lane base + i), v[j] = column j
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+// D (+)= A * B with both operands in shared memory, K-major (scale_d = 0: D = A * B)
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-// 32 lanes x 8 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma_m64n208k16_ss(float (&d)[104], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-      "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),
-      "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]),
-      "r"(v[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %106, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n208k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103}, %104, %105, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+// A from registers (a[0..3]: the m64k16 bf16 fragment), B MN-major in shared memory
+__device__ __forceinline__ void wgmma_m64n128k16_rs_tb(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+// A from registers (a[0..3]: the m64k16 bf16 fragment), B MN-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 
-// TMEM address = (lane << 16) | column
-__device__ __forceinline__ uint32_t tmem_addr(uint32_t base, uint32_t lane, uint32_t col) {
-  return base + (lane << 16) + col;
+// One 64-deep k-block of a 128-row x PART_N tile for one warpgroup (A: interleaved 128-row K-major tile, B: PART_N
+// K-major rows; a_plane / b_plane: offsets of the lo planes), with nterms = split ? 3 : 1 bf16 products (lo*hi, hi*lo,
+// hi*hi).  The tensor cores accumulate each 64-column chunk of the k-block in a fresh register fragment, which is then
+// added into acc0 / acc1 with fp32 adds on the CUDA cores.  The tensor cores' own fp32 accumulation rounds toward zero:
+// carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
+// instead, the bias stays at the level of a 64-long sum.
+// One 64-deep k-block of a 128-row x PART_N tile for one warpgroup (A: interleaved 128-row K-major tile, B: PART_N
+// K-major rows; a_plane / b_plane: offsets of the lo planes), with nterms = split ? 3 : 1 bf16 products (lo*hi, hi*lo,
+// hi*hi).  The tensor cores accumulate each 64-column chunk of the k-block in a fresh register fragment, which is then
+// added into acc0 / acc1 with fp32 adds on the CUDA cores.  The tensor cores' own fp32 accumulation rounds toward zero:
+// carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
+// instead, the bias stays at the level of a 64-long sum.  (Measured on H100: double-buffering 32-column chunks so that
+// the adds of one chunk overlap the MMAs of the next is no faster.)
+template <int PART_N>
+__device__ __forceinline__ void mma_kblock_promoted(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], uint32_t sa, uint32_t sb,
+                                                    uint32_t a_plane, uint32_t b_plane, bool split) {
+  static_assert(PART_N % 64 == 0, "64-column chunks");
+  const int nterms = split ? 3 : 1;
+#pragma unroll
+  for (int c = 0; c < PART_N / 64; ++c) {
+    float t0[32], t1[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { t0[i] = 0.f; t1[i] = 0.f; }
+    wgmma_fence_operands(t0);
+    wgmma_fence_operands(t1);
+    wgmma_fence();
+#pragma unroll
+    for (int term = 0; term < 3; ++term) {
+      if (term >= nterms) break;
+      const uint64_t da = make_desc_kmajor_sw128_interleaved(sa + ((split && term == 0) ? a_plane : 0u));
+      const uint64_t db = make_desc_kmajor_sw128(sb + ((split && term == 1) ? b_plane : 0u) + c * 64 * 128);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        wgmma_m64n64k16_ss(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
+        wgmma_m64n64k16_ss(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(t0);
+    wgmma_fence_operands(t1);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      acc0[32 * c + i] += t0[i];
+      acc1[32 * c + i] += t1[i];
+    }
+  }
+}
+
+// The 32 accumulator values of one warp for 32 columns [8 j0, 8 j0 + 32) of an interleaved 128-row tile (acc0 / acc1: the
+// two m64 halves, see make_desc_kmajor_sw128_interleaved) -> row-per-lane layout: lane i receives row 32 w + i,
+// v[c] = column c.  Through the warp's 4 KB staging tile (16-byte chunks XOR-swizzled by row & 7).
+template <int R>
+__device__ __forceinline__ void acc_rows_to_lanes(const float (&acc0)[R], const float (&acc1)[R], int j0, uint32_t stage, int lane,
+                                                  uint32_t (&v)[32]) {
+  __syncwarp();
+  const int q = lane >> 2, c2 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float(&a)[R] = h ? acc1 : acc0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        const int r = 16 * g + 8 * h + q, c = 8 * j + c2;
+        const uint32_t addr = stage + r * 128 + ((((uint32_t)c >> 2) ^ ((uint32_t)r & 7u)) << 4) + (c & 3) * 4;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a[4 * (j0 + j) + 2 * g]), "f"(a[4 * (j0 + j) + 2 * g + 1])
+                     : "memory");
+      }
+    }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    uint32_t x, y, z, w;
+    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w)
+                 : "r"(stage + lane * 128 + (((uint32_t)k ^ ((uint32_t)lane & 7u)) << 4)) : "memory");
+    v[4 * k] = x; v[4 * k + 1] = y; v[4 * k + 2] = z; v[4 * k + 3] = w;
+  }
+  __syncwarp();
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -306,72 +347,6 @@ __device__ __forceinline__ void st_global_v4(void* p, uint32_t a, uint32_t b, ui
 }
 __device__ __forceinline__ void st_global_v4f(float* p, float a, float b, float c, float d) {
   asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-}  // namespace cmdi
-
-// ==============================================================================================
-// CTA-pair (cta_group::2) variants: two SMs of one cluster cooperate on one 256-row MMA tile
-// ==============================================================================================
-namespace cmdi {
-
-// In the shared::cluster window bit 24 of a CTA-local shared address selects the odd CTA of a pair;
-// clearing it addresses the same offset in the even ("leader") CTA.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load issued by either CTA of the pair; the transaction bytes are counted on the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the leader CTA's copy of `bar` (works from both CTAs of the pair)
-__device__ __forceinline__ void mbar_arrive_on_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem, 256 rows over both CTAs] (+)= A[smem of both CTAs] * B[smem of both CTAs]; issued by the leader only
-__device__ __forceinline__ void umma_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ... with A read from tensor memory (each CTA's lanes hold its 128 rows of A)
-__device__ __forceinline__ void umma_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on `bar` in every CTA of `cta_mask` once the pair's previously issued MMAs have completed
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
 }
 
 }  // namespace cmdi

@@ -601,7 +601,7 @@ __global__ void __launch_bounds__(256) recover_from_ric_kernel(const RicParams p
 
 inline int grid_for(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (g < 1) g = 1;
   return (int)g;
 }

@@ -97,7 +97,7 @@ struct GraphKey {
 
 struct cmdi_engine {
   cmdi_model_cfg cfg{};
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   int nsplit = 3;
   int bn_qkv = kBnWide;
   int debug = 0, bn_wide = kBnWide, bn_narrow = kBnNarrow;  // CMDI_DEBUG / CMDI_BN_WIDE / CMDI_BN_NARROW (bring-up knobs)
@@ -678,8 +678,8 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
   CK(cudaSetDevice(device));
   cudaDeviceProp prop{};
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_last_error("device %d is sm_%d%d; this library contains sm_100a code only (B200)", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_last_error("device %d is sm_%d%d; this library contains sm_90a code only (H100)", device, prop.major, prop.minor);
     return 1;
   }
   const bool is_unet = cfg->arch == CMDI_ARCH_UNET;

@@ -1,34 +1,33 @@
-// Several linear layers of an encoder layer in ONE persistent launch of CTA pairs (tcgen05.mma.cta_group::2).
+// Several linear layers of an encoder layer in ONE persistent launch (wgmma, 128 x 256 tiles per CTA).
 //
-// Why.  Launched one by one (gemm2.cu), every linear layer pays (a) its own tile quantisation -- QKV is 300 pair
-// tiles on 74 clusters = 4.05 rounds, i.e. 5; the N = 512 layers 2.7 rounds, i.e. 3 -- and (b) a kernel boundary
-// whose cost is the tail imbalance of the last round + the prologue + the first TMA round trip, because every one of
-// these kernels owns all shared memory and all 512 TMEM columns of its SM and a successor cannot become resident
-// early.  Here the tiles of out-proj, FFN1, FFN2 and the NEXT layer's QKV projection (or the output head) form one
-// list of 700 tiles (256 x 256 each) walked by the 74 clusters in order; the smem rings, the TMEM double buffer and the
-// warp roles simply keep running across phase boundaries.
+// Why.  Launched one by one (gemm2.cu), every linear layer pays its own tile quantisation and a kernel boundary (the
+// tail imbalance of the last round + the prologue + the first TMA round trip).  Here the tiles of out-proj, FFN1, FFN2
+// and the NEXT layer's QKV projection (or the output head) form one list of 256 x 256 tiles walked in order by CTA pairs
+// (CTA 2 c + r of pair c owns rows [128 r, 128 r + 128) of each of the pair's tiles); the smem ring and the warp roles
+// simply keep running across phase boundaries.
 //
 // Dependencies.  Phase p + 1 reads, as its A operand, rows that phase p writes.  Tiles are ordered row-pair-major
 // inside a phase; when a CTA's half of a tile is in memory it bumps a per-(phase, row-pair) counter, and the TMA
 // producer of a consuming tile spins on that counter (acquire) before it issues the first load of the tile.
-// All clusters are co-resident (grid = 2 x 74 <= SM count, checked at start-up with the occupancy API) and walk
-// their tiles in increasing global index, and a tile only ever waits for tiles of LOWER index: no deadlock.
+// All CTAs are co-resident (grid <= SM count, checked at start-up with the occupancy API), walk their tiles in increasing
+// global index and publish every tile before they start the MMAs of the next one, and a tile only ever waits for tiles of
+// LOWER index: no deadlock.  The producer (thread 0, also an MMA thread) therefore only ever blocks on a counter at the
+// start of a tile; while the MMAs of a tile run it prefetches the next tile's operands only if their counter is ready.
 //
-//   epilogue warp:     TMA stores -> cp.async.bulk.wait_group 0 -> mbarrier.arrive(publish[tile & 3])     (release.cta;
-//                      the other lanes' plain stores are ordered before lane 0's arrive by __syncwarp)
-//   publisher warp:    mbarrier wait(publish[..]) (acquire.cta) -> fence.proxy.async -> __threadfence -> atomicAdd(counter)
-//   consumer TMA lane: ld.acquire.gpu(counter) >= target -> fence.proxy.async -> cp.async.bulk.tensor loads
-//   consumer epilogue: ordered after the TMA lane's acquire through full[] -> MMA -> tmem_full[]; its reads of
-//                      activations written in this launch use ld.global.cg
+//   all warps:      TMA stores -> cp.async.bulk.wait_group 0 (lane 0) -> CTA barrier
+//   thread 0:       fence.proxy.async -> __threadfence -> atomicAdd(counter)
+//   consumer TMA:   ld.acquire.gpu(counter) >= target -> fence.proxy.async -> cp.async.bulk.tensor loads
+//   epilogue reads of activations written in this launch use ld.global.cg
 //
-// Epilogue (see also the measurements at kNumEpiWarps).  Eight warps, two per TMEM lane group.  A tile of a phase with
-// a residual (out-proj, FFN2) is cut into eight 32-column slices, four per warp: bias, the residual LayerNorm(v)
-// re-derived from v's bf16 planes (coalesced loads transposed through the warp's 4 KB staging tile, the next slice's block
-// prefetched into registers), partial row statistics, one store of both bf16 planes through 64-byte-swizzled boxes.  A
-// tile of a planes-only phase (FFN1, QKV) is cut into four 64-column pairs, two per warp: folded-LayerNorm scale / shift,
-// bias, GELU (branch-free rational erf), hi plane then lo plane through 128-byte-swizzled boxes.  Per-column constants
-// are loaded once per tile into registers and handed out by shuffle; the release fence / counter bump lives in a warp of
-// its own.  Shared memory: A ring 2 x 32 KB, W ring 3 x 32 KB (separate barriers), 8 x 4 KB staging tiles = 192 KB.
+// Epilogue.  Two warpgroups; warpgroup j holds the accumulator of the tile's columns [128 j, 128 j + 128) (two m64 halves,
+// interleaved so that warp w owns rows 32 w .. 32 w + 31; k-block sums of the tensor cores added up in fp32 registers,
+// see mma_kblock_promoted).  A tile of a phase with a residual (out-proj, FFN2)
+// is cut into 32-column slices, four per warp: bias, the residual LayerNorm(v) re-derived from v's bf16 planes (coalesced
+// loads transposed through the warp's 4 KB staging tile, the next slice's block prefetched into registers), partial row
+// statistics, one store of both bf16 planes through 64-byte-swizzled boxes.  A tile of a planes-only phase (FFN1, QKV) is
+// cut into 64-column pairs, two per warp: folded-LayerNorm scale / shift, bias, GELU (branch-free rational erf), hi plane
+// then lo plane through 128-byte-swizzled boxes.  Per-column constants are loaded once per tile into registers and
+// handed out by shuffle.  Shared memory: 2 operand stages x 96 KB (A and W, hi + lo), 8 x 4 KB staging tiles.
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include "kernels.h"
@@ -40,47 +39,21 @@ namespace {
 constexpr int kBlockM = 128;  // per CTA; 256 per pair
 constexpr int kBlockN = 256;
 constexpr int kBlockK = 64;
-constexpr int kUmmaK = 16;
-// Epilogue warps, ring depths and the L1 left beside the shared memory, measured at B = 64 (same box, A/B/A/B):
-//   12 epilogue warps (128 registers), A 3 + W 2 stages        482 steps/s
-//   12 warps with 2 KB staging tiles,  A 3 + W 3               504
-//    8 warps (168 registers),          A 3 + W 3  (224 KB)     520   <- round-2 mid-point
-//    8 warps, 64-column pairs in the planes-only phases, A 3 + W 3 (224 KB)   514-523 (another box)
-//    same, A 2 + W 3 (192 KB) or A 2 + W 2 (160 KB)            528-535
-//    same, A 2 + W 3 + a second staging tile per warp (224 KB) 514
-// The epilogue is issue- and latency-bound, not occupancy-bound (fewer warps with more registers win), and what the
-// third A stage buys the producer is less than what its 32 KB cost the epilogue as L1: the per-tile constants, the row
-// statistics and the few spilled registers around the barrier waits live there, and at 224 KB of shared memory only
-// ~25 KB of L1 remain.  A second staging tile per warp (stores never waiting for the previous store's read) bought
-// nothing at equal shared memory.
-#ifndef CMDI_CHAIN_STAGES_W
-#define CMDI_CHAIN_STAGES_W 3
-#endif
-constexpr int kNumEpiWarps = 8;  // the slice / pair assignment below is written for two warps per lane group
+constexpr int kNumEpiWarps = 8;  // two warpgroups; the slice / pair assignment below is written for two warps per row group
 constexpr int kWarpsPerLaneGroup = kNumEpiWarps / 4;
-constexpr int kFirstEpiWarp = 3;
-constexpr int kNumThreads = (kFirstEpiWarp + kNumEpiWarps) * 32;
-#ifndef CMDI_CHAIN_STAGES_A
-#define CMDI_CHAIN_STAGES_A 2
-#endif
-constexpr int kStagesA = CMDI_CHAIN_STAGES_A, kStagesW = CMDI_CHAIN_STAGES_W;
+constexpr int kNumThreads = kNumEpiWarps * 32;
+constexpr int kStages = 2;
 constexpr int kPlaneBytes = kBlockM * kBlockK * 2;   // one bf16 plane of a 128-row x 64-column operand block = 16 KB
-constexpr int kOperandBytes = 2 * kPlaneBytes;       // hi + lo
+constexpr int kWPlaneBytes = kBlockN * kBlockK * 2;  // one bf16 plane of the 256-row W block = 32 KB
+constexpr int kStageBytes = 2 * (kPlaneBytes + kWPlaneBytes);
 constexpr int kSlices = kBlockN / 32;                // 32-column slices per tile
-constexpr int kAccStride = 256;                      // TMEM columns per accumulator buffer
-constexpr uint32_t kTmemCols = 512;
-constexpr int kPublishBars = 4;
+constexpr int kPartN = kBlockN / 2;                  // columns per warpgroup
 
 struct __align__(8) ChainBarriers {
-  uint64_t full_a[kStagesA], empty_a[kStagesA];
-  uint64_t full_w[kStagesW], empty_w[kStagesW];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint64_t publish[kPublishBars];
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t full[kStages], empty[kStages];
 };
 
-constexpr int kSmemBytes = 1024 + (kStagesA + kStagesW) * kOperandBytes + kNumEpiWarps * kEpiStageBytes + (int)sizeof(ChainBarriers) +
+constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kNumEpiWarps * kEpiStageBytes + (int)sizeof(ChainBarriers) +
                            kMaxChainPhases * (int)sizeof(ChainPhaseInfo);
 static_assert(kSmemBytes <= 232448, "shared memory budget");
 
@@ -198,12 +171,9 @@ __device__ __forceinline__ float pick(const float (&a)[kSlicesPerWarp], int k) {
   return v;
 }
 
-// Start of a tile for one epilogue warp: per-column constants of its (up to) four 32-column slices and the statistics of
-// its row.  `wide`: the warp owns two 64-column pairs (slices 2q, 2q+1 for q = warp_in_group, warp_in_group + 2) instead
-// of the alternating slices warp_in_group + 2k.
-__device__ __forceinline__ int warp_slice(int k, int warp_in_group, bool wide) {
-  return wide ? 2 * (warp_in_group + kWarpsPerLaneGroup * (k >> 1)) + (k & 1) : warp_in_group + k * kWarpsPerLaneGroup;
-}
+// Start of a tile for one epilogue warp: per-column constants of its four 32-column slices and the statistics of its row.
+// Warp group j (= warp_in_group) owns the slices 4 j .. 4 j + 3 (in the `wide` phases: the 64-column pairs 2 j, 2 j + 1).
+__device__ __forceinline__ int warp_slice(int k, int warp_in_group, bool /*wide*/) { return warp_in_group * kSlicesPerWarp + k; }
 // The constants do not depend on anything computed in this launch: they are requested BEFORE the warp waits for the tile's
 // accumulator, all loads of a vector in flight together (indices clamped instead of predicated; measured before: one
 // predicated load at a time, each followed by the spill of its result, was 11 % of this kernel's stall samples).
@@ -242,17 +212,18 @@ __device__ __forceinline__ void load_row_statistics(const LinearParams& p, RowSt
 }
 
 // A 64-column pair of slices of a phase that writes planes only (FFN1, QKV): one accumulator read, one pass of math over
-// 64 values and two {128 B x 32 rows} plane stores -- half the per-slice synchronisation (TMEM load wait, staging-tile
+// 64 values and two {128 B x 32 rows} plane stores -- half the per-slice synchronisation (accumulator transpose, staging-tile
 // turn-around, proxy fence) per column of the 32-column path, which needs its registers for the residual instead.
-__device__ __forceinline__ void epilogue_pair(const LinearParams& p, const ChainPhaseDesc& pd, uint32_t tmem_acc, int m_blk, int n_blk,
-                                              int pair, int k2, int lane_group, int lane, uint32_t stage, const RowStats& rs) {
+__device__ __forceinline__ void epilogue_pair(const LinearParams& p, const ChainPhaseDesc& pd, const float (&acc0)[kPartN / 2],
+                                              const float (&acc1)[kPartN / 2], int m_blk, int n_blk, int pair, int k2, int lane_group,
+                                              int lane, uint32_t stage, const RowStats& rs) {
   const int n0 = n_blk * kBlockN + pair * 64;
   if (n0 >= p.N) return;  // warp-uniform
   const int warp_row0 = m_blk * kBlockM + lane_group * 32;
+  if (lane == 0) tma_store_wait_read();  // the staging tile is about to be rewritten
   uint32_t v[64];
-  tmem_ld32(tmem_acc + pair * 64, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-  tmem_ld32(tmem_acc + pair * 64 + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-  tmem_ld_wait();
+  acc_rows_to_lanes(acc0, acc1, k2 * 8, stage, lane, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
+  acc_rows_to_lanes(acc0, acc1, k2 * 8 + 4, stage, lane, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
   float f[64];
 #pragma unroll
   for (int j = 0; j < 64; ++j) f[j] = __uint_as_float(v[j]);
@@ -296,10 +267,10 @@ __device__ __forceinline__ void epilogue_pair(const LinearParams& p, const Chain
   }
 }
 
-// One 32-column slice of a 128-row accumulator: TMEM -> registers -> [folded LayerNorm] -> bias -> [residual] ->
+// One 32-column slice of a 128-row accumulator: fragments -> row-per-thread registers -> [folded LayerNorm] -> bias -> [residual] ->
 // [partial statistics] -> [GELU] -> fp32 rows and/or bf16 hi/lo planes.
-__device__ __forceinline__ void epilogue_slice(const LinearParams& p, const ChainPhaseDesc& pd, uint32_t tmem_acc, int m_blk, int n_blk,
-                                               int slice, int k_in_tile, int lane_group, int lane, uint32_t stage, RowStats& rs, uint4 (&rv)[8],
+__device__ __forceinline__ void epilogue_slice(const LinearParams& p, const ChainPhaseDesc& pd, const float (&acc0)[kPartN / 2],
+                                               const float (&acc1)[kPartN / 2], int m_blk, int n_blk, int slice, int k_in_tile, int lane_group, int lane, uint32_t stage, RowStats& rs, uint4 (&rv)[8],
                                                bool& rv_ready, int next_slice, int warp_in_group, long long* dbg) {
   long long t0 = clock64(), t1;
 #define CMDI_T(i) do { if (dbg) { t1 = clock64(); dbg[i] += t1 - t0; t0 = t1; } } while (0)
@@ -337,8 +308,7 @@ __device__ __forceinline__ void epilogue_slice(const LinearParams& p, const Chai
   if (has_res && !rv_ready) fetch_residual(n0);
   rv_ready = false;
   uint32_t v[32];
-  tmem_ld32(tmem_acc + slice * 32, v);
-  tmem_ld_wait();
+  acc_rows_to_lanes(acc0, acc1, k_in_tile * 4, stage, lane, v);
   CMDI_T(10);  // residual loads issued + accumulator read
   float f[32];
 #pragma unroll
@@ -472,276 +442,169 @@ __device__ __forceinline__ void epilogue_slice(const LinearParams& p, const Chai
 #undef CMDI_T
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kNumThreads, 1)
+// The operand stream of one CTA (thread 0): k-block after k-block of its tiles, one ring stage each.
+struct ChainProducer {
+  const ChainPhaseDesc* phases;
+  const ChainPhaseInfo* info;
+  uint8_t* ring;
+  ChainBarriers* bars;
+  int cluster_id, num_clusters, rank, my_tiles;
+  int seq, kb, ph, stage;
+  uint32_t phase;
+  int issued;  // k-blocks issued so far
+
+  // Issues the next k-block.  A tile's first k-block waits for its dependency counter: blocking, or (blocking = false)
+  // only if it is already satisfied -- returns false then without issuing.
+  __device__ bool issue_next(bool blocking) {
+    if (seq >= my_tiles) return false;
+    const int tile = cluster_id + seq * num_clusters;
+    while (tile >= info[ph].tile_end) ++ph;
+    const ChainPhaseInfo& pi = info[ph];
+    const ChainPhaseDesc& pd = phases[ph];
+    const int local = tile - pi.tile_begin;
+    const int m_pair = local / pi.num_n_blocks;
+    const int m_blk = 2 * m_pair + rank;
+    const int n_blk = local % pi.num_n_blocks;
+    if (kb == 0 && pi.wait_ctr) {
+      // the A rows of this row pair are written by an earlier phase of this launch
+      if (!blocking && ld_acquire_gpu(pi.wait_ctr + m_pair) < pi.wait_target) return false;
+      wait_counter(pi.wait_ctr + m_pair, pi.wait_target);
+      fence_proxy_async_all();
+    }
+    const int nplanes = (pi.p.nsplit == 3) ? 2 : 1;
+    mbar_wait(&bars->empty[stage], phase ^ 1);
+    uint8_t* da = ring + (size_t)stage * kStageBytes;
+    uint8_t* dw = da + 2 * kPlaneBytes;
+    if (pi.p.debug & 4) {
+      // bring-up decomposition (CMDI_DEBUG=4): no operand loads, only the pipeline bookkeeping
+      mbar_arrive(&bars->full[stage]);
+    } else {
+      mbar_arrive_expect_tx(&bars->full[stage], nplanes * (kPlaneBytes + kWPlaneBytes));
+      const int kc = kb * kBlockK;
+      tma_load_2d(da, &pd.a_hi, &bars->full[stage], kc, m_blk * kBlockM);
+      tma_load_2d(dw, &pd.w_hi, &bars->full[stage], kc, n_blk * kBlockN);
+      tma_load_2d(dw + kWPlaneBytes / 2, &pd.w_hi, &bars->full[stage], kc, n_blk * kBlockN + kBlockN / 2);
+      if (nplanes == 2) {
+        tma_load_2d(da + kPlaneBytes, &pd.a_lo, &bars->full[stage], kc, m_blk * kBlockM);
+        tma_load_2d(dw + kWPlaneBytes, &pd.w_lo, &bars->full[stage], kc, n_blk * kBlockN);
+        tma_load_2d(dw + kWPlaneBytes + kWPlaneBytes / 2, &pd.w_lo, &bars->full[stage], kc, n_blk * kBlockN + kBlockN / 2);
+      }
+    }
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
+    if (++kb == pi.num_k_blocks) { kb = 0; ++seq; }
+    ++issued;
+    return true;
+  }
+};
+
+__global__ void __launch_bounds__(kNumThreads, 1)
 linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_phases, const int total_tiles, long long* dbg) {
-  // dbg (bring-up, CMDI_CHAIN_DBG=1): [gridDim.x][kMaxChainPhases][8] cycle counters per CTA and phase:
-  //   0 tiles  1 tma: dependency wait  2 tma: slot wait  3 mma: operand wait  4 mma: accumulator wait
-  //   5 epilogue warp 0: accumulator wait  6 its slice work  7 its publish wait
+  // dbg (bring-up, CMDI_CHAIN_DBG=1): [gridDim.x][kMaxChainPhases][16] cycle counters per CTA and phase:
+  //   0 tiles  1 dependency wait at the tile start  5 warp 0: operand wait  6 its epilogue work  7 its publish wait
   long long* dbg_me = dbg ? dbg + (size_t)blockIdx.x * kMaxChainPhases * 16 : nullptr;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ring_a = smem;
-  uint8_t* ring_w = ring_a + kStagesA * kOperandBytes;
-  uint8_t* epi_stage = ring_w + kStagesW * kOperandBytes;  // kNumEpiWarps x 4 KB store-staging tiles
+  uint8_t* ring = smem;
+  uint8_t* epi_stage = ring + kStages * kStageBytes;  // kNumEpiWarps x 4 KB store-staging tiles
   ChainBarriers* bars = reinterpret_cast<ChainBarriers*>(epi_stage + kNumEpiWarps * kEpiStageBytes);
   ChainPhaseInfo* info = reinterpret_cast<ChainPhaseInfo*>(bars + 1);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
+  const int rank = (int)(blockIdx.x & 1);
   const int cluster_id = blockIdx.x >> 1;
   const int num_clusters = gridDim.x >> 1;
   const int my_tiles = (total_tiles - cluster_id + num_clusters - 1) / num_clusters;
+  const bool is_producer = threadIdx.x == 0;
 
   // phase descriptors (all but the tensor maps) into shared memory: every role reads them per tile
   for (int i = threadIdx.x; i < num_phases * (int)(sizeof(ChainPhaseInfo) / 4); i += kNumThreads) {
     const int ph = i / (int)(sizeof(ChainPhaseInfo) / 4), w = i % (int)(sizeof(ChainPhaseInfo) / 4);
     reinterpret_cast<uint32_t*>(info + ph)[w] = reinterpret_cast<const uint32_t*>(&phases[ph].info)[w];
   }
-  if (warp_idx == 0 && lane == 0) {
+  if (is_producer) {
     for (int ph = 0; ph < num_phases; ++ph) {
       tma_prefetch_desc(&phases[ph].a_hi);
       tma_prefetch_desc(&phases[ph].w_hi);
     }
-    for (int s = 0; s < kStagesA; ++s) {
-      mbar_init(&bars->full_a[s], 1);
-      mbar_init(&bars->empty_a[s], 1);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&bars->full[s], 1);
+      mbar_init(&bars->empty[s], kNumEpiWarps);
     }
-    for (int s = 0; s < kStagesW; ++s) {
-      mbar_init(&bars->full_w[s], 1);
-      mbar_init(&bars->empty_w[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], 2 * 4 * kSlices);  // every (CTA, lane group, slice) arrives once per tile
-    }
-    for (int s = 0; s < kPublishBars; ++s) mbar_init(&bars->publish[s], kNumEpiWarps);
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc_2sm(&bars->tmem_base, kTmemCols);
-    tmem_relinquish_2sm();
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();  // barrier inits + TMEM allocation visible to both CTAs
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
+  ChainProducer prod{phases, info, ring, bars, cluster_id, num_clusters, rank, my_tiles, 0, 0, 0, 0, 0u, 0};
 
-  if (warp_idx == 0) {
-    // ===================================== TMA producer (both CTAs) =====================================
-    if (lane == 0) {
-      int sa = 0, sw = 0, ph = 0;
-      uint32_t pa = 0, pw = 0;
-      for (int seq = 0; seq < my_tiles; ++seq) {
-        const int tile = cluster_id + seq * num_clusters;
-        while (tile >= info[ph].tile_end) ++ph;
-        const ChainPhaseInfo& pi = info[ph];
-        const ChainPhaseDesc& pd = phases[ph];
-        const int local = tile - pi.tile_begin;
-        const int m_pair = local / pi.num_n_blocks;
-        const int m_blk = 2 * m_pair + (int)cta_rank;
-        const int n_blk = local % pi.num_n_blocks;
-        const int nplanes = (pi.p.nsplit == 3) ? 2 : 1;
-        const uint32_t tx_bytes = 2u * nplanes * kPlaneBytes;  // both CTAs' loads complete on the leader's barrier
-        long long c0 = clock64();
-        if (pi.wait_ctr) {
-          // the A rows of this row pair are written by an earlier phase of this launch
-          wait_counter(pi.wait_ctr + m_pair, pi.wait_target);
-          fence_proxy_async_all();
-        }
-        if (dbg_me) { dbg_me[ph * 16 + 0] += 1; dbg_me[ph * 16 + 1] += clock64() - c0; }
-        for (int kb = 0; kb < pi.num_k_blocks; ++kb) {
-          c0 = clock64();
-          mbar_wait(&bars->empty_w[sw], pw ^ 1);
-          if (pi.p.debug & 4) {
-            // bring-up decomposition (CMDI_DEBUG=4): no operand loads, only the pipeline bookkeeping
-            mbar_wait(&bars->empty_a[sa], pa ^ 1);
-            if (leader) { mbar_arrive(&bars->full_w[sw]); mbar_arrive(&bars->full_a[sa]); }
-            if (++sa == kStagesA) { sa = 0; pa ^= 1; }
-            if (++sw == kStagesW) { sw = 0; pw ^= 1; }
-            continue;
-          }
-          uint8_t* dw = ring_w + (size_t)sw * kOperandBytes;
-          if (leader) mbar_arrive_expect_tx(&bars->full_w[sw], tx_bytes);
-          tma_load_2d_2sm(dw, &pd.w_hi, &bars->full_w[sw], kb * kBlockK, n_blk * kBlockN + (int)cta_rank * (kBlockN / 2));
-          if (nplanes == 2)
-            tma_load_2d_2sm(dw + kPlaneBytes, &pd.w_lo, &bars->full_w[sw], kb * kBlockK, n_blk * kBlockN + (int)cta_rank * (kBlockN / 2));
-          mbar_wait(&bars->empty_a[sa], pa ^ 1);
-          if (dbg_me) dbg_me[ph * 16 + 2] += clock64() - c0;
-          uint8_t* da = ring_a + (size_t)sa * kOperandBytes;
-          if (leader) mbar_arrive_expect_tx(&bars->full_a[sa], tx_bytes);
-          tma_load_2d_2sm(da, &pd.a_hi, &bars->full_a[sa], kb * kBlockK, m_blk * kBlockM);
-          if (nplanes == 2) tma_load_2d_2sm(da + kPlaneBytes, &pd.a_lo, &bars->full_a[sa], kb * kBlockK, m_blk * kBlockM);
-          if (++sa == kStagesA) { sa = 0; pa ^= 1; }
-          if (++sw == kStagesW) { sw = 0; pw ^= 1; }
-        }
+  const int j3 = warp_idx >> 2;          // warpgroup = column half of the tile
+  const int lane_group = warp_idx & 3;   // rows 32 * lane_group .. + 31 of the CTA's 128
+  const uint32_t epi_stage_addr = smem_u32(epi_stage + warp_idx * kEpiStageBytes);
+  const uint32_t w_off = 2 * kPlaneBytes + j3 * kPartN * 128;  // this warpgroup's W rows in a stage
+  float acc0[kPartN / 2], acc1[kPartN / 2];
+  RowStats rs{};
+  int ph = 0, stage = 0, consumed = 0;
+  uint32_t phase = 0;
+  for (int seq = 0; seq < my_tiles; ++seq) {
+    long long c0 = clock64();
+    const int tile = cluster_id + seq * num_clusters;
+    while (tile >= info[ph].tile_end) ++ph;
+    const ChainPhaseInfo& pi = info[ph];
+    const int local = tile - pi.tile_begin;
+    const int m_blk = 2 * (local / pi.num_n_blocks) + rank;
+    const int n_blk = local % pi.num_n_blocks;
+    const bool wide = pi.wide != 0;
+    const bool split = pi.p.nsplit == 3;
+    load_tile_constants(pi.p, rs, n_blk, j3, wide, lane);
+    // ---- mainloop ----
+#pragma unroll
+    for (int i = 0; i < kPartN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    for (int kb = 0; kb < pi.num_k_blocks; ++kb) {
+      if (is_producer) {
+        // every earlier tile of this CTA is published: blocking on a dependency counter is safe here
+        long long d0 = clock64();
+        while (prod.issued <= consumed) prod.issue_next(true);
+        if (dbg_me && kb == 0) { dbg_me[ph * 16 + 0] += 1; dbg_me[ph * 16 + 1] += clock64() - d0; }
+      }
+      mbar_wait(&bars->full[stage], phase);
+      const uint32_t sa = smem_u32(ring + (size_t)stage * kStageBytes);
+      if (!(pi.p.debug & 2)) mma_kblock_promoted<kPartN>(acc0, acc1, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, split);
+      // the tensor cores have read this stage: it may be refilled
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->empty[stage]);
+      ++consumed;
+      if (is_producer && prod.issued < consumed + kStages) prod.issue_next(false);
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    long long c1 = clock64();
+    // ---- epilogue ----
+    load_row_statistics(pi.p, rs, m_blk * kBlockM + lane_group * 32 + lane);
+    long long* dbg_w = (dbg_me && warp_idx == 0 && lane == 0) ? dbg_me + ph * 16 : nullptr;
+    if (wide) {
+#pragma unroll
+      for (int k2 = 0; k2 < kSlicesPerWarp / 2; ++k2)
+        epilogue_pair(pi.p, phases[ph], acc0, acc1, m_blk, n_blk, 2 * j3 + k2, k2, lane_group, lane, epi_stage_addr, rs);
+    } else {
+      uint4 rv[8];  // residual block in flight for this warp's next slice (see epilogue_slice)
+      bool rv_ready = false;
+#pragma unroll
+      for (int k = 0; k < kSlicesPerWarp; ++k) {
+        const int slice = warp_slice(k, j3, false);
+        const int next_slice = k + 1 < kSlicesPerWarp ? slice + 1 : -1;
+        epilogue_slice(pi.p, phases[ph], acc0, acc1, m_blk, n_blk, slice, k, lane_group, lane, epi_stage_addr, rs, rv, rv_ready,
+                       next_slice, j3, nullptr);
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ====================================== MMA issuer (leader CTA only) ======================================
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * kBlockM, kBlockN, 0);
-      int sa = 0, sw = 0, ph = 0;
-      uint32_t pa = 0, pw = 0;
-      for (int seq = 0; seq < my_tiles; ++seq) {
-        const int tile = cluster_id + seq * num_clusters;
-        while (tile >= info[ph].tile_end) ++ph;
-        const ChainPhaseInfo& pi = info[ph];
-        const bool split = pi.p.nsplit == 3;
-        const int acc = seq & 1;
-        long long c0 = clock64();
-        mbar_wait(&bars->tmem_empty[acc], ((seq >> 1) & 1) ^ 1);
-        if (dbg_me) dbg_me[ph * 16 + 4] += clock64() - c0;
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccStride;
-        for (int kb = 0; kb < pi.num_k_blocks; ++kb) {
-          c0 = clock64();
-          mbar_wait(&bars->full_w[sw], pw);
-          mbar_wait(&bars->full_a[sa], pa);
-          if (dbg_me) dbg_me[ph * 16 + 3] += clock64() - c0;
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(ring_a + (size_t)sa * kOperandBytes);
-          const uint32_t w_addr = smem_u32(ring_w + (size_t)sw * kOperandBytes);
-          const uint64_t da_hi = make_desc_kmajor_sw128(a_addr);
-          const uint64_t db_hi = make_desc_kmajor_sw128(w_addr);
-          if (pi.p.debug & 2) {
-            // bring-up decomposition (CMDI_DEBUG=2): no MMAs, only the pipeline bookkeeping
-          } else if (split) {
-            const uint64_t da_lo = make_desc_kmajor_sw128(a_addr + kPlaneBytes);
-            const uint64_t db_lo = make_desc_kmajor_sw128(w_addr + kPlaneBytes);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_ss_2sm(d_tmem, desc_advance(da_lo, k * kUmmaK * 2), desc_advance(db_hi, k * kUmmaK * 2), idesc,
-                          (kb > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_ss_2sm(d_tmem, desc_advance(da_hi, k * kUmmaK * 2), desc_advance(db_lo, k * kUmmaK * 2), idesc, 1u);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_ss_2sm(d_tmem, desc_advance(da_hi, k * kUmmaK * 2), desc_advance(db_hi, k * kUmmaK * 2), idesc, 1u);
-          } else {
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_ss_2sm(d_tmem, desc_advance(da_hi, k * kUmmaK * 2), desc_advance(db_hi, k * kUmmaK * 2), idesc,
-                          (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit_2sm(&bars->empty_a[sa], 0x3);  // frees the slots in BOTH CTAs
-          umma_commit_2sm(&bars->empty_w[sw], 0x3);
-          if (++sa == kStagesA) { sa = 0; pa ^= 1; }
-          if (++sw == kStagesW) { sw = 0; pw ^= 1; }
-        }
-        umma_commit_2sm(&bars->tmem_full[acc], 0x3);  // both CTAs' epilogues may read their half of the tile
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx == 2) {
-    // ============ publisher: one release fence + counter bump per tile, off the epilogue warps' critical path ============
-    if (lane == 0) {
-      int ph = 0;
-      for (int seq = 0; seq < my_tiles; ++seq) {
-        const int tile = cluster_id + seq * num_clusters;
-        while (tile >= info[ph].tile_end) ++ph;
-        const ChainPhaseInfo& pi = info[ph];
-        mbar_wait(&bars->publish[seq & (kPublishBars - 1)], (seq / kPublishBars) & 1);
-        if (pi.done_ctr) {
-          fence_proxy_async_all();
-          __threadfence();
-          atomicAdd(pi.done_ctr + (tile - pi.tile_begin) / pi.num_n_blocks, 1);
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============ epilogue warps: two per TMEM lane group; four 32-column slices or two 64-column pairs per warp and tile ============
-    const int ew = warp_idx - kFirstEpiWarp;
-    const int lane_group = warp_idx & 3;  // the TMEM lanes a warp may touch: 32 * (warp index % 4)
-    const int j3 = ew >> 2;               // index within the lane group
-    const uint32_t epi_stage_addr = smem_u32(epi_stage + ew * kEpiStageBytes);
-    const uint32_t tmem_lane = tmem_base + ((uint32_t)(lane_group * 32) << 16);
-    int ph = 0, stored_seq = -1;
-    RowStats rs{};
-    // everything this warp stored for tile `seq` is in memory: tell the publisher
-    auto publish = [&](int seq) {
-      __syncwarp();  // the other lanes' plain stores (row-mapped outputs, partial statistics) before lane 0's release
-      if (lane == 0) {
-        tma_store_wait_all();
-        mbar_arrive(&bars->publish[seq & (kPublishBars - 1)]);
-      }
-    };
-    for (int seq = 0; seq < my_tiles; ++seq) {
-      long long c0 = clock64();
-      const int tile = cluster_id + seq * num_clusters;
-      while (tile >= info[ph].tile_end) ++ph;
-      const ChainPhaseInfo& pi = info[ph];
-      const int local = tile - pi.tile_begin;
-      const int m_blk = 2 * (local / pi.num_n_blocks) + (int)cta_rank;
-      const int n_blk = local % pi.num_n_blocks;
-      const int acc = seq & 1;
-      const bool wide = pi.wide != 0;
-      load_tile_constants(pi.p, rs, n_blk, j3, wide, lane);
-      mbar_wait(&bars->tmem_full[acc], (seq >> 1) & 1);
-      long long c1 = clock64();
-      tc_fence_after();
-      if (stored_seq >= 0) {
-        publish(stored_seq);  // deferred from the previous tile: its stores have landed while the mainloop ran
-        stored_seq = -1;
-      }
-      long long c2 = clock64();
-      load_row_statistics(pi.p, rs, m_blk * kBlockM + lane_group * 32 + lane);
-      const uint32_t tmem_acc = tmem_lane + acc * kAccStride;
-      long long* dbg_w = (dbg_me && ew == 0 && lane == 0) ? dbg_me + ph * 16 : nullptr;
-      if (wide) {
-#pragma unroll 1
-        for (int k2 = 0; k2 < kSlicesPerWarp / 2; ++k2) {
-          epilogue_pair(pi.p, phases[ph], tmem_acc, m_blk, n_blk, j3 + kWarpsPerLaneGroup * k2, k2, lane_group, lane, epi_stage_addr, rs);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {  // one arrival per 32-column slice keeps the barrier's count independent of the phase
-            mbar_arrive_on_leader(&bars->tmem_empty[acc]);
-            mbar_arrive_on_leader(&bars->tmem_empty[acc]);
-          }
-        }
-      } else {
-        uint4 rv[8];  // residual block in flight for this warp's next slice (see epilogue_slice)
-        bool rv_ready = false;
-#pragma unroll 1
-        for (int k = 0; k < kSlicesPerWarp; ++k) {
-          const int slice = j3 + k * kWarpsPerLaneGroup;
-          const int next_slice = k + 1 < kSlicesPerWarp ? slice + kWarpsPerLaneGroup : -1;
-          epilogue_slice(pi.p, phases[ph], tmem_acc, m_blk, n_blk, slice, k, lane_group, lane, epi_stage_addr, rs, rv, rv_ready,
-                         next_slice, j3, dbg_w);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_on_leader(&bars->tmem_empty[acc]);
-        }
-      }
-      stored_seq = seq;
-      long long c3 = clock64();
-      {
-        // If this cluster's next tile belongs to a later phase (or does not exist) it may depend on this one: publish
-        // now; otherwise at the start of the next tile.
-        const int next_tile = cluster_id + (seq + 1) * num_clusters;
-        if (next_tile >= pi.tile_end || pi.publish_now) {
-          publish(seq);
-          stored_seq = -1;
-        }
-      }
-      if (dbg_me && ew == 0 && lane == 0) {
-        dbg_me[ph * 16 + 5] += c1 - c0; dbg_me[ph * 16 + 6] += c3 - c2; dbg_me[ph * 16 + 7] += (c2 - c1) + (clock64() - c3);
-      }
-    }
-    if (stored_seq >= 0) publish(stored_seq);
+    long long c2 = clock64();
+    // ---- publish: everything this CTA stored for the tile is in memory, then one counter bump ----
+    __syncwarp();  // the other lanes' plain stores (row-mapped outputs, partial statistics) before lane 0's wait
     if (lane == 0) tma_store_wait_all();
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // nobody touches the pair's TMEM / barriers after this point
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, kTmemCols);
+    __syncthreads();
+    if (is_producer && pi.done_ctr) {
+      fence_proxy_async_all();
+      __threadfence();
+      atomicAdd(pi.done_ctr + (tile - pi.tile_begin) / pi.num_n_blocks, 1);
+    }
+    if (dbg_w) { dbg_w[5] += c1 - c0; dbg_w[6] += c2 - c1; dbg_w[7] += clock64() - c2; }
   }
 }
 
@@ -754,16 +617,12 @@ cudaError_t configure_linear_chain_kernel() {
 // how many CTA pairs of this kernel can be resident at once on the current device (they spin on each other's counters:
 // the launch must never exceed this)
 int linear_chain_max_clusters(int num_sms) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * (num_sms / 2));
-  cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, linear_chain_kernel, &cfg) != cudaSuccess) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_chain_kernel, kNumThreads, kSmemBytes) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
-  return n;
+  return per_sm * num_sms / 2;
 }
 
 cudaError_t launch_linear_chain(const ChainPhaseDesc* phases_dev, int num_phases, int total_tiles, int num_sms, cudaStream_t stream,

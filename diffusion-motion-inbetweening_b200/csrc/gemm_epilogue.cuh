@@ -1,18 +1,14 @@
-// Epilogue shared by the 1-CTA and 2-CTA linear kernels: one 128 x BLOCK_N accumulator tile, TMEM -> registers ->
+// Epilogue of the linear kernels: one 128 x BLOCK_N accumulator tile, wgmma fragments -> row-per-thread registers ->
 // bias / positional encoding / residual / GELU -> fp32 and bf16 hi/lo planes in global memory.
 //
-// Thread mapping: epilogue warp w owns TMEM lanes 32*(w%4).. (thread = output row) and half of the tile's columns,
-// processed 64 columns at a time.  A thread therefore holds a ROW fragment, which is the wrong shape for global
+// Thread mapping: epilogue warp w owns rows 32*(w%4).. of the tile (thread = output row, after acc_rows_to_lanes) and
+// one column part of the tile (the columns its warpgroup's MMAs produced), processed 64 columns at a time.  A thread therefore holds a ROW fragment, which is the wrong shape for global
 // memory: every 32-row x 128-byte block is transposed through a per-warp 4 KB shared-memory staging tile (16-byte
 // chunks XOR-swizzled by row & 7: conflict-free both ways) and moved with fully coalesced 16-byte accesses, 4
 // complete 128-byte row segments per instruction.
 //
-// Latency notes from the r01 cycle-counter probe (profiles/r01c_*): the first version spent ~18k cycles per tile
-// here (> the 12k-cycle MMA mainloop it should hide under) because (a) the 16 bias loads of a 64-column chunk sat
-// behind per-group bounds branches and were exposed one after the other, and (b) each staged row was load ->
-// shuffle -> store serially.  Now: the bias of a warp's columns is ONE coalesced load per tile (broadcast by shuffle),
-// the row offsets of the 8 rows a lane stores are precomputed per tile, and staging reads are batched ahead of the
-// global stores.
+// The bias of a warp's columns is ONE coalesced load per tile (broadcast by shuffle), the row offsets of the 8 rows a
+// lane stores are precomputed per tile, and staging reads are batched ahead of the global stores.
 #pragma once
 
 #include "common.cuh"
@@ -160,14 +156,19 @@ struct EpiStoreMaps {
   const CUtensorMap* f32;
 };
 
+// the two column parts of a tile (one per MMA warpgroup): halves, except BLOCK_N = 192 -> 128 + 64 (whole 64-column chunks)
 template <int BLOCK_N>
-__device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiStoreMaps& maps, uint32_t tmem_base, uint32_t acc_col,
-                                              int m_blk, int n_blk, int lane_group, int col_part, int lane, uint32_t stage) {
+__host__ __device__ constexpr int epi_part0_cols() { return (BLOCK_N == 192) ? 128 : BLOCK_N / 2; }
+
+// acc0 / acc1: the warpgroup's two m64 x PART_N accumulator halves of the interleaved 128-row tile
+template <int BLOCK_N, int PART_N>
+__device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiStoreMaps& maps, const float (&acc0)[PART_N / 2],
+                                              const float (&acc1)[PART_N / 2], int m_blk, int n_blk, int lane_group, int col_part,
+                                              int lane, uint32_t stage) {
   constexpr int kBlockM = kEpiBlockM;
-  // the two column parts of a tile: halves, except BLOCK_N = 192 -> 128 + 64 (whole 64-column chunks per warp)
-  constexpr int kPart0Cols = (BLOCK_N == 192) ? 128 : BLOCK_N / 2;
+  constexpr int kPart0Cols = epi_part0_cols<BLOCK_N>();
   const int col_start = col_part == 0 ? 0 : kPart0Cols;
-  const int part_cols = col_part == 0 ? kPart0Cols : BLOCK_N - kPart0Cols;
+  constexpr int part_cols = PART_N;
   const int warp_row0 = m_blk * kBlockM + lane_group * 32;
   RowSlots rows;
   rows.ok = 0;
@@ -206,7 +207,7 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
     if (warp_row0 + lane < p.M) ln_st = p.ln_stats[warp_row0 + lane];
   }
 
-#pragma unroll 1
+#pragma unroll
   for (int c64 = 0; c64 < part_cols / 64; ++c64) {
     const int col_in_tile = col_start + c64 * 64;
     const int n0 = n_blk * BLOCK_N + col_in_tile;
@@ -216,14 +217,10 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
       if (lane == 0) tma_store_wait_read();
       __syncwarp();
     }
+    if (n0 >= p.N) continue;  // warp-uniform: nothing to write for this chunk
     uint32_t v0[32], v1[32];
-    tmem_ld32(tmem_addr(tmem_base, lane_group * 32, acc_col + col_in_tile), v0);
-    tmem_ld32(tmem_addr(tmem_base, lane_group * 32, acc_col + col_in_tile + 32), v1);
-    if (n0 >= p.N) {  // warp-uniform: nothing to write for this chunk
-      tmem_ld_wait();
-      continue;
-    }
-    tmem_ld_wait();
+    acc_rows_to_lanes(acc0, acc1, c64 * 8, stage, lane, v0);
+    acc_rows_to_lanes(acc0, acc1, c64 * 8 + 4, stage, lane, v1);
     float f[64];
 #pragma unroll
     for (int j = 0; j < 32; ++j) {

@@ -1,4 +1,4 @@
-// Host-visible launch interface of the sm_100a kernels (internal to the shared library).
+// Host-visible launch interface of the sm_90a kernels (internal to the shared library).
 #pragma once
 
 #include <cuda.h>
@@ -25,7 +25,7 @@ struct LinearStoreMaps {
   const CUtensorMap* hi = nullptr;
   const CUtensorMap* lo = nullptr;
   const CUtensorMap* f32 = nullptr;
-  // optional A-operand maps with a {64, 136} box: let a k-tap convolution load the A rows of all taps once (gemm2.cu)
+  // A-operand maps with a {64, 136} box (the rows of all taps of a k-tap convolution; not read by the sm_90a GEMM)
   const CUtensorMap* a_tap_hi = nullptr;
   const CUtensorMap* a_tap_lo = nullptr;
 };
@@ -93,14 +93,14 @@ struct LinearParams {
   int tma_store;   // set by the launcher when LinearStoreMaps are given: outputs leave through cp.async.bulk.tensor stores
 };
 
-// CTA-pair (cta_group::2) version: 256-row tiles shared by two SMs of a cluster. W box is {64, block_n / 2}.   (gemm2.cu)
+// One CTA per 128 x block_n tile (wgmma, persistent).  W box is {64, block_n / 2} (two boxes per k-block).   (gemm2.cu)
 cudaError_t configure_linear2_kernels();
 cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                                const CUtensorMap& w_lo, const LinearParams& p, int block_n, int num_sms,
                                cudaStream_t stream, const LinearStoreMaps* st = nullptr);
 
 // A chain of linear layers in ONE persistent launch (gemm_chain.cu): the tiles of all phases form one list walked by
-// the 74 CTA pairs; a tile whose A rows are produced by an earlier phase of the same launch waits on a per-row-pair
+// CTA pairs (one CTA per SM); a tile whose A rows are produced by an earlier phase of the same launch waits on a per-row-pair
 // counter the producing epilogues bump.  Removes the kernel boundaries and the per-kernel tile quantisation.
 constexpr int kMaxChainPhases = 4;
 struct ChainPhaseInfo {
@@ -343,7 +343,7 @@ struct AttnBwdParams {
 cudaError_t configure_attention_bwd_kernel();
 cudaError_t launch_attention_bwd(const AttnBwdParams& p, cudaStream_t stream);  // fp32 CUDA cores: the independent
                                                                                // implementation the unit tests compare against (attention_bwd_simt_test.cu)
-// tcgen05 version (attention_bwd_tc.cu).  Maps over the bf16 planes, box {64, rows}: *_t = 128-row tiles, *_f = 208-row
+// wgmma version (attention_bwd_tc.cu).  Maps over the bf16 planes, box {64, rows}: *_t = 128-row tiles, *_f = 208-row
 // operands; out_* = the dqkv planes as TMA-store targets, box {64, 32}.
 struct AttnBwdTcMaps {
   const CUtensorMap *qkv_t_hi, *qkv_t_lo, *qkv_f_hi, *qkv_f_lo, *do_t_hi, *do_t_lo, *do_f_hi, *do_f_lo, *out_hi, *out_lo;

@@ -80,4 +80,4 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t ro
 #include "../../include/condmdi_b200.h"
 
 extern "C" const char* cmdi_last_error(void) { return cmdi::get_last_error(); }
-extern "C" const char* cmdi_version(void) { return "condmdi_b200 0.1 (sm_100a: tcgen05 + TMA)"; }
+extern "C" const char* cmdi_version(void) { return "condmdi_b200 0.1 (sm_90a: wgmma + TMA)"; }

@@ -192,7 +192,7 @@ __global__ void convt_weight_planes_kernel(const float* __restrict__ w, int Ci, 
 
 inline dim3 grid_1d(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > 132 * 32) g = 132 * 32;
   if (g < 1) g = 1;
   return dim3((unsigned)g);
 }

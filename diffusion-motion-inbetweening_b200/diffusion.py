@@ -1,4 +1,4 @@
-"""Drop-in mirror of the reference's sampler classes, backed by the native B200 engine.
+"""Drop-in mirror of the reference's sampler classes, backed by the native H100 engine.
 
 Mirrors (same names, argument meaning and error behaviour; paths relative to the reference repository):
     get_named_beta_schedule / betas_for_alpha_bar   diffusion/gaussian_diffusion.py:24-71
@@ -140,7 +140,7 @@ class GaussianDiffusion:
         if randomize_class:
             raise NotImplementedError("randomize_class is a class-conditional feature the MDM path does not use")
         if _enum_name(self.model_mean_type) != "START_X" or _enum_name(self.model_var_type) != "FIXED_SMALL":
-            raise NotImplementedError("the B200 engine implements START_X / FIXED_SMALL (utils/model_util.py:142-148)")
+            raise NotImplementedError("the engine implements START_X / FIXED_SMALL (utils/model_util.py:142-148)")
         if self.rescale_timesteps:
             raise NotImplementedError("rescale_timesteps=True is not used by the reference (model_util.py:130)")
         y = model_kwargs["y"]  # the reference indexes it unconditionally (gaussian_diffusion.py:1280)

@@ -1,4 +1,4 @@
-"""Drop-in mirror of the reference's denoiser interface, backed by the native B200 engine.
+"""Drop-in mirror of the reference's denoiser interface, backed by the native H100 engine.
 
     MDM                          model/mdm.py:10-315   (arch='trans_enc', data_rep='hml_vec', cond_mode no_cond|text)
     ClassifierFreeSampleModel    model/cfg_sampler.py:5-35
@@ -59,7 +59,7 @@ def engine_for(self, device: torch.device, max_batch: int = 64, precision: int =
             njoints = sd["unet.final_conv.1.weight"].shape[0]
             in_ch = sd["unet.downs.0.0.blocks.0.block1.0.weight"].shape[1]
             if in_ch not in (njoints, 2 * njoints) or "unet.downs.0.0.blocks.0.block.0.weight" in sd:
-                raise NotImplementedError("the B200 engine implements MDM_UNET with adagn=True and input_feats or 2 * input_feats channels")
+                raise NotImplementedError("the engine implements MDM_UNET with adagn=True and input_feats or 2 * input_feats channels")
             eng = Engine(device, njoints=njoints, nframes=nframes, latent_dim=d, max_batch=max_batch, has_text="embed_text.weight" in sd,
                          precision=precision, arch=capi.ARCH_UNET, unet_dim_mults=mults, keyframe_conditioned=in_ch == 2 * njoints)
         else:
@@ -90,7 +90,7 @@ class MDM(nn.Module):
                  emb_trans_dec=False, clip_version=None, **kargs):
         super().__init__()
         if arch != "trans_enc" or activation != "gelu" or nfeats != 1:
-            raise NotImplementedError("the B200 engine implements arch='trans_enc', activation='gelu', nfeats=1")
+            raise NotImplementedError("the engine implements arch='trans_enc', activation='gelu', nfeats=1")
         self.modeltype, self.njoints, self.nfeats, self.num_actions = modeltype, njoints, nfeats, num_actions
         self.data_rep, self.dataset, self.pose_rep, self.glob, self.glob_rot = data_rep, dataset, pose_rep, glob, glob_rot
         self.translation, self.latent_dim, self.ff_size, self.num_layers = translation, latent_dim, ff_size, num_layers
@@ -180,7 +180,7 @@ class MDM_UNET(nn.Module):
                  keyframe_selection_scheme="in-between", zero_keyframe_loss=False, **kwargs):
         super().__init__()
         if arch != "unet" or attention or not adagn or xz_only or train_keypoint_mask != "none" or nfeats != 1:
-            raise NotImplementedError("the B200 engine implements MDM_UNET arch='unet', adagn=True, attention=False")
+            raise NotImplementedError("the engine implements MDM_UNET arch='unet', adagn=True, attention=False")
         if len(set(dim_mults)) != 1 or not 2 <= len(dim_mults) <= 4:
             raise NotImplementedError("dim_mults must be 2..4 equal multipliers (every published configuration)")
         self.njoints, self.nfeats, self.latent_dim, self.dim_mults = njoints, nfeats, latent_dim, tuple(dim_mults)
@@ -342,7 +342,7 @@ def resolve_model(model) -> Tuple[nn.Module, bool]:
         inner = inner.model
     arch = getattr(inner, "arch", "trans_enc")
     if arch not in ("trans_enc", "unet"):
-        raise NotImplementedError(f"the B200 engine implements MDM arch='trans_enc' and MDM_UNET arch='unet' (got {arch!r})")
+        raise NotImplementedError(f"the engine implements MDM arch='trans_enc' and MDM_UNET arch='unet' (got {arch!r})")
     if not hasattr(inner, "engine_for"):
         keys = inner.state_dict().keys()
         if "seqTransEncoder.layers.0.self_attn.in_proj_weight" not in keys and "unet.time_mlp.0.weight" not in keys:

@@ -20,6 +20,7 @@ sys.path.insert(0, ROOT)
 
 from oracle import condmdi_oracle as O  # noqa: E402
 from oracle import reference_harness as RH  # noqa: E402
+from oracle.golden_io import save_golden  # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 B, D, L = 2, 263, 196
@@ -58,7 +59,7 @@ def golden_schedules():
         r = ref.editing_util.get_gradient_schedule(sched, 1000)
         assert np.array_equal(r, O.get_gradient_schedule(sched, 1000))
         out[f"grad.{sched}"] = r
-    np.savez_compressed(os.path.join(GOLDEN, "schedules.npz"), **out)
+    save_golden(GOLDEN, "schedules", **out)
 
 
 def golden_masks():
@@ -83,7 +84,7 @@ def golden_masks():
                 out[key + ".lengths"] = ls.numpy()
                 out[key + ".bits"] = np.packbits(r.numpy().reshape(-1))
                 out[key + ".sums"] = r.sum(dim=(1, 2, 3)).numpy()
-    np.savez_compressed(os.path.join(GOLDEN, "masks.npz"), **out)
+    save_golden(GOLDEN, "masks", **out)
     print("  sums sparse T=5:", out["benchmark_sparse.5.pos_rot_vel.sums"])
 
 
@@ -188,7 +189,7 @@ def golden_model_and_sampler():
     out["recon.sample"] = r[-1]["sample"].numpy()
     out["recon.pred_xstart"] = r[-1]["pred_xstart"].numpy()
 
-    np.savez_compressed(os.path.join(GOLDEN, "sampler.npz"), **out)
+    save_golden(GOLDEN, "sampler", **out)
 
 
 def golden_postprocess():
@@ -213,7 +214,7 @@ def golden_postprocess():
         rag = ref_ric(inp["ragged"].clone(), 22, abs_3d=abs_3d)
         close(rag, O.recover_from_ric(inp["ragged"], 22, abs_3d), 1e-4, f"recover_from_ric[{tag}] 57 frames")
         out[f"{tag}.ragged"] = rag.numpy()
-    np.savez_compressed(os.path.join(GOLDEN, "postprocess.npz"), **out)
+    save_golden(GOLDEN, "postprocess", **out)
 
 
 def golden_long_loop():
@@ -238,7 +239,7 @@ def golden_long_loop():
         for t in range(4, -1, -1):
             x = O.p_sample(sd, O.make_tables(""), x, torch.full((2,), t), c, tape[1 + 999 - t])["sample"]
     close(sample, x, 2e-5, "last 5 of 1000 steps")
-    np.savez_compressed(os.path.join(GOLDEN, "long_loop.npz"), sample=sample.numpy(), x_at_t4=near_end.numpy(),
+    save_golden(GOLDEN, "long_loop", sample=sample.numpy(), x_at_t4=near_end.numpy(),
                         tape_checksum=np.array([float(tape.double().sum()), float(tape[500].double().abs().sum())]))
 
 
@@ -324,7 +325,7 @@ def golden_chains():
     out["recon50.f64_final"] = o4d[49]["sample"].numpy()
     out["recon50.ref_err_vs_f64"] = np.array([(r4[49].double() - o4d[49]["sample"]).abs().max().item(),
                                               (r4[49].double() - o4d[49]["sample"]).abs().mean().item()])
-    np.savez_compressed(os.path.join(GOLDEN, "chains.npz"), **out)
+    save_golden(GOLDEN, "chains", **out)
 
 
 def golden_unet():
@@ -377,7 +378,7 @@ def golden_unet():
     o_tail = O.sample_loop(sd, tab, (B, D, 1, L), c, tape, "ddpm", skip_timesteps=996, init_image=x_obs)
     close(r_tail, o_tail, 5e-5, "unet ddpm tail")
     out["tail4.sample"] = r_tail.numpy()
-    np.savez_compressed(os.path.join(GOLDEN, "unet.npz"), **out)
+    save_golden(GOLDEN, "unet", **out)
 
 
 def main():

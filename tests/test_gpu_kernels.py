@@ -46,7 +46,7 @@ def run_linear(M, N, K, prec, bn, act=0, bias=True, res=False, seed=0, scale=1.0
 @pytest.mark.parametrize("M,N,K,bn", [
     (128, 128, 64, 128), (128, 256, 64, 256), (1, 8, 8, 128), (130, 264, 512, 128), (1000, 1536, 512, 256),
     (12608, 1536, 512, 256), (12544, 512, 263, 128), (12608, 264, 512, 128), (25216, 512, 1024, 128),
-    # negative block_n: the CTA-pair kernel (cta_group::2), tile 256 x |block_n|
+    # negative block_n: the persistent wgmma kernel, tile 128 x |block_n|
     (256, 256, 64, -256), (1, 8, 8, -128), (130, 264, 512, -128), (1000, 1536, 512, -256), (12608, 1536, 512, -256),
     (12608, 512, 1024, -128), (256, 192, 64, -192), (1000, 1536, 512, -192), (12608, 1536, 512, -192), (300, 1000, 512, -192),
     (25216, 1536, 512, -192),
@@ -174,7 +174,7 @@ def test_attention_backward_matches_autograd(nseq, S, H):
     got = torch.full_like(qkv, float("nan"))
     C.capi.check(_lib().cmdi_test_attention_bwd(_p(qkv), _p(dO), _p(got), nseq, S, H, None))
     torch.cuda.synchronize()
-    # tcgen05 kernel: every product with the bf16 hi/lo split (attention_bwd_tc.cu)
+    # wgmma kernel: every product with the bf16 hi/lo split (attention_bwd_tc.cu)
     assert torch.allclose(got.double(), ref, rtol=1e-3, atol=1e-4)
     assert (got.double() - ref).abs().max() < 1e-4
 

@@ -13,6 +13,7 @@ import torch
 
 import condmdi_b200 as C
 from oracle import condmdi_oracle as O
+from oracle.golden_io import load_golden
 
 pytestmark = pytest.mark.gpu
 GATE = dict(rtol=1e-3, atol=1e-4)
@@ -22,7 +23,7 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return np.load(os.path.join(golden_dir, "sampler.npz"))
+    return load_golden(golden_dir, "sampler")
 
 
 @pytest.fixture(scope="module")
@@ -110,7 +111,7 @@ def test_p_sample_loop_three_steps_vs_reference_golden(plain, gi, gold):
 def test_full_1000_step_ddpm_loop_vs_reference_golden(plain, golden_dir):
     """configs[1] at B=2, the whole chain: 1000 engine steps against the reference's own CPU run of the same loop on the
     same noise (tests/golden/long_loop.npz) -- error growth over the full length, through the public API and the graph."""
-    g = np.load(os.path.join(golden_dir, "long_loop.npz"))
+    g = load_golden(golden_dir, "long_loop")
     m, _ = plain
     diff = C.create_gaussian_diffusion()
     diff.noise_tape = O.long_loop_tape().to(DEV)
@@ -348,7 +349,7 @@ def test_drop_in_under_reference_objects(gi):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("tag,abs_3d", [("rel", False), ("abs", True)])
 def test_sample_to_joints_vs_reference_golden(golden_dir, tag, abs_3d):
-    g = np.load(os.path.join(golden_dir, "postprocess.npz"))
+    g = load_golden(golden_dir, "postprocess")
     inp = O.postprocess_inputs()
     got = C.sample_to_joints(inp["sample"].to(DEV), g[f"{tag}.mean"], g[f"{tag}.std"], 22, abs_3d)
     assert got.is_cuda and got.shape == (3, 22, 3, 196)

@@ -15,6 +15,7 @@ import torch
 
 import condmdi_b200 as C
 from oracle import condmdi_oracle as O
+from oracle.golden_io import load_golden
 
 pytestmark = pytest.mark.gpu
 GATE = dict(rtol=1e-3, atol=1e-4)
@@ -24,7 +25,7 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return np.load(os.path.join(golden_dir, "unet.npz"))
+    return load_golden(golden_dir, "unet")
 
 
 @pytest.fixture(scope="module")

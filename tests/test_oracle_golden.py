@@ -7,18 +7,19 @@ import pytest
 import torch
 
 from oracle import condmdi_oracle as O
+from oracle.golden_io import load_golden
 
 B, D, L = 2, 263, 196
 
 
 @pytest.fixture(scope="module")
 def sched(golden_dir):
-    return np.load(os.path.join(golden_dir, "schedules.npz"))
+    return load_golden(golden_dir, "schedules")
 
 
 @pytest.fixture(scope="module")
 def samp(golden_dir):
-    return np.load(os.path.join(golden_dir, "sampler.npz"))
+    return load_golden(golden_dir, "sampler")
 
 
 @pytest.mark.parametrize("name,resp", [("full", ""), ("ddim50", "ddim50"), ("ddim100", "ddim100"), ("sect", "10,15,20")])
@@ -37,8 +38,8 @@ def test_gradient_schedule(sched, name):
 
 
 def test_keyframe_masks_bit_exact(golden_dir):
-    g = np.load(os.path.join(golden_dir, "masks.npz"))
-    keys = sorted(k[:-5] for k in g.files if k.endswith(".bits"))
+    g = load_golden(golden_dir, "masks")
+    keys = sorted(k[:-5] for k in g if k.endswith(".bits"))
     assert len(keys) == 27
     for key in keys:
         mode, T, fm = key.split(".")
@@ -118,7 +119,7 @@ def test_ddim50_full_loop_matches_reference(samp):
 def test_recover_from_ric_matches_reference(golden_dir, tag, abs_3d):
     """Post-processing row (SURVEY 8f-2): the restatement of recover_from_ric / inv_transform against the
     reference's own output (sample/synthesize.py:153-157 chain)."""
-    g = np.load(os.path.join(golden_dir, "postprocess.npz"))
+    g = load_golden(golden_dir, "postprocess")
     inp = O.postprocess_inputs()
     got = O.sample_to_joints(inp["sample"], g[f"{tag}.mean"], g[f"{tag}.std"], 22, abs_3d)
     assert got.shape == (3, 22, 3, 196)
@@ -131,7 +132,7 @@ def test_recover_from_ric_matches_reference(golden_dir, tag, abs_3d):
 def test_full_length_loop_fixture_last_steps(golden_dir):
     """tests/golden/long_loop.npz = the reference's own 1000-step DDPM loop (B=2).  The CPU suite replays its last
     five steps from the reference's state at t=4 (the whole chain takes minutes on a CPU; the GPU suite runs all of it)."""
-    g = np.load(os.path.join(golden_dir, "long_loop.npz"))
+    g = load_golden(golden_dir, "long_loop")
     tape = O.long_loop_tape()
     assert np.allclose([float(tape.double().sum()), float(tape[500].double().abs().sum())], g["tape_checksum"], rtol=1e-12)
     sd, tab, c = O.random_state_dict(seed=7, text=False), O.make_tables(""), O.Conditioning()
@@ -164,7 +165,7 @@ def test_stock_torch_standin_equals_oracle_on_cpu():
 
 def test_oracle_long_chains_vs_reference_golden(golden_dir):
     """tests/golden/chains.npz (reference outputs): whole DDIM-100 loop and the t = 49..0 tail of CFG + imputation."""
-    g = np.load(os.path.join(golden_dir, "chains.npz"))
+    g = load_golden(golden_dir, "chains")
     gi = O.golden_inputs()
     tape = gi["tape"]
     sd = O.random_state_dict(seed=7, text=False)
@@ -180,7 +181,7 @@ def test_oracle_long_chains_vs_reference_golden(golden_dir):
 
 def test_oracle_unet_vs_reference_golden(golden_dir):
     """tests/golden/unet.npz: the reference's MDM_UNET (dim 512 x (2,2,2,2), AdaGN, keyframe-conditioned, text)."""
-    g = np.load(os.path.join(golden_dir, "unet.npz"))
+    g = load_golden(golden_dir, "unet")
     gi = O.golden_inputs()
     sd = O.random_unet_state_dict(seed=11, text=True)
     assert O.is_unet(sd) and O.unet_levels_of(sd) == 4
