@@ -15,7 +15,8 @@ import types
 
 from .diffusion import GaussianDiffusion, from_reference_diffusion
 
-_LOOPS = ("p_sample_loop", "p_sample_loop_progressive", "ddim_sample_loop", "ddim_sample_loop_progressive")
+_LOOPS = ("p_sample_loop", "p_sample_loop_progressive", "ddim_sample_loop", "ddim_sample_loop_progressive",
+          "plms_sample_loop", "plms_sample_loop_progressive")
 
 
 def accelerate(ref_diffusion):
@@ -26,7 +27,8 @@ def accelerate(ref_diffusion):
 
 
 def install(ref_diffusion, fallback_to_reference: bool = False):
-    """Replace the four sampling loops of a reference diffusion object by the engine's, in place.
+    """Replace the six sampling loops (DDPM, DDIM, PLMS and their progressive forms) of a reference diffusion object by
+    the engine's, in place.
 
     Configurations the engine does not implement raise NotImplementedError.  With fallback_to_reference=True those
     (and only those) are forwarded to the reference's original PyTorch loop instead -- an explicit opt-in for
@@ -35,7 +37,7 @@ def install(ref_diffusion, fallback_to_reference: bool = False):
     fast = from_reference_diffusion(ref_diffusion)
     ref_diffusion._condmdi_b200 = fast
     for name in _LOOPS:
-        original = getattr(ref_diffusion, name)
+        original = getattr(ref_diffusion, name, None)  # None: an object without this loop gains the engine's
 
         def make(name=name, original=original):
             def loop(self, *args, **kwargs):
@@ -44,7 +46,7 @@ def install(ref_diffusion, fallback_to_reference: bool = False):
                     # generator, so an unsupported configuration surfaces inside this try block too)
                     return getattr(fast, name)(*args, **kwargs)
                 except NotImplementedError:
-                    if fallback_to_reference:
+                    if fallback_to_reference and original is not None:
                         return original(*args, **kwargs)
                     raise
             return loop

@@ -16,6 +16,7 @@ PRECISION_BF16 = 1
 RNG_ENGINE, RNG_TORCH = 0, 1
 SAMPLER_DDPM = 0
 SAMPLER_DDIM = 1
+SAMPLER_PLMS = 2
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
 
 EXPORTS = [
@@ -51,7 +52,8 @@ class SampleArgs(Structure):
                 ("inpainted_motion", c_void_p), ("inpainting_mask", c_void_p), ("recon_guidance", c_int32),
                 ("stop_recguidance_at", c_int32), ("recon_coef", POINTER(c_float)), ("pred_xstart_out", c_void_p),
                 ("dump_xstart", c_void_p), ("dump_steps", POINTER(c_int32)), ("n_dump", c_int32),
-                ("host_buffers", c_int32), ("use_graph", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p)]
+                ("host_buffers", c_int32), ("use_graph", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p),
+                ("plms_order", c_int32), ("plms_old_eps_out", c_void_p)]
 
 
 class LibraryMissing(RuntimeError):

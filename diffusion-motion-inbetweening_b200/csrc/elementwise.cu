@@ -6,6 +6,7 @@
 //   diffusion_step         p_mean_variance tail + p_sample / ddim_sample           gaussian_diffusion.py:352-534,656-713,1358-1416
 //                          + ClassifierFreeSampleModel combine                     cfg_sampler.py:25-35
 //                          + keyframe imputation blend                             gaussian_diffusion.py:427-435
+//   plms_step              plms_sample (pseudo linear multistep), same combine      gaussian_diffusion.py:1589-1687
 //   layout converters      reference [B,D,1,L] <-> frame-major [B*L, D_pad]
 //
 // The step kernel uses explicit non-contracted fp32 intrinsics (__fmul_rn/__fadd_rn) in the
@@ -201,6 +202,167 @@ __global__ void fill_normal_ref_kernel(float* out, int B, size_t per_sample, uns
 }
 
 // ---------------------------------------------------------------------------------------------
+// pred_xstart of one element (START_X, no clipping, :513-515): the model output (+ classifier-free guidance:
+// out_uncond + scale * (out - out_uncond), cfg_sampler.py:35), then reconstruction guidance or the imputation blend
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float step_x0(float mo, float mu, float ob, unsigned char mk, float gg, float gu, int cfg, int guided,
+                                         bool do_impute, float text_scale, float guide_c) {
+  float out = mo;
+  if (cfg) out = __fadd_rn(mu, __fmul_rn(text_scale, __fsub_rn(out, mu)));
+  if (guided) {
+    // reconstruction guidance (:416-425): cond_grad = grad * ~M ; tilde = hat - (w_r sqrt(abar) / 2) cond_grad ;
+    // output = tilde * ~M + (imputing ? x_obs : hat) * M
+    const float m = mk ? 1.0f : 0.0f;
+    float g = gg;
+    if (cfg) g = __fadd_rn(g, gu);
+    g = __fmul_rn(g, 1.0f - m);
+    const float tilde = __fsub_rn(out, __fmul_rn(guide_c, g));
+    out = __fadd_rn(__fmul_rn(tilde, 1.0f - m), __fmul_rn(do_impute ? ob : out, m));
+  } else if (do_impute) {
+    // imputation: (hat_x * ~M) + (x_obs * M)   (gaussian_diffusion.py:435)
+    const float m = mk ? 1.0f : 0.0f;
+    out = __fadd_rn(__fmul_rn(out, 1.0f - m), __fmul_rn(ob, m));
+  }
+  return out;
+}
+
+// Bumps the block-arrival counter at step_ptr[1]; the last block to arrive stores `next` as the step index (every
+// block has read the old one by then).
+__device__ __forceinline__ void advance_step(int* step_ptr, int next) {
+  __shared__ bool is_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0 && threadIdx.y == 0) {
+    const unsigned int total = gridDim.x * gridDim.y * gridDim.z;
+    unsigned int* counter = reinterpret_cast<unsigned int*>(step_ptr + 1);
+    const unsigned int prev = atomicAdd(counter, 1u);
+    is_last = (prev == total - 1);
+    if (is_last) {
+      *counter = 0;
+      *step_ptr = next;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// PLMS step (plms_sample, gaussian_diffusion.py:1589-1687, cond_fn = None) on frame-major state [B*L, D_pad].  One
+// thread = 4 consecutive features of one frame.  No noise is drawn.  The eps history lives in a ring of three
+// [B*L, D_pad] buffers: eps of loop iteration k is at slot k % 3, with k = step_ptr[2] - t (step_ptr[2] holds the
+// step index the history started at), so one kernel serves every Adams-Bashforth step.
+//   phase 0  Adams-Bashforth step at t: one evaluation; advances t -> t - 1
+//   phase 1  first step, after the evaluation at t: stores eps_0 and x_t, writes the second evaluation's input
+//            m = x0 sqrt(abp) + sqrt(1 - abp) eps_0 (or, at t = 0, the sample x0); advances t -> t - 1
+//   phase 2  first step, after the evaluation at t - 1 (= step_ptr[0]): the improved Euler sample from the kept x_t;
+//            leaves the step index at t - 1
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, const PlmsParams q) {
+  const int t_eval = *p.step_ptr;                    // step index of the evaluation in model_out
+  const int t = q.phase == 2 ? t_eval + 1 : t_eval;  // step index of the PLMS step
+  const int k = p.step_ptr[2] - t;                   // loop iteration since the history started
+  const int cur_order = min(q.order, k + 1);
+  const float r1e = p.tab.sqrt_recip_acp[t_eval], r2e = p.tab.sqrt_recipm1_acp[t_eval];
+  const float r1 = p.tab.sqrt_recip_acp[t], r2 = p.tab.sqrt_recipm1_acp[t];
+  const float abp = p.tab.acp_prev[t];
+  const float sq_abp = sqrtf(abp), sq_1m_abp = sqrtf(__fsub_rn(1.0f, abp));
+  const bool do_impute = p.impute && (t_eval >= p.stop_imputation_at);
+  const float guide_c = p.guided ? p.guide_coef[t_eval] : 0.f;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i4 < n4) {
+    const size_t idx = i4 * 4;
+    const int c = (int)(idx % p.D_pad);
+    const int b = (int)(idx / ((size_t)p.L * p.D_pad));
+    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
+    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
+    const bool need_obs = p.guided || do_impute;
+    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
+    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
+    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
+    if (p.guided) {
+      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
+      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
+    }
+    float* slot0 = q.eps_hist;
+    float* cur = q.eps_hist + (size_t)(k % 3) * q.hist_stride;
+    const float* h2 = q.eps_hist + (size_t)((k + 2) % 3) * q.hist_stride;  // iteration k - 1
+    const float* h3 = q.eps_hist + (size_t)((k + 1) % 3) * q.hist_stride;  // k - 2
+    const float* h4 = cur;                                                 // k - 3 (read before it is overwritten)
+    float4 e2v = make_float4(0.f, 0.f, 0.f, 0.f), e3v = e2v, e4v = e2v, xkv = e2v;
+    if (q.phase == 0) {
+      if (cur_order >= 2) e2v = *reinterpret_cast<const float4*>(h2 + idx);
+      if (cur_order >= 3) e3v = *reinterpret_cast<const float4*>(h3 + idx);
+      if (cur_order >= 4) e4v = *reinterpret_cast<const float4*>(h4 + idx);
+    } else if (q.phase == 2) {
+      e2v = *reinterpret_cast<const float4*>(slot0 + idx);  // eps_0
+      xkv = *reinterpret_cast<const float4*>(q.x_keep + idx);
+    }
+    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
+    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
+    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
+    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
+    const float e2[4] = {e2v.x, e2v.y, e2v.z, e2v.w}, e3[4] = {e3v.x, e3v.y, e3v.z, e3v.w}, e4[4] = {e4v.x, e4v.y, e4v.z, e4v.w};
+    const float xk[4] = {xkv.x, xkv.y, xkv.z, xkv.w};
+    float xn4[4], x04[4], ep4[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float xn = 0.f, x0 = 0.f, eps = 0.f;
+      if (c + j < p.D) {
+        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
+        // _predict_eps_from_xstart at the evaluation's (x, t) (:551-555)
+        eps = __fdiv_rn(__fsub_rn(__fmul_rn(r1e, xtv[j]), x0), r2e);
+        float ep, x;
+        if (q.phase == 1) {
+          // pseudo improved Euler, first half (:1647-1654): the input of the evaluation at t - 1
+          xn = t != 0 ? __fadd_rn(__fmul_rn(x0, sq_abp), __fmul_rn(sq_1m_abp, eps)) : x0;
+        } else {
+          if (q.phase == 2) {
+            ep = __fdiv_rn(__fadd_rn(e2[j], eps), 2.0f);  // (eps_0 + eps_2) / 2 (:1655)
+            x = xk[j];
+          } else {
+            // Adams-Bashforth (:1660-1673), e_1 = eps the newest
+            if (cur_order == 2) {
+              ep = __fdiv_rn(__fsub_rn(__fmul_rn(3.0f, eps), e2[j]), 2.0f);
+            } else if (cur_order == 3) {
+              ep = __fdiv_rn(__fadd_rn(__fsub_rn(__fmul_rn(23.0f, eps), __fmul_rn(16.0f, e2[j])), __fmul_rn(5.0f, e3[j])), 12.0f);
+            } else if (cur_order == 4) {
+              ep = __fdiv_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(55.0f, eps), __fmul_rn(59.0f, e2[j])), __fmul_rn(37.0f, e3[j])),
+                                       __fmul_rn(9.0f, e4[j])), 24.0f);
+            } else {
+              ep = eps;
+            }
+            x = xtv[j];
+          }
+          // pred' = _predict_xstart_from_eps(x, t, eps') (:536-541); mean = pred' sqrt(abp) + sqrt(1 - abp) eps'
+          const float pp = __fsub_rn(__fmul_rn(r1, x), __fmul_rn(r2, ep));
+          const float mean = __fadd_rn(__fmul_rn(pp, sq_abp), __fmul_rn(sq_1m_abp, ep));
+          xn = t != 0 ? mean : x0;  // :1679-1681
+        }
+      }
+      xn4[j] = xn;
+      x04[j] = x0;
+      ep4[j] = eps;
+    }
+    if (q.phase == 0) *reinterpret_cast<float4*>(cur + idx) = make_float4(ep4[0], ep4[1], ep4[2], ep4[3]);
+    if (q.phase == 1) {
+      *reinterpret_cast<float4*>(slot0 + idx) = make_float4(ep4[0], ep4[1], ep4[2], ep4[3]);
+      *reinterpret_cast<float4*>(q.x_keep + idx) = xt4;
+    }
+    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
+    uint32_t h01, l01, h23, l23;
+    split_bf16x2(xn4[0], xn4[1], h01, l01);
+    split_bf16x2(xn4[2], xn4[3], h23, l23);
+    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
+    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
+    // pred_xstart is the FIRST evaluation's x0 (:1685)
+    if (p.pred_xstart && q.phase != 2) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+  }
+  if (q.phase != 2) advance_step(p.step_ptr, t - 1);
+}
+
+// ---------------------------------------------------------------------------------------------
 // diffusion step. grid: (ceil(L/32), ceil(D_pad/32), B); block 32x8. Each block owns a 32(l) x 32(c)
 // tile: frame-major operands are read/written with c fastest, the reference-layout noise tape with
 // l fastest, through a padded smem tile.
@@ -293,24 +455,7 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
       for (int j = 0; j < 4; ++j) {
         float xn = 0.f, x0 = 0.f;
         if (c + j < p.D) {
-          // model output (+ classifier-free guidance: out_uncond + scale * (out - out_uncond), cfg_sampler.py:35)
-          float out = mo[j];
-          if (p.cfg) out = __fadd_rn(mu[j], __fmul_rn(text_scale, __fsub_rn(out, mu[j])));
-          if (p.guided) {
-            // reconstruction guidance (:416-425): cond_grad = grad * ~M ; tilde = hat - (w_r sqrt(abar) / 2) cond_grad ;
-            // output = tilde * ~M + (imputing ? x_obs : hat) * M
-            const float m = mk[j] ? 1.0f : 0.0f;
-            float g = gg[j];
-            if (p.cfg) g = __fadd_rn(g, gu[j]);
-            g = __fmul_rn(g, 1.0f - m);
-            const float tilde = __fsub_rn(out, __fmul_rn(guide_c, g));
-            out = __fadd_rn(__fmul_rn(tilde, 1.0f - m), __fmul_rn(do_impute ? ob[j] : out, m));
-          } else if (do_impute) {
-            // imputation: (hat_x * ~M) + (x_obs * M)   (gaussian_diffusion.py:435)
-            const float m = mk[j] ? 1.0f : 0.0f;
-            out = __fadd_rn(__fmul_rn(out, 1.0f - m), __fmul_rn(ob[j], m));
-          }
-          x0 = out;  // START_X, no clipping (:513-515)
+          x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
           const float xt = xtv[j];
           const float noise = s_noise[cq + j][ll];
           if (p.sampler == 2) {
@@ -628,6 +773,14 @@ cudaError_t launch_token_rows(const TokenParams& p, cudaStream_t stream) {
 cudaError_t launch_diffusion_step(const StepParams& p, cudaStream_t stream) {
   dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
   return launch_kernel(diffusion_step_kernel, grid, block, 0, stream, p);
+}
+
+cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStream_t stream) {
+  if (q.order < 2 || q.order > 4 || q.phase < 0 || q.phase > 2 || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.eps_hist ||
+      !q.x_keep)
+    return cudaErrorInvalidValue;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  return launch_kernel(plms_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_ref_to_frames(const float* ref, int B, int D, int L, int D_pad, float* out_f32, __nv_bfloat16* out_hi,

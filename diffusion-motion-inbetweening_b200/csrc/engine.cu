@@ -11,6 +11,7 @@
 // The step index lives on the device (decremented by diffusion_step), so the same graph is replayed for
 // every step of a loop with no host work in between (reference: one Python iteration + ~150 PyTorch ops
 // + several H2D table copies per step, gaussian_diffusion.py:1270-1297, :2225, respace.py:129).
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -90,6 +91,7 @@ struct GraphKey {
   float eta;
   const void* tape;
   int t0, uncond, guided, group;
+  int plms_order, plms_phase, guided2;  // PLMS: order, step kind (PlmsStep), guidance of the first step's second evaluation
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -169,6 +171,11 @@ struct cmdi_engine {
   long long* chain_dbg = nullptr;               // CMDI_CHAIN_DBG=1: cycle counters of layer 1's chain during cmdi_profile_pass
   std::map<int, ChainTables> chain_tables;
   UnetModel* unet = nullptr;  // MDM_UNET denoiser (cfg.arch == CMDI_ARCH_UNET): engine_unet.inc
+  // PLMS (allocated by the first PLMS call): the eps history ring [3][maxB*L, D_pad] and the first step's x_t; the host
+  // side of the running history, which a `resume` call continues
+  float *plms_hist = nullptr, *plms_keep = nullptr;
+  bool plms_live = false;
+  int plms_order = 0, plms_B = 0, plms_t_start = 0, plms_steps = 0;
   std::map<GraphKey, cudaGraphExec_t> graphs;
   int64_t launches = 0;
 };
@@ -1150,8 +1157,17 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CK(cudaSetDevice(e->device));
   const int B = a->batch;
   CKI(check_ready(e, B, true));
-  if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM) {
+  if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS) {
     set_last_error("unknown sampler %d", a->sampler);
+    return 1;
+  }
+  const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
+  if (plms && (a->plms_order < 2 || a->plms_order > 4)) {
+    set_last_error("plms_order %d outside [2, 4]", a->plms_order);
+    return 1;
+  }
+  if (plms && (a->noise_tape || a->dump_xstart)) {
+    set_last_error("PLMS draws no per-step noise and has no dump_steps: noise_tape and dump_xstart must be NULL");
     return 1;
   }
   if (a->cfg && (!a->cond_emb || !a->text_scale)) {
@@ -1183,6 +1199,25 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const size_t n = (size_t)B * e->D * e->L;
   const int t0 = e->T - 1 - a->skip_timesteps;
   const int nsteps = (a->num_steps > 0 && a->num_steps < t0 + 1) ? a->num_steps : t0 + 1;
+  // PLMS: a call without `resume` starts a new eps history at t0; a `resume` call continues the running one
+  int hist_t0 = t0;
+  if (plms) {
+    if (a->resume) {
+      if (!e->plms_live || e->plms_order != a->plms_order || e->plms_B != B || t0 != e->plms_t_start - e->plms_steps) {
+        set_last_error("PLMS resume at step %d does not continue the running history", t0);
+        return 1;
+      }
+      hist_t0 = e->plms_t_start;
+    } else {
+      if (!e->plms_hist) {
+        const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
+        CKI(dev_alloc(e, &e->plms_hist, 3 * slot));
+        CKI(dev_alloc(e, &e->plms_keep, slot));
+      }
+      e->plms_live = true;
+      e->plms_order = a->plms_order; e->plms_B = B; e->plms_t_start = t0; e->plms_steps = 0;
+    }
+  }
   CKI(ensure_temb(e, s));
   CKI(prepare_chain(e, a->cfg ? 2 * B : B));
   int rc = 0;
@@ -1243,7 +1278,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CKI(prepare_cond(e, B, a->cond_emb, host, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, t0, s));
-  CK(launch_set_int(e->step_ctr + 2, t0, s));
+  CK(launch_set_int(e->step_ctr + 2, hist_t0, s));
   e->launches += 2;
 
   const float* tape = a->noise_tape;
@@ -1308,9 +1343,78 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int group = e->steps_per_graph > 1 ? e->steps_per_graph : 1;
   cudaGraphExec_t exec1[2] = {nullptr, nullptr}, execg[2] = {nullptr, nullptr};  // [guided]
 
+  // ---- PLMS (gaussian_diffusion.py:1589-1804) ----
+  // The first step of a history is the pseudo improved Euler step: evaluation at t, plms_step_kernel phase 1, evaluation
+  // at t - 1 (its guidance and imputation predicates tested at t - 1), phase 2; at t = 0 the second evaluation cannot
+  // change the result (sample = x0) and is skipped.  Every later step is one evaluation and one Adams-Bashforth kernel.
+  enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
+  auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
+    StepParams sp{};
+    sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.B = B; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
+    sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
+    sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
+    sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
+    sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
+    sp.pred_xstart = e->pred_x0;
+    PlmsParams q{};
+    q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
+    q.eps_hist = e->plms_hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
+    const bool guided[2] = {g1, g2};
+    for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
+      CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided[ev] ? &e->stash : nullptr));
+      if (guided[ev]) CKI(run_backward(e, B, a->cfg != 0, st));
+      sp.guided = guided[ev];
+      if (ev == 1) q.phase = 2;
+      CK(launch_plms_step(sp, q, st));
+    }
+    return 0;
+  };
+  auto plms_step = [&](int k) -> int {
+    const int t = t0 - k;
+    const int kind = e->plms_steps + k > 0 ? kPlmsSteady : (t > 0 ? kPlmsFirst : kPlmsFirstAtZero);
+    const bool g1 = a->recon_guidance && t >= a->stop_recguidance_at;
+    const bool g2 = kind == kPlmsFirst && a->recon_guidance && t - 1 >= a->stop_recguidance_at;
+    GraphKey key{};
+    memset(&key, 0, sizeof(key));
+    key.B = B; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
+    key.stop_at = a->stop_imputation_at; key.has_cond = has_cond; key.uncond = a->uncond != 0;
+    key.guided = g1; key.group = 1; key.plms_order = a->plms_order; key.plms_phase = kind; key.guided2 = g2;
+    const bool via_graph = a->use_graph && !e->no_graph && (nsteps >= 3 || a->use_graph >= 2 || e->graphs.count(key) != 0);
+    if (via_graph) {
+      auto it = e->graphs.find(key);
+      if (it == e->graphs.end()) {
+        cudaStream_t cs = nullptr;
+        CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+        cudaGraph_t graph = nullptr;
+        CK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+        const int erc = enqueue_plms(cs, kind, g1, g2);
+        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
+        cudaStreamDestroy(cs);
+        if (erc) return 1;
+        CK(ce);
+        cudaGraphExec_t ex = nullptr;
+        CK(cudaGraphInstantiate(&ex, graph, 0));
+        cudaGraphDestroy(graph);
+        it = e->graphs.emplace(key, ex).first;
+      }
+      CK(cudaGraphLaunch(it->second, s));
+    } else {
+      CKI(enqueue_plms(s, kind, g1, g2));
+    }
+    const int per_eval = launches_per_pass(e, g1) + 1 + (g1 ? launches_per_backward(e) : 0);
+    e->launches += per_eval;
+    if (kind == kPlmsFirst) e->launches += launches_per_pass(e, g2) + 1 + (g2 ? launches_per_backward(e) : 0);
+    return 0;
+  };
+
   int dump_i = 0;
   auto guided_at = [&](int k) { return a->recon_guidance && (t0 - k) >= a->stop_recguidance_at; };
   for (int k = 0; k < nsteps;) {
+    if (plms) {
+      CKI(plms_step(k));
+      ++k;
+      continue;
+    }
     // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
     const bool guided = guided_at(k);
     int run = 1;
@@ -1369,6 +1473,23 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     if (a->pred_xstart_out) CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, a->pred_xstart_out, s));
   }
   e->launches += a->pred_xstart_out ? 2 : 1;
+  if (plms) {
+    e->plms_steps += nsteps;
+    if (a->plms_old_eps_out) {
+      // the reference's old_eps list after this call's last step: eps of the last min(steps, order - 1) iterations,
+      // oldest first
+      const int n_hist = std::min(e->plms_steps, a->plms_order - 1);
+      for (int j = 0; j < n_hist; ++j) {
+        const int it = e->plms_steps - n_hist + j;
+        const float* src = e->plms_hist + (size_t)(it % 3) * e->maxB * e->L * e->D_pad;
+        float* dst = a->plms_old_eps_out + (size_t)j * n;
+        CK(launch_frames_to_ref(src, B, e->D, e->L, e->D_pad, host ? e->ref_b : dst, s));
+        if (host) CK(cudaMemcpyAsync(dst, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));
+      }
+      if (host) CK(cudaStreamSynchronize(s));
+      e->launches += n_hist;
+    }
+  }
   return 0;
 }
 

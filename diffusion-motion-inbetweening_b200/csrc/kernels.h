@@ -236,6 +236,20 @@ struct StepParams {
   float* pred_xstart;          // [B*L, D_pad] or null
 };
 cudaError_t launch_diffusion_step(const StepParams& p, cudaStream_t stream);
+// PLMS step (gaussian_diffusion.py:1589-1687) on the same state and combine inputs as StepParams (its sampler, eta,
+// noise, rng, tape and advance fields are not read; x_next / x_next_hi are required).  The eps history is a device
+// ring indexed by the loop iteration k = step_ptr[2] - t, so one captured graph serves every Adams-Bashforth step.
+struct PlmsParams {
+  int order;           // 2..4
+  int phase;           // 0: Adams-Bashforth step after the evaluation at t (advances t -> t - 1);
+                       // 1: first step, after the evaluation at t: keeps eps_0 and x_t, writes the input of the
+                       //    evaluation at t - 1 (at t = 0: the sample) and advances t -> t - 1;
+                       // 2: first step, after the evaluation at t - 1 = step_ptr[0]: writes the sample, step unchanged
+  float* eps_hist;     // [3][B*L, D_pad]: eps of iteration k at slot k % 3 (the first step's eps_0 at slot 0)
+  size_t hist_stride;  // elements between slots
+  float* x_keep;       // [B*L, D_pad] the first step's x_t, kept across its second evaluation
+};
+cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStream_t stream);
 
 // HumanML3D vectors -> joint positions (recover_from_ric), strides in elements; mean/stdv null = already de-normalised
 cudaError_t launch_recover_from_ric(const float* data, long long sb, long long sf, long long sc, const float* mean,

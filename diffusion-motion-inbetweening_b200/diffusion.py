@@ -3,14 +3,14 @@
 Mirrors (same names, argument meaning and error behaviour; paths relative to the reference repository):
     get_named_beta_schedule / betas_for_alpha_bar   diffusion/gaussian_diffusion.py:24-71
     ModelMeanType / ModelVarType / DiffusionConfig  :74-136
-    GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1454-1587
+    GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1454-1587, :1589-1804
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
-`p_sample_loop` / `ddim_sample_loop` run the WHOLE loop in one native call (`cmdi_sample`): no per-step
-Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
+`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` run the WHOLE loop in one native call (`cmdi_sample`): no
+per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
-`p_mean_variance` / `p_sample` / `ddim_sample_with_grad` is done by the CUDA kernels in csrc/.
+`p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` is done by the CUDA kernels in csrc/.
 
 Not accelerated (raise NotImplementedError, like the reference does for its own unsupported branches):
 cond_fn / 'gmd' classifier guidance, learned variances, EPSILON/PREVIOUS_X parametrisations,
@@ -152,10 +152,11 @@ class GaussianDiffusion:
         return y
 
     def _run(self, sampler, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image, randomize_class,
-             dump_steps, const_noise, eta, progressive=False):
+             dump_steps, const_noise, eta, progressive=False, order=2):
         if model_kwargs is None:
             model_kwargs = {}
         y = self._check_supported(cond_fn, const_noise, randomize_class, model_kwargs)
+        plms = sampler == capi.SAMPLER_PLMS
         if sampler == capi.SAMPLER_DDPM:
             assert cond_fn is None, "only support the case where cond_fn is None"  # gaussian_diffusion.py:685
         elif cond_fn is not None:
@@ -231,7 +232,13 @@ class GaussianDiffusion:
         if tape is not None:
             tape = tape[1:]
         seed, rng_args = 0, {}
-        if tape is None:
+        if plms:
+            # plms_sample_loop_progressive draws nothing after x_T (:1767-1770): a tape contributes tape[0] only, torch's
+            # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine"
+            tape = None
+            if x_T is None:
+                seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+        elif tape is None:
             n_draws = self.num_timesteps - skip_timesteps  # one randn_like per loop iteration (:696, :1407)
             rng_args = _torch_stream_args(device, int(np.prod(shape)), n_draws, lazy=progressive) if self.rng == "torch" else None
             if rng_args is None:
@@ -259,6 +266,11 @@ class GaussianDiffusion:
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
+        if plms:
+            common["plms_order"] = int(order)
+            if progressive:
+                return self._plms_progressive(eng, x_T, init_image, skip_timesteps, common)
+            return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T, **common)
         if not progressive:
             res = eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T,
                              noise_tape=None if tape is None else tape, want_pred_xstart=False, dump_steps=dump_steps, **common)
@@ -283,6 +295,20 @@ class GaussianDiffusion:
                 # breaks out of the generator early leaves it where the reference would
                 _advance_torch_generator(eng.device, inc)
             yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
+
+    def _plms_progressive(self, eng, x_T, init_image, skip_timesteps, common):
+        """plms_sample_loop_progressive's generator: one native call per step, each continuing the eps history the engine
+        keeps on the device, so the samples equal the fused loop's bit for bit.  old_eps holds the values of the
+        reference's history list at that yield (the reference yields one list it keeps mutating)."""
+        n = self.num_timesteps - skip_timesteps
+        state = x_T
+        common = dict(common)
+        common["use_graph"] = 2 if common.get("use_graph", True) else 0
+        for k in range(n):
+            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, resume=(k > 0), init_image=init_image if k == 0 else None,
+                             x_T=state, want_pred_xstart=True, want_old_eps=True, **common)
+            state = res["sample"]
+            yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"], "old_eps": res["old_eps"]}
 
     # ------------------------------------------------------------------------------------------
     def p_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
@@ -321,6 +347,36 @@ class GaussianDiffusion:
         """gaussian_diffusion.py:1514-1587."""
         return self._run(capi.SAMPLER_DDIM, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
                              init_image, randomize_class, None, False, eta, progressive=True)
+
+    def plms_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
+                         device=None, progress=False, skip_timesteps=0, init_image=None, randomize_class=False,
+                         cond_fn_with_grad=False, order=2):
+        """gaussian_diffusion.py:1689-1736: pseudo linear multistep, deterministic after x_T.  The whole loop is one
+        native call; the eps history stays on the device."""
+        _check_plms_order(order)
+        return self._run(capi.SAMPLER_PLMS, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image,
+                         randomize_class, None, False, 0.0, order=order)["sample"]
+
+    def plms_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                                     model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                                     randomize_class=False, cond_fn_with_grad=False, order=2):
+        """gaussian_diffusion.py:1738-1804.  Yields {"sample", "pred_xstart", "old_eps"} per step; the configuration is
+        validated at the call (the reference defers its checks to the first next())."""
+        _check_plms_order(order)
+        return self._run(capi.SAMPLER_PLMS, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image,
+                         randomize_class, None, False, 0.0, progressive=True, order=order)
+
+
+def _check_plms_order(order) -> None:
+    """plms_sample's check (gaussian_diffusion.py:1608-1609), and errors at the call for the orders the reference accepts
+    there but cannot run: order 1 (its first step reads old_out["old_eps"] from None) and non-integral orders (the
+    Adams-Bashforth branch has no weights for them)."""
+    if not int(order) or not 1 <= order <= 4:
+        raise ValueError("order is invalid (should be int from 1-4).")
+    if order != int(order):
+        raise NotImplementedError(f"PLMS order {order!r} is not an integer")
+    if int(order) == 1:
+        raise TypeError("PLMS order 1 fails on the reference's first step ('NoneType' object is not subscriptable)")
 
 
 def space_timesteps(num_timesteps, section_counts):

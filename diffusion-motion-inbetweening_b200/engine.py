@@ -42,6 +42,7 @@ class Engine:
                    "cmdi_engine_create")
         self._h = handle
         self.schedule_key = None
+        self._plms_steps = 0  # iterations of the engine's running PLMS history (mirrors the native side)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -122,12 +123,14 @@ class Engine:
                recon_guidance: bool = False, stop_recguidance_at: int = 0, recon_coef: Optional[Sequence[float]] = None,
                want_pred_xstart: bool = False, dump_steps: Optional[Sequence[int]] = None, host_buffers: bool = False,
                use_graph: bool = True, out: Optional[torch.Tensor] = None, obs_x0: Optional[torch.Tensor] = None,
-               obs_mask: Optional[torch.Tensor] = None):
+               obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
         call is stream-ordered.  host_buffers=True: every tensor must be a CPU tensor (pinned for best speed); the
         H2D/D2H copies happen inside the call and the result is a CPU tensor valid on return.
+        sampler=SAMPLER_PLMS: `plms_order` is plms_sample's order; want_old_eps adds result["old_eps"], the eps history
+        list after the last step (oldest first), as plms_sample_loop_progressive yields it.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         dev = torch.device("cpu") if host_buffers else self.device
@@ -173,17 +176,29 @@ class Engine:
             if coef.shape != (self.num_timesteps,):
                 raise ValueError(f"recon_coef must have one entry per sampler step ({self.num_timesteps})")
             coef_arr = coef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+        n_iter = self.num_timesteps - int(skip_timesteps)
+        if num_steps:
+            n_iter = min(n_iter, int(num_steps))
+        plms_steps = n_iter + (self._plms_steps if resume else 0)  # iterations of the PLMS history after this call
+        old_eps, n_old = None, 0
+        if want_old_eps and sampler == capi.SAMPLER_PLMS:
+            n_old = min(plms_steps, int(plms_order) - 1)  # the length of the reference's list after that many steps
+            old_eps = torch.empty((max(n_old, 1),) + shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
         a = capi.SampleArgs(batch, sampler, float(eta), int(skip_timesteps), int(num_steps), int(resume), _ptr(init_image), _ptr(x_T), _ptr(noise_tape),
                             int(seed) & (2 ** 64 - 1), int(sample_offset), int(rng_mode), int(aten_offset), int(aten_increment),
                             int(aten_threads), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale),
                             _ptr(y_mask), int(imputate), int(stop_imputation_at), _ptr(inpainted_motion),
                             _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
                             dump_arr, n_dump, int(host_buffers),
-                            int(use_graph), _ptr(obs_x0), _ptr(obs_mask))
+                            int(use_graph), _ptr(obs_x0), _ptr(obs_mask), int(plms_order), _ptr(old_eps))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
         result = {"sample": out}
+        if sampler == capi.SAMPLER_PLMS:
+            self._plms_steps = plms_steps
+            if old_eps is not None:
+                result["old_eps"] = [old_eps[i] for i in range(n_old)]
         if pred is not None:
             result["pred_xstart"] = pred
         if dump is not None:

@@ -13,6 +13,7 @@
  *                                                      model/cfg_sampler.py:25-35 (ClassifierFreeSampleModel.forward)
  *   cmdi_sample             the sampling loop       <- diffusion/gaussian_diffusion.py:1149-1297 (p_sample_loop[_progressive]),
  *                                                      :1454-1587 (ddim_sample_loop[_progressive]),
+ *                                                      :1589-1804 (plms_sample_loop[_progressive]),
  *                                                      :352-534 (p_mean_variance), :656-713 (p_sample), :1358-1416 (ddim_sample_with_grad)
  *
  * Conventions
@@ -48,7 +49,8 @@ enum {
   CMDI_PRECISION_BF16 = 1    /* single bf16 MMA, fp32 accumulate: "fast" mode, does NOT meet rtol 1e-3 / atol 1e-4 */
 };
 
-enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1 };
+/* PLMS: pseudo linear multistep (plms_sample_loop, gaussian_diffusion.py:1589-1804): deterministic, no per-step noise */
+enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2 };
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
 
@@ -141,6 +143,12 @@ typedef struct {
      constant over the loop; NULL for models that do not consume them */
   const float* obs_x0;          /* ref layout */
   const uint8_t* obs_mask;      /* ref layout, bool bytes (NOT and-ed with y['mask']) */
+  /* CMDI_SAMPLER_PLMS only.  The eps history stays on the device: a call with resume = 0 starts a new one, a call with
+     resume = 1 continues it (x_T = the previous call's sample, skip_timesteps advanced by its steps).  noise_tape and
+     dump_xstart must be NULL: the only draw is x_T. */
+  int32_t plms_order;           /* 2..4 (plms_sample's `order`) */
+  float* plms_old_eps_out;      /* NULL, or (min(steps so far, plms_order - 1), B, 263, 1, 196): the reference's old_eps
+                                   list after the last step, oldest first (ref layout) */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
