@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("CONDMDI_B200_LIB") or os.path.join(HERE, "libcondmdi_
 
 PRECISION_BF16X3 = 3
 PRECISION_BF16 = 1
+PRECISION_FP16 = 2  # "autocast", MDM_UNET only: the arithmetic of torch.autocast("cuda", float16) (use_fp16 checkpoints)
 RNG_ENGINE, RNG_TORCH = 0, 1
 SAMPLER_DDPM = 0
 SAMPLER_DDIM = 1

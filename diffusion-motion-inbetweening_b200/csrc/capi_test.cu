@@ -60,8 +60,16 @@ extern "C" int cmdi_test_linear(const float* A, const float* W, const float* bia
   CK(a_lo.alloc((size_t)Mp * Kp * 2));
   CK(w_hi.alloc((size_t)Np * Kp * 2));
   CK(w_lo.alloc((size_t)Np * Kp * 2));
-  CK(launch_split_planes(A, M, K, K, a_hi.as<__nv_bfloat16>(), a_lo.as<__nv_bfloat16>(), Kp, stream));
-  CK(launch_split_planes(W, N, K, K, w_hi.as<__nv_bfloat16>(), w_lo.as<__nv_bfloat16>(), Kp, stream));
+  // precision 2 (CMDI_PRECISION_FP16): one fp16 plane per operand, bias and results rounded to fp16 like autocast
+  const bool f16 = precision == 2;
+  if (f16) {
+    CK(launch_conv_weight_planes(A, M, K, 1, K, a_hi.as<__nv_bfloat16>(), nullptr, Kp, stream, true));
+    CK(launch_conv_weight_planes(W, N, K, 1, K, w_hi.as<__nv_bfloat16>(), nullptr, Kp, stream, true));
+    precision = 1;
+  } else {
+    CK(launch_split_planes(A, M, K, K, a_hi.as<__nv_bfloat16>(), a_lo.as<__nv_bfloat16>(), Kp, stream));
+    CK(launch_split_planes(W, N, K, K, w_hi.as<__nv_bfloat16>(), w_lo.as<__nv_bfloat16>(), Kp, stream));
+  }
   const bool pair = true;  // every linear layer runs on the CTA-pair kernel (the sign of block_n is accepted and ignored)
   if (block_n < 0) block_n = -block_n;
   CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;
@@ -112,9 +120,9 @@ extern "C" int cmdi_test_linear(const float* A, const float* W, const float* bia
       p.out_lo = o_lo.as<__nv_bfloat16>();
       p.ld_bf = Np;
       if (getenv("CMDI_TEST_NOF32")) p.out_f32 = nullptr;
-      CK(launch_linear_pair(ma_hi, ma_lo, mw_hi, mw_lo, p, block_n, num_sms_of_current_device(), stream, stp));
+      CK(launch_linear_pair(ma_hi, ma_lo, mw_hi, mw_lo, p, block_n, num_sms_of_current_device(), stream, stp, f16));
     }
-    CK(launch_linear_pair(ma_hi, ma_lo, mw_hi, mw_lo, p, block_n, num_sms_of_current_device(), stream, stp));
+    CK(launch_linear_pair(ma_hi, ma_lo, mw_hi, mw_lo, p, block_n, num_sms_of_current_device(), stream, stp, f16));
     if (want_dbg) {
       std::vector<long long> h(148 * 16);
       CK(cudaStreamSynchronize(stream));

@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda.h>
 #include <stdio.h>
 #include <stdint.h>
@@ -47,6 +48,14 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi_word
   const float ha = __uint_as_float(hi_word << 16), hb = __uint_as_float(hi_word & 0xffff0000u);
   const __nv_bfloat162 l = __floats2bfloat162_rn(a - ha, b - hb);
   lo_word = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// fp32 -> the nearest fp16 value, as fp32 (the rounding CUDA autocast applies to every conv / linear output)
+__device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
+// fp16 x 2 -> one 32-bit word {a (low half), b (high half)}
+__device__ __forceinline__ uint32_t pack_f16x2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 // y = (x - mean) * rstd * gamma + beta with a fixed operation order: the LayerNorm kernel and the epilogues that
@@ -226,6 +235,14 @@ __device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(da), "l"(db), "r"(scale_d));
 }
+// the same MMA on fp16 operands (autocast precision: one fp16 plane per operand)
+__device__ __forceinline__ void wgmma_m64n64k16_ss_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
 __device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -270,7 +287,8 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
 // carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
 // instead, the bias stays at the level of a 64-long sum.  (Measured on H100: double-buffering 32-column chunks so that
 // the adds of one chunk overlap the MMAs of the next is no faster.)
-template <int PART_N>
+// F16: the operands are single fp16 planes (CMDI_PRECISION_FP16; `split` must be false), same descriptors and swizzle.
+template <int PART_N, bool F16 = false>
 __device__ __forceinline__ void mma_kblock_promoted(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], uint32_t sa, uint32_t sb,
                                                     uint32_t a_plane, uint32_t b_plane, bool split) {
   static_assert(PART_N % 64 == 0, "64-column chunks");
@@ -290,8 +308,13 @@ __device__ __forceinline__ void mma_kblock_promoted(float (&acc0)[PART_N / 2], f
       const uint64_t db = make_desc_kmajor_sw128(sb + ((split && term == 1) ? b_plane : 0u) + c * 64 * 128);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        wgmma_m64n64k16_ss(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
-        wgmma_m64n64k16_ss(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
+        if constexpr (F16) {
+          wgmma_m64n64k16_ss_f16(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
+          wgmma_m64n64k16_ss_f16(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
+        } else {
+          wgmma_m64n64k16_ss(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
+          wgmma_m64n64k16_ss(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
+        }
       }
     }
     wgmma_commit();

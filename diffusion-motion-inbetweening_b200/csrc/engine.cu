@@ -101,6 +101,7 @@ struct cmdi_engine {
   cmdi_model_cfg cfg{};
   int device = 0, num_sms = 132;
   int nsplit = 3;
+  bool f16 = false;  // CMDI_PRECISION_FP16 (MDM_UNET only): fp16 operands and CUDA autocast's rounding points, nsplit = 1
   int bn_qkv = kBnWide;
   int debug = 0, bn_wide = kBnWide, bn_narrow = kBnNarrow;  // CMDI_DEBUG / CMDI_BN_WIDE / CMDI_BN_NARROW (bring-up knobs)
   int steps_per_graph = 1;  // CMDI_GRAPH_STEPS: consecutive steps captured into one graph (10 and 50 measured: no gain over 1)
@@ -241,31 +242,39 @@ int upload_planes(cmdi_engine* e, Planes& pl, const cmdi_tensor_desc& t, int row
 }
 
 int run_linear(cmdi_engine* e, const Planes& a, const Planes& w, const LinearParams& p_in, int block_n, cudaStream_t s,
-               const Planes* out_planes = nullptr, const CUtensorMap* out_f32 = nullptr);
+               const Planes* out_planes = nullptr, const CUtensorMap* out_f32 = nullptr, bool f16 = false);
 
 int ensure_temb(cmdi_engine* e, cudaStream_t s) {
   if (e->temb_valid) return 0;
   // TimestepEmbedder (mdm.py:345-353) for every original timestep: time_embed(pe[t]), once per weight load, as two
   // launches of the pair GEMM (round 1 ran this table on fp32 CUDA cores: 2 x 0.65 ms on every weight load)
+  // fp16 mode: the same two layers under autocast (fp16 operands, fp16 results, SiLU on fp16): the table holds fp16 values
   const int n = 5000;
-  CK(launch_split_planes(e->pe, n, kDModel, kDModel, e->pe_p.hi, e->pe_p.lo, kDModel, s));
-  CK(launch_split_planes(e->te_w0, kDModel, kDModel, kDModel, e->te_w0_p.hi, e->te_w0_p.lo, kDModel, s));
-  CK(launch_split_planes(e->te_w2, kDModel, kDModel, kDModel, e->te_w2_p.hi, e->te_w2_p.lo, kDModel, s));
+  const int split = e->f16 ? 1 : 3;
+  if (e->f16) {
+    CK(launch_conv_weight_planes(e->pe, n, kDModel, 1, kDModel, e->pe_p.hi, nullptr, kDModel, s, true));
+    CK(launch_conv_weight_planes(e->te_w0, kDModel, kDModel, 1, kDModel, e->te_w0_p.hi, nullptr, kDModel, s, true));
+    CK(launch_conv_weight_planes(e->te_w2, kDModel, kDModel, 1, kDModel, e->te_w2_p.hi, nullptr, kDModel, s, true));
+  } else {
+    CK(launch_split_planes(e->pe, n, kDModel, kDModel, e->pe_p.hi, e->pe_p.lo, kDModel, s));
+    CK(launch_split_planes(e->te_w0, kDModel, kDModel, kDModel, e->te_w0_p.hi, e->te_w0_p.lo, kDModel, s));
+    CK(launch_split_planes(e->te_w2, kDModel, kDModel, kDModel, e->te_w2_p.hi, e->te_w2_p.lo, kDModel, s));
+  }
   LinearParams t0{};
-  t0.M = n; t0.N = kDModel; t0.K = kDModel; t0.nsplit = 3; t0.nsplit_out = 3; t0.bias = e->te_b0; t0.act = 2;
+  t0.M = n; t0.N = kDModel; t0.K = kDModel; t0.nsplit = split; t0.nsplit_out = split; t0.bias = e->te_b0; t0.act = 2;
   t0.out_hi = e->temb_h_p.hi; t0.out_lo = e->temb_h_p.lo; t0.ld_bf = kDModel;
-  CKI(run_linear(e, e->pe_p, e->te_w0_p, t0, kBnNarrow, s, &e->temb_h_p));
+  CKI(run_linear(e, e->pe_p, e->te_w0_p, t0, kBnNarrow, s, &e->temb_h_p, nullptr, e->f16));
   LinearParams t2{};
-  t2.M = n; t2.N = kDModel; t2.K = kDModel; t2.nsplit = 3; t2.nsplit_out = 3; t2.bias = e->te_b2;
+  t2.M = n; t2.N = kDModel; t2.K = kDModel; t2.nsplit = split; t2.nsplit_out = split; t2.bias = e->te_b2;
   t2.out_f32 = e->temb_table; t2.ld_f32 = kDModel;
-  CKI(run_linear(e, e->temb_h_p, e->te_w2_p, t2, kBnNarrow, s, nullptr, &e->temb_st));
+  CKI(run_linear(e, e->temb_h_p, e->te_w2_p, t2, kBnNarrow, s, nullptr, &e->temb_st, e->f16));
   e->launches += 5;
   e->temb_valid = true;
   return 0;
 }
 
 int run_linear(cmdi_engine* e, const Planes& a, const Planes& w, const LinearParams& p_in, int block_n, cudaStream_t s,
-               const Planes* out_planes, const CUtensorMap* out_f32) {
+               const Planes* out_planes, const CUtensorMap* out_f32, bool f16) {
   LinearParams p = p_in;
   p.debug = e->debug;
   LinearStoreMaps st;
@@ -274,7 +283,7 @@ int run_linear(cmdi_engine* e, const Planes& a, const Planes& w, const LinearPar
     st.f32 = out_f32;
   }
   if (a.has_tap) { st.a_tap_hi = &a.tap_hi; st.a_tap_lo = &a.tap_lo; }
-  CK(launch_linear_pair(a.map_hi, a.map_lo, w.pair_hi, w.pair_lo, p, block_n, e->num_sms, s, &st));
+  CK(launch_linear_pair(a.map_hi, a.map_lo, w.pair_hi, w.pair_lo, p, block_n, e->num_sms, s, &st, f16));
   return 0;
 }
 
@@ -694,8 +703,13 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
     set_last_error("unknown architecture %d", cfg->arch);
     return 1;
   }
+  if (cfg->precision == CMDI_PRECISION_FP16 && !is_unet) {
+    // no transformer checkpoint is trained or sampled with use_fp16
+    set_last_error("precision CMDI_PRECISION_FP16 (autocast) is implemented for the MDM_UNET denoiser only (arch = CMDI_ARCH_UNET)");
+    return 1;
+  }
   if (cfg->latent_dim != kDModel || cfg->njoints < 8 || cfg->max_batch < 1 ||
-      (cfg->precision != CMDI_PRECISION_BF16X3 && cfg->precision != CMDI_PRECISION_BF16) ||
+      (cfg->precision != CMDI_PRECISION_BF16X3 && cfg->precision != CMDI_PRECISION_BF16 && cfg->precision != CMDI_PRECISION_FP16) ||
       (!is_unet && (cfg->num_heads * 128 != cfg->latent_dim || cfg->ff_size % 256 != 0 || cfg->nframes + 1 > kAttnKeyPad))) {
     set_last_error("unsupported model configuration (need latent_dim=512, 4 heads of 128, ff %% 256 == 0, nframes <= 207)");
     return 1;
@@ -717,6 +731,7 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
   if (const char* g = getenv("CMDI_CHAIN_WIDE")) e->chain_wide = atoi(g) != 0;
   if (const char* g = getenv("CMDI_CHAIN_PUBLISH")) e->chain_publish_now = strcmp(g, "deferred") != 0;
   e->cfg = *cfg; e->device = device; e->num_sms = prop.multiProcessorCount; e->nsplit = cfg->precision;
+  if (cfg->precision == CMDI_PRECISION_FP16) { e->f16 = true; e->nsplit = 1; }
   // the chained launches spin on counters other CTA pairs bump: every pair must be resident at once
   if (e->use_chain && linear_chain_max_clusters(e->num_sms) < e->num_sms / 2) e->use_chain = false;
   e->D = cfg->njoints; e->D_pad = round_up(cfg->njoints, 8); e->L = cfg->nframes; e->S = cfg->nframes + 1;
@@ -1068,7 +1083,8 @@ int prepare_cond(cmdi_engine* e, int B, const float* cond_emb_user, bool host, c
   }
   CK(cudaMemcpyAsync(e->cond_emb, cond_emb_user, (size_t)B * 512 * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
   // embed_text(enc_text): once per call instead of once per step and pass (mdm.py:249-250 re-runs it every step)
-  CK(launch_small_linear(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, 0, s));
+  if (e->f16) CK(launch_small_linear_f16(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, s));
+  else CK(launch_small_linear(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, 0, s));
   e->launches += 1;
   return 0;
 }

@@ -2,6 +2,8 @@
 // persistent over the tile list.
 //
 // The W operand is loaded as two {64, BLOCK_N / 2} boxes (the tensor maps the engine builds for this kernel).
+// Operands are bf16 (one plane, or hi/lo planes with nsplit = 3) or, in the F16 instantiations, one fp16 plane each
+// (CMDI_PRECISION_FP16: CUDA autocast's arithmetic, see gemm_epilogue.cuh).
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include "kernels.h"
@@ -67,7 +69,7 @@ struct Producer {
   }
 };
 
-template <int BLOCK_N, int PART_N>
+template <int BLOCK_N, int PART_N, bool F16>
 __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const EpiStoreMaps& maps, Producer<BLOCK_N>& prod, bool is_producer,
                                                  int col_part, int lane_group, int lane, uint32_t epi_stage_addr) {
   constexpr int kPart0 = epi_part0_cols<BLOCK_N>();
@@ -87,14 +89,14 @@ __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const Ep
     for (int kb = 0; kb < num_k_blocks; ++kb) {
       mbar_wait(&bars->full[stage], phase);
       const uint32_t sa = smem_u32(prod.ring + (size_t)stage * prod.stage_bytes);
-      if (!(p.debug & 2)) mma_kblock_promoted<PART_N>(acc0, acc1, sa, sa + b_off, a_plane, b_plane, split);
+      if (!(p.debug & 2)) mma_kblock_promoted<PART_N, F16>(acc0, acc1, sa, sa + b_off, a_plane, b_plane, split);
       // the tensor cores have read this stage: it may be refilled
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars->empty[stage]);
       if (is_producer) prod.issue_next();
       if (++stage == num_stages) { stage = 0; phase ^= 1; }
     }
-    epilogue_tile<BLOCK_N, PART_N>(p, maps, acc0, acc1, m_blk, n_blk, lane_group, col_part, lane, epi_stage_addr);
+    epilogue_tile<BLOCK_N, PART_N, F16>(p, maps, acc0, acc1, m_blk, n_blk, lane_group, col_part, lane, epi_stage_addr);
   }
 }
 
@@ -105,7 +107,7 @@ __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const Ep
 // `num_stages` k-blocks ahead of the MMAs and across tile boundaries (the next tile's operands arrive under the epilogue).
 // Barriers: full[s] (1 arrival + the TMA transaction bytes), empty[s] (one arrival per warp once its wgmmas that read
 // stage s have completed).
-template <int BLOCK_N>
+template <int BLOCK_N, bool F16>
 __global__ void __launch_bounds__(kNumThreads, 1)
 linear2_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -151,13 +153,13 @@ linear2_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const uint32_t epi_stage_addr = smem_u32(epi_stage + warp_idx * kEpiStageBytes);
   const EpiStoreMaps epi_maps{&map_o_hi, &map_o_lo, &map_o_f32};
   if (col_part == 0)
-    mma_and_epilogue<BLOCK_N, kPart0>(p, epi_maps, prod, is_producer, col_part, lane_group, lane, epi_stage_addr);
+    mma_and_epilogue<BLOCK_N, kPart0, F16>(p, epi_maps, prod, is_producer, col_part, lane_group, lane, epi_stage_addr);
   else
-    mma_and_epilogue<BLOCK_N, BLOCK_N - kPart0>(p, epi_maps, prod, false, col_part, lane_group, lane, epi_stage_addr);
+    mma_and_epilogue<BLOCK_N, BLOCK_N - kPart0, F16>(p, epi_maps, prod, false, col_part, lane_group, lane, epi_stage_addr);
   if (p.tma_store && lane == 0) tma_store_wait_all();
 }
 
-template <int BLOCK_N>
+template <int BLOCK_N, bool F16>
 cudaError_t launch_impl2(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi, const CUtensorMap& w_lo,
                          const LinearParams& p_in, int num_sms, cudaStream_t stream, const LinearStoreMaps* st) {
   LinearParams p = p_in;
@@ -182,7 +184,7 @@ cudaError_t launch_impl2(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const
   int num_stages = (kSmemLimit - fixed) / stage_bytes;
   if (num_stages > kMaxStages) num_stages = kMaxStages;
   const size_t smem = (size_t)fixed + (size_t)num_stages * stage_bytes;
-  return launch_kernel(linear2_kernel<BLOCK_N>, dim3(ctas), dim3(kNumThreads), smem, stream, a_hi, a_lo, w_hi, w_lo,
+  return launch_kernel(linear2_kernel<BLOCK_N, F16>, dim3(ctas), dim3(kNumThreads), smem, stream, a_hi, a_lo, w_hi, w_lo,
                        o_hi, o_lo, o_f32, p, num_stages, num_m_blocks, num_n_blocks);
 }
 
@@ -193,21 +195,31 @@ cudaError_t configure_linear2_kernels() {
   auto set = [&](auto kernel) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
   };
-  set(linear2_kernel<128>); set(linear2_kernel<192>); set(linear2_kernel<256>);
+  set(linear2_kernel<128, false>); set(linear2_kernel<192, false>); set(linear2_kernel<256, false>);
+  set(linear2_kernel<128, true>); set(linear2_kernel<256, true>);
   return e;
 }
 
 // Tensor maps: A box {64, 128}; W box {64, block_n / 2}.
 cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi, const CUtensorMap& w_lo,
                                const LinearParams& p, int block_n, int num_sms, cudaStream_t stream,
-                               const LinearStoreMaps* st) {
+                               const LinearStoreMaps* st, bool f16) {
   if (p.N % 8 != 0 || (p.nsplit != 1 && p.nsplit != 3)) {
     set_last_error("launch_linear_pair: N must be a multiple of 8 and nsplit 1 or 3 (N=%d nsplit=%d)", p.N, p.nsplit);
     return cudaErrorInvalidValue;
   }
-  if (block_n == 256) return launch_impl2<256>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
-  if (block_n == 192) return launch_impl2<192>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
-  if (block_n == 128) return launch_impl2<128>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+  if (f16) {
+    if (p.nsplit != 1 || (block_n != 128 && block_n != 256)) {
+      set_last_error("launch_linear_pair: fp16 operands take one plane (nsplit 1) and block_n 128 or 256 (nsplit=%d block_n=%d)",
+                     p.nsplit, block_n);
+      return cudaErrorInvalidValue;
+    }
+    if (block_n == 256) return launch_impl2<256, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+    return launch_impl2<128, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+  }
+  if (block_n == 256) return launch_impl2<256, false>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+  if (block_n == 192) return launch_impl2<192, false>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+  if (block_n == 128) return launch_impl2<128, false>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
   set_last_error("launch_linear_pair: unsupported block_n %d", block_n);
   return cudaErrorInvalidValue;
 }

@@ -160,8 +160,11 @@ struct EpiStoreMaps {
 template <int BLOCK_N>
 __host__ __device__ constexpr int epi_part0_cols() { return (BLOCK_N == 192) ? 128 : BLOCK_N / 2; }
 
-// acc0 / acc1: the warpgroup's two m64 x PART_N accumulator halves of the interleaved 128-row tile
-template <int BLOCK_N, int PART_N>
+// acc0 / acc1: the warpgroup's two m64 x PART_N accumulator halves of the interleaved 128-row tile.
+// F16 (CMDI_PRECISION_FP16, CUDA autocast's arithmetic): the bias is rounded to fp16 like autocast's cast of it, the result
+// is rounded to fp16 before and after the activation (convolutions, num_taps > 0: also before the bias), out_f32 receives
+// those fp16 values as fp32 and out_hi one fp16 plane.
+template <int BLOCK_N, int PART_N, bool F16 = false>
 __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiStoreMaps& maps, const float (&acc0)[PART_N / 2],
                                               const float (&acc1)[PART_N / 2], int m_blk, int n_blk, int lane_group, int col_part,
                                               int lane, uint32_t stage) {
@@ -192,6 +195,7 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
   {
     const int nb = n_blk * BLOCK_N + col_start + lane * 4;
     if (p.bias && lane * 4 < part_cols && nb < p.N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + nb));
+    if constexpr (F16) bias4 = make_float4(round_f16(bias4.x), round_f16(bias4.y), round_f16(bias4.z), round_f16(bias4.w));
   }
 
   // residual re-derived from LayerNorm's input: gamma / beta of this warp's columns like the bias, and the
@@ -226,6 +230,13 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
     for (int j = 0; j < 32; ++j) {
       f[j] = __uint_as_float(v0[j]);
       f[32 + j] = __uint_as_float(v1[j]);
+    }
+    if constexpr (F16) {
+      // a convolution's bias is a separate fp16 add in PyTorch (cuDNN result + bias): the sum is rounded before it
+      if (p.num_taps > 0) {
+#pragma unroll
+        for (int j = 0; j < 64; ++j) f[j] = round_f16(f[j]);
+      }
     }
     if (p.bias) {
       // lane (c64*16 + g) holds the bias of columns [n0 + 4g, n0 + 4g + 4)
@@ -288,6 +299,10 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
       }
     }
     if (ncopies == 0) continue;
+    if constexpr (F16) {
+#pragma unroll
+      for (int j = 0; j < 64; ++j) f[j] = round_f16(f[j]);
+    }
     if (p.f32_pre && p.out_f32) {
       // stash the pre-activation value (fp32) before the activation is applied
       const long long dup = (long long)p.dup_row_offset * p.ld_f32 * 4;
@@ -315,6 +330,12 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
 #pragma unroll
       for (int j = 0; j < 64; ++j) f[j] = mish_f(f[j]);
     }
+    if constexpr (F16) {
+      if (p.act) {
+#pragma unroll
+        for (int j = 0; j < 64; ++j) f[j] = round_f16(f[j]);
+      }
+    }
     if (p.row_period && p.rowmap == ROWMAP_IDENTITY) {
       // halo rows between sequences: the value computed there is meaningless, the consumer relies on zeros
       const int rr = (warp_row0 + lane) % p.row_period;
@@ -336,11 +357,18 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
         }
       }
       if (p.out_hi) {
-        uint32_t hw[32], lw[32];
+        if constexpr (F16) {
+          uint32_t hw[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) split_bf16x2(f[2 * j], f[2 * j + 1], hw[j], lw[j]);
-        store_block_tma(stage, lane, hw, maps.hi, oc, warp_row0);
-        if (p.nsplit_out == 3) store_block_tma(stage, lane, lw, maps.lo, oc, warp_row0);
+          for (int j = 0; j < 32; ++j) hw[j] = pack_f16x2(f[2 * j], f[2 * j + 1]);
+          store_block_tma(stage, lane, hw, maps.hi, oc, warp_row0);
+        } else {
+          uint32_t hw[32], lw[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) split_bf16x2(f[2 * j], f[2 * j + 1], hw[j], lw[j]);
+          store_block_tma(stage, lane, hw, maps.hi, oc, warp_row0);
+          if (p.nsplit_out == 3) store_block_tma(stage, lane, lw, maps.lo, oc, warp_row0);
+        }
       }
       continue;
     }
@@ -360,16 +388,24 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
     }
     if (p.out_hi) {
       // one 64-column bf16 block per plane: 128 B per row
-      uint32_t hw[32], lw[32];
+      if constexpr (F16) {
+        uint32_t hw[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) split_bf16x2(f[2 * j], f[2 * j + 1], hw[j], lw[j]);
-      const long long dup = (long long)p.dup_row_offset * p.ld_bf * 2;
-      const int chunks = (p.N - n0) / 8;  // 16-byte chunks (8 bf16) still inside N
-      store_block_coalesced(stage, lane, hw, reinterpret_cast<char*>(p.out_hi + n0), rows, (long long)p.ld_bf * 2, chunks,
-                            ncopies, dup);
-      if (p.nsplit_out == 3)
-        store_block_coalesced(stage, lane, lw, reinterpret_cast<char*>(p.out_lo + n0), rows, (long long)p.ld_bf * 2,
-                              chunks, ncopies, dup);
+        for (int j = 0; j < 32; ++j) hw[j] = pack_f16x2(f[2 * j], f[2 * j + 1]);
+        store_block_coalesced(stage, lane, hw, reinterpret_cast<char*>(p.out_hi + n0), rows, (long long)p.ld_bf * 2,
+                              (p.N - n0) / 8, ncopies, (long long)p.dup_row_offset * p.ld_bf * 2);
+      } else {
+        uint32_t hw[32], lw[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) split_bf16x2(f[2 * j], f[2 * j + 1], hw[j], lw[j]);
+        const long long dup = (long long)p.dup_row_offset * p.ld_bf * 2;
+        const int chunks = (p.N - n0) / 8;  // 16-byte chunks (8 bf16) still inside N
+        store_block_coalesced(stage, lane, hw, reinterpret_cast<char*>(p.out_hi + n0), rows, (long long)p.ld_bf * 2, chunks,
+                              ncopies, dup);
+        if (p.nsplit_out == 3)
+          store_block_coalesced(stage, lane, lw, reinterpret_cast<char*>(p.out_lo + n0), rows, (long long)p.ld_bf * 2,
+                                chunks, ncopies, dup);
+      }
     }
   }
 }

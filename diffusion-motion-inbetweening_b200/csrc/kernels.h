@@ -97,7 +97,7 @@ struct LinearParams {
 cudaError_t configure_linear2_kernels();
 cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                                const CUtensorMap& w_lo, const LinearParams& p, int block_n, int num_sms,
-                               cudaStream_t stream, const LinearStoreMaps* st = nullptr);
+                               cudaStream_t stream, const LinearStoreMaps* st = nullptr, bool f16 = false);
 
 // A chain of linear layers in ONE persistent launch (gemm_chain.cu): the tiles of all phases form one list walked by
 // CTA pairs (one CTA per SM); a tile whose A rows are produced by an earlier phase of the same launch waits on a per-row-pair
@@ -296,10 +296,13 @@ struct UnetInputParams {
   int ld;                      // destination row pitch (elements, even)
   __nv_bfloat16* out_hi;
   __nv_bfloat16* out_lo;
+  int f16;                     // 1: out_hi receives one fp16 plane (CMDI_PRECISION_FP16), out_lo is unused
 };
 cudaError_t launch_unet_input(const UnetInputParams& p, cudaStream_t stream);
-// emb planes [num_seqs, 512]; TokenParams::seq_len carries B (conditioning row = seq % B), x_f32 is unused
-cudaError_t launch_unet_emb(const TokenParams& p, cudaStream_t stream);
+// emb planes [num_seqs, 512]; TokenParams::seq_len carries B (conditioning row = seq % B), x_f32 is unused.
+// f16: temb_table and cond_proj hold fp16 values, the sum is rounded to fp16 (autocast's `emb += embed_text(..)`) and
+// x_hi receives one fp16 plane
+cudaError_t launch_unet_emb(const TokenParams& p, cudaStream_t stream, bool f16 = false);
 struct GroupNormParams {
   int C, groups, L;            // channels, groups, positions per sequence
   int row_period, row_lo;      // halo layout (rows of sequence b: b * row_period + row_lo + l)
@@ -317,13 +320,23 @@ struct GroupNormParams {
   __nv_bfloat16* out_hi;       // planes [rows, ld_out] (pointer already offset to the first output column)
   __nv_bfloat16* out_lo;
   int ld_out;
+  // CMDI_PRECISION_FP16 (CUDA autocast): y and ada hold fp16 values, `1 + scale` is rounded to fp16, res_hi is one fp16
+  // plane (res_lo unused), out_hi receives one fp16 plane and out_f32 (if set) the fp32 value the next residual adds
+  int f16;
+  float* out_f32;
+  int ld_out_f32;
 };
 cudaError_t configure_groupnorm_kernel();
 cudaError_t launch_groupnorm_mish(const GroupNormParams& p, int num_seqs, cudaStream_t stream);
 // weight re-layouts: Conv1d [Co,Ci,k] -> tap-major planes [Co, k*Cp]; ConvTranspose1d(4,2,1) [Ci,Co,4] -> planes [2Co, 3Ci]
+// f16: one fp16 plane into `hi` (lo unused).  With k = 1, Cp = Ci the first is a plain [Co, Ci] matrix -> plane conversion.
 cudaError_t launch_conv_weight_planes(const float* w, int Co, int Ci, int k, int Cp, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld,
-                                      cudaStream_t stream);
-cudaError_t launch_convt_weight_planes(const float* w, int Ci, int Co, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld, cudaStream_t stream);
+                                      cudaStream_t stream, bool f16 = false);
+cudaError_t launch_convt_weight_planes(const float* w, int Ci, int Co, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld, cudaStream_t stream,
+                                       bool f16 = false);
+// out[r, n] = fp16(sum_k fp16(in[r, k]) fp16(W[n, k]) + fp16(bias[n])), fp32 accumulation: an autocast Linear on CUDA cores
+cudaError_t launch_small_linear_f16(const float* in, const float* W, const float* bias, float* out, int rows, int N, int K,
+                                    cudaStream_t stream);
 
 // ----------------------------------------------------------------------------------------------
 // backward pieces for reconstruction guidance      (backward.cu)

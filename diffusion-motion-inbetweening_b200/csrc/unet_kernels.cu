@@ -10,6 +10,9 @@
 //   unet_emb_kernel          emb = time_embed(pe[t]) (+ embed_text(cond))  mdm_unet.py:794-803
 //   groupnorm_mish_kernel    GroupNorm(8) -> [AdaGN scale/shift] -> Mish -> [+ residual]   mdm_unet.py:33-100, :159-218
 //   conv / conv-transpose weight re-layouts (once per weight load)
+//
+// Each kernel also has an F16 instantiation for CMDI_PRECISION_FP16, the arithmetic of CUDA autocast (fp16 planes in, fp16
+// planes out, GroupNorm / AdaGN / Mish in fp32 between them; DESIGN.md section 3).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -23,6 +26,7 @@ __device__ __forceinline__ float mish_dev(float x) { return x * tanhf(x > 20.0f 
 // network input: planes [rows0, ld] (hi, lo), channels [0, D) = keyframe-blended x_t, [D, 2D) = mask (keyframe-
 // conditioned models), zero elsewhere.  One thread per (sequence copy, frame, channel pair).
 // ---------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void __launch_bounds__(256) unet_input_kernel(const UnetInputParams p) {
   const int pairs = p.ld / 2;
   const size_t total = (size_t)p.B * p.L * pairs;
@@ -44,12 +48,13 @@ __global__ void __launch_bounds__(256) unet_input_kernel(const UnetInputParams p
       }
       v[j] = val;
     }
-    uint32_t hw, lw;
-    split_bf16x2(v[0], v[1], hw, lw);
+    uint32_t hw, lw = 0;
+    if constexpr (F16) hw = pack_f16x2(v[0], v[1]);  // the blend is fp32; the first conv casts its input to fp16
+    else split_bf16x2(v[0], v[1], hw, lw);
     for (int copy = 0; copy < p.copies; ++copy) {
       const size_t row = (size_t)(b + copy * p.B) * p.row_period + p.row_lo + l;
       *reinterpret_cast<uint32_t*>(p.out_hi + row * p.ld + cp * 2) = hw;
-      if (p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + row * p.ld + cp * 2) = lw;
+      if (!F16 && p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + row * p.ld + cp * 2) = lw;
     }
   }
 }
@@ -57,6 +62,7 @@ __global__ void __launch_bounds__(256) unet_input_kernel(const UnetInputParams p
 // ---------------------------------------------------------------------------------------------
 // emb[seq, :] = temb_table[tmap[t], :] + (cond_proj[seq % B] if seq < n_cond else uncond_proj)   -> bf16 planes [rows, 512]
 // ---------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void __launch_bounds__(128) unet_emb_kernel(const TokenParams p) {
   const int seq = blockIdx.x;
   int t = *p.step_ptr;
@@ -66,7 +72,17 @@ __global__ void __launch_bounds__(128) unet_emb_kernel(const TokenParams p) {
   if (p.cond_proj) {
     const float* c = (seq < p.n_cond_seqs) ? p.cond_proj + (size_t)(seq % p.seq_len) * 512 : p.uncond_proj;  // seq_len carries B here
     const float4 cv = *reinterpret_cast<const float4*>(c + col);
-    e.x += cv.x; e.y += cv.y; e.z += cv.z; e.w += cv.w;
+    if constexpr (F16) {
+      // fp16 + fp16 -> fp16; the unconditional row is embed_text(0) = the bias, cast to fp16
+      e.x = round_f16(e.x + round_f16(cv.x)); e.y = round_f16(e.y + round_f16(cv.y));
+      e.z = round_f16(e.z + round_f16(cv.z)); e.w = round_f16(e.w + round_f16(cv.w));
+    } else {
+      e.x += cv.x; e.y += cv.y; e.z += cv.z; e.w += cv.w;
+    }
+  }
+  if constexpr (F16) {
+    *reinterpret_cast<uint2*>(p.x_hi + (size_t)seq * 512 + col) = make_uint2(pack_f16x2(e.x, e.y), pack_f16x2(e.z, e.w));
+    return;
   }
   uint32_t h01, l01, h23, l23;
   split_bf16x2(e.x, e.y, h01, l01);
@@ -80,6 +96,7 @@ __global__ void __launch_bounds__(128) unet_emb_kernel(const TokenParams p) {
 // One CTA per (group, sequence): the [L, Cg] fp32 slab is staged in shared memory (<= 224 x 128 x 4 = 112 KB), the
 // statistics are two-pass over that copy (mean, then centred squares: torch's group_norm numerics to fp32 rounding).
 // ---------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void __launch_bounds__(512) groupnorm_mish_kernel(const GroupNormParams p) {
   extern __shared__ float slab[];  // [L][Cg]
   __shared__ float red[16];
@@ -128,15 +145,31 @@ __global__ void __launch_bounds__(512) groupnorm_mish_kernel(const GroupNormPara
       // cond = time_mlp(t) as [scale | shift] (mdm_unet.py:95-99): x * (1 + scale) + shift
       const float4 sc = *reinterpret_cast<const float4*>(p.ada + (size_t)b * p.ld_ada + c);
       const float4 sh = *reinterpret_cast<const float4*>(p.ada + (size_t)b * p.ld_ada + p.C + c);
-      o[0] = o[0] * (1.0f + sc.x) + sh.x; o[1] = o[1] * (1.0f + sc.y) + sh.y;
-      o[2] = o[2] * (1.0f + sc.z) + sh.z; o[3] = o[3] * (1.0f + sc.w) + sh.w;
+      if constexpr (F16) {
+        // scale / shift are fp16: `1 + scale` is an fp16 op, the product and sum with the fp32 GroupNorm output are fp32
+        o[0] = __fadd_rn(__fmul_rn(o[0], round_f16(1.0f + sc.x)), sh.x); o[1] = __fadd_rn(__fmul_rn(o[1], round_f16(1.0f + sc.y)), sh.y);
+        o[2] = __fadd_rn(__fmul_rn(o[2], round_f16(1.0f + sc.z)), sh.z); o[3] = __fadd_rn(__fmul_rn(o[3], round_f16(1.0f + sc.w)), sh.w);
+      } else {
+        o[0] = o[0] * (1.0f + sc.x) + sh.x; o[1] = o[1] * (1.0f + sc.y) + sh.y;
+        o[2] = o[2] * (1.0f + sc.z) + sh.z; o[3] = o[3] * (1.0f + sc.w) + sh.w;
+      }
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) o[j] = mish_dev(o[j]);
     const size_t row = row0 + l;
     if (p.res_f32) {
       const float4 r = *reinterpret_cast<const float4*>(p.res_f32 + row * p.ld_res + c);
-      o[0] += r.x; o[1] += r.y; o[2] += r.z; o[3] += r.w;
+      if constexpr (F16) {
+        o[0] = __fadd_rn(o[0], r.x); o[1] = __fadd_rn(o[1], r.y); o[2] = __fadd_rn(o[2], r.z); o[3] = __fadd_rn(o[3], r.w);
+      } else {
+        o[0] += r.x; o[1] += r.y; o[2] += r.z; o[3] += r.w;
+      }
+    } else if (F16 && p.res_hi) {
+      // an fp16 identity residual (a Downsample1d output): exact in fp32
+      const uint2 rh = *reinterpret_cast<const uint2*>(p.res_hi + row * p.ld_res + c);
+      const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&rh.x));
+      const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&rh.y));
+      o[0] = __fadd_rn(o[0], a.x); o[1] = __fadd_rn(o[1], a.y); o[2] = __fadd_rn(o[2], b.x); o[3] = __fadd_rn(o[3], b.y);
     } else if (p.res_hi) {
       const uint2 rh = *reinterpret_cast<const uint2*>(p.res_hi + row * p.ld_res + c);
       const uint2 rl = *reinterpret_cast<const uint2*>(p.res_lo + row * p.ld_res + c);
@@ -144,6 +177,11 @@ __global__ void __launch_bounds__(512) groupnorm_mish_kernel(const GroupNormPara
       o[1] += __uint_as_float(rh.x & 0xffff0000u) + __uint_as_float(rl.x & 0xffff0000u);
       o[2] += __uint_as_float(rh.y << 16) + __uint_as_float(rl.y << 16);
       o[3] += __uint_as_float(rh.y & 0xffff0000u) + __uint_as_float(rl.y & 0xffff0000u);
+    }
+    if constexpr (F16) {
+      *reinterpret_cast<uint2*>(p.out_hi + row * p.ld_out + c) = make_uint2(pack_f16x2(o[0], o[1]), pack_f16x2(o[2], o[3]));
+      if (p.out_f32) *reinterpret_cast<float4*>(p.out_f32 + row * p.ld_out_f32 + c) = make_float4(o[0], o[1], o[2], o[3]);
+      continue;
     }
     uint32_t h01, l01, h23, l23;
     split_bf16x2(o[0], o[1], h01, l01);
@@ -154,6 +192,7 @@ __global__ void __launch_bounds__(512) groupnorm_mish_kernel(const GroupNormPara
 }
 
 // Conv1d weight [Co, Ci, k] fp32 -> tap-major planes [Co, k * Cp] (Cp >= Ci, zero padded):  W2[o, j * Cp + c] = W[o, c, j]
+template <bool F16>
 __global__ void conv_weight_planes_kernel(const float* __restrict__ w, int Co, int Ci, int k, int Cp, __nv_bfloat16* hi,
                                           __nv_bfloat16* lo, int ld) {
   const size_t total = (size_t)Co * k * Cp;
@@ -162,6 +201,10 @@ __global__ void conv_weight_planes_kernel(const float* __restrict__ w, int Co, i
     const int j = (int)((i / Cp) % k);
     const int o = (int)(i / ((size_t)Cp * k));
     const float v = c < Ci ? w[((size_t)o * Ci + c) * k + j] : 0.f;
+    if constexpr (F16) {
+      reinterpret_cast<__half*>(hi)[(size_t)o * ld + (size_t)j * Cp + c] = __float2half_rn(v);
+      continue;
+    }
     __nv_bfloat16 h, l;
     split_bf16(v, h, l);
     hi[(size_t)o * ld + (size_t)j * Cp + c] = h;
@@ -172,6 +215,7 @@ __global__ void conv_weight_planes_kernel(const float* __restrict__ w, int Co, i
 // ConvTranspose1d(k = 4, s = 2, p = 1) weight [Ci, Co, 4] -> planes [2 Co, 3 Ci]: even outputs (rows [0, Co)) use
 // in[m - 1] W[..3] + in[m] W[..1], odd outputs (rows [Co, 2 Co)) use in[m] W[..2] + in[m + 1] W[..0]; tap blocks are
 // ordered (m - 1, m, m + 1) and the two unused blocks are zero.
+template <bool F16>
 __global__ void convt_weight_planes_kernel(const float* __restrict__ w, int Ci, int Co, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld) {
   const size_t total = (size_t)2 * Co * 3 * Ci;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -183,11 +227,32 @@ __global__ void convt_weight_planes_kernel(const float* __restrict__ w, int Ci, 
     if (!odd) j = tap == 0 ? 3 : (tap == 1 ? 1 : -1);
     else j = tap == 1 ? 2 : (tap == 2 ? 0 : -1);
     const float v = j >= 0 ? w[((size_t)c * Co + o) * 4 + j] : 0.f;
+    if constexpr (F16) {
+      reinterpret_cast<__half*>(hi)[(size_t)n * ld + (size_t)tap * Ci + c] = __float2half_rn(v);
+      continue;
+    }
     __nv_bfloat16 h, l;
     split_bf16(v, h, l);
     hi[(size_t)n * ld + (size_t)tap * Ci + c] = h;
     lo[(size_t)n * ld + (size_t)tap * Ci + c] = l;
   }
+}
+
+// autocast Linear on CUDA cores (embed_text, once per call): one warp per output element, K split across lanes
+__global__ void __launch_bounds__(256) small_linear_f16_kernel(const float* __restrict__ in, const float* __restrict__ W,
+                                                               const float* __restrict__ bias, float* __restrict__ out, int rows,
+                                                               int N, int K) {
+  const long long w = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (w >= (long long)rows * N) return;
+  const int r = (int)(w / N), n = (int)(w % N);
+  const float* a = in + (size_t)r * K;
+  const float* b = W + (size_t)n * K;
+  float s = 0.f;
+  for (int k = lane; k < K; k += 32) s = fmaf(round_f16(a[k]), round_f16(b[k]), s);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) out[(size_t)r * N + n] = round_f16(s + (bias ? round_f16(bias[n]) : 0.f));
 }
 
 inline dim3 grid_1d(size_t n, int block) {
@@ -200,17 +265,21 @@ inline dim3 grid_1d(size_t n, int block) {
 }  // namespace
 
 cudaError_t launch_unet_input(const UnetInputParams& p, cudaStream_t stream) {
-  unet_input_kernel<<<grid_1d((size_t)p.B * p.L * (p.ld / 2), 256), 256, 0, stream>>>(p);
+  if (p.f16) unet_input_kernel<true><<<grid_1d((size_t)p.B * p.L * (p.ld / 2), 256), 256, 0, stream>>>(p);
+  else unet_input_kernel<false><<<grid_1d((size_t)p.B * p.L * (p.ld / 2), 256), 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
-cudaError_t launch_unet_emb(const TokenParams& p, cudaStream_t stream) {
-  unet_emb_kernel<<<p.num_seqs, 128, 0, stream>>>(p);
+cudaError_t launch_unet_emb(const TokenParams& p, cudaStream_t stream, bool f16) {
+  if (f16) unet_emb_kernel<true><<<p.num_seqs, 128, 0, stream>>>(p);
+  else unet_emb_kernel<false><<<p.num_seqs, 128, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t configure_groupnorm_kernel() {
-  return cudaFuncSetAttribute(groupnorm_mish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 256 * 4);
+  const cudaError_t e = cudaFuncSetAttribute(groupnorm_mish_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 256 * 4);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(groupnorm_mish_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 256 * 4);
 }
 
 cudaError_t launch_groupnorm_mish(const GroupNormParams& p, int num_seqs, cudaStream_t stream) {
@@ -219,18 +288,29 @@ cudaError_t launch_groupnorm_mish(const GroupNormParams& p, int num_seqs, cudaSt
     set_last_error("launch_groupnorm_mish: unsupported shape C=%d groups=%d L=%d", p.C, p.groups, p.L);
     return cudaErrorInvalidValue;
   }
-  groupnorm_mish_kernel<<<dim3(p.groups, num_seqs), 512, (size_t)p.L * Cg * 4, stream>>>(p);
+  if (p.f16) groupnorm_mish_kernel<true><<<dim3(p.groups, num_seqs), 512, (size_t)p.L * Cg * 4, stream>>>(p);
+  else groupnorm_mish_kernel<false><<<dim3(p.groups, num_seqs), 512, (size_t)p.L * Cg * 4, stream>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_conv_weight_planes(const float* w, int Co, int Ci, int k, int Cp, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld,
-                                      cudaStream_t stream) {
-  conv_weight_planes_kernel<<<grid_1d((size_t)Co * k * Cp, 256), 256, 0, stream>>>(w, Co, Ci, k, Cp, hi, lo, ld);
+                                      cudaStream_t stream, bool f16) {
+  if (f16) conv_weight_planes_kernel<true><<<grid_1d((size_t)Co * k * Cp, 256), 256, 0, stream>>>(w, Co, Ci, k, Cp, hi, lo, ld);
+  else conv_weight_planes_kernel<false><<<grid_1d((size_t)Co * k * Cp, 256), 256, 0, stream>>>(w, Co, Ci, k, Cp, hi, lo, ld);
   return cudaGetLastError();
 }
 
-cudaError_t launch_convt_weight_planes(const float* w, int Ci, int Co, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld, cudaStream_t stream) {
-  convt_weight_planes_kernel<<<grid_1d((size_t)2 * Co * 3 * Ci, 256), 256, 0, stream>>>(w, Ci, Co, hi, lo, ld);
+cudaError_t launch_convt_weight_planes(const float* w, int Ci, int Co, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld, cudaStream_t stream,
+                                       bool f16) {
+  if (f16) convt_weight_planes_kernel<true><<<grid_1d((size_t)2 * Co * 3 * Ci, 256), 256, 0, stream>>>(w, Ci, Co, hi, lo, ld);
+  else convt_weight_planes_kernel<false><<<grid_1d((size_t)2 * Co * 3 * Ci, 256), 256, 0, stream>>>(w, Ci, Co, hi, lo, ld);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_small_linear_f16(const float* in, const float* W, const float* bias, float* out, int rows, int N, int K,
+                                    cudaStream_t stream) {
+  const long long warps = (long long)rows * N;
+  small_linear_f16_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(in, W, bias, out, rows, N, K);
   return cudaGetLastError();
 }
 

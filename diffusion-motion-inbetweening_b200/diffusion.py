@@ -112,6 +112,8 @@ class GaussianDiffusion:
         self.data_get_mean_fn = None
         self.log_trajectory_fn = None
         # engine options
+        # capi.PRECISION_FP16 (MDM_UNET only) samples with CUDA autocast's fp16 arithmetic, as the reference does for
+        # checkpoints with use_fp16; it is never chosen from conf.fp16 by itself
         self.precision = capi.PRECISION_BF16X3
         self.max_batch = None          # default: the batch of the first call
         self.noise_tape = None         # test aid: (1 + num_steps, B, njoints, 1, nframes) on the device

@@ -46,7 +46,10 @@ typedef struct cmdi_engine cmdi_engine;
 /* numerics of the tensor-core contractions */
 enum {
   CMDI_PRECISION_BF16X3 = 3, /* bf16 hi/lo operand split, 3 MMAs per product, fp32 accumulate: meets the fp32 parity gate */
-  CMDI_PRECISION_BF16 = 1    /* single bf16 MMA, fp32 accumulate: "fast" mode, does NOT meet rtol 1e-3 / atol 1e-4 */
+  CMDI_PRECISION_BF16 = 1,   /* single bf16 MMA, fp32 accumulate: "fast" mode, does NOT meet rtol 1e-3 / atol 1e-4 */
+  CMDI_PRECISION_FP16 = 2    /* "autocast", MDM_UNET only: what torch.autocast("cuda", float16) computes -- fp16 conv / linear
+                                operands and outputs (one MMA, fp32 accumulate), GroupNorm / AdaGN / Mish / residual sums in
+                                fp32 -- the arithmetic of checkpoints trained and sampled with use_fp16 */
 };
 
 /* PLMS: pseudo linear multistep (plms_sample_loop, gaussian_diffusion.py:1589-1804): deterministic, no per-step noise */
@@ -164,7 +167,8 @@ CMDI_API const char* cmdi_last_error(void);
 CMDI_API const char* cmdi_version(void);
 
 /* ---- kernel-level entry points (used by the parity tests; device pointers, fp32 row-major) ---- */
-/* C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ residual); block_n in {128, 256}: one CTA per tile; {-128, -256}: CTA-pair kernel */
+/* C[M,N] = act(A[M,K] W[N,K]^T + bias) (+ residual); block_n in {128, 256}: one CTA per tile; {-128, -256}: CTA-pair kernel.
+   precision: CMDI_PRECISION_*; with CMDI_PRECISION_FP16 A, W and bias are rounded to fp16 and C holds fp16 values */
 CMDI_API int cmdi_test_linear(const float* A, const float* W, const float* bias, const float* residual, float* C, int M, int N,
                      int K, int act, int precision, int block_n, void* stream);
 /* O = softmax(Q K^T / sqrt(128)) V for `num_seqs` sequences of length S and H heads; qkv: [num_seqs*S, 3*H*128] */
