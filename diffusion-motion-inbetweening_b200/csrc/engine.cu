@@ -708,10 +708,25 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
     set_last_error("precision CMDI_PRECISION_FP16 (autocast) is implemented for the MDM_UNET denoiser only (arch = CMDI_ARCH_UNET)");
     return 1;
   }
-  if (cfg->latent_dim != kDModel || cfg->njoints < 8 || cfg->max_batch < 1 ||
+  if (cfg->njoints < 8) {
+    // the frame rows are read and written 4 and 8 features at a time; the reference's traj_only models (4) are not served
+    set_last_error("njoints = %d is not supported: the engine needs njoints >= 8", cfg->njoints);
+    return 1;
+  }
+  if (cfg->nframes < 1 || (!is_unet && cfg->nframes + 1 > kAttnKeyPad)) {
+    // the attention kernel holds one sequence of nframes + 1 tokens in kAttnKeyPad key rows
+    set_last_error("nframes = %d is not supported: the transformer engine needs 1 <= nframes <= %d", cfg->nframes, kAttnKeyPad - 1);
+    return 1;
+  }
+  if (is_unet && cfg->nframes > kUnetFrames) {
+    // MDM_UNET right-pads its input to 224 frames (mdm_unet.py:820) and cannot take more
+    set_last_error("nframes = %d is not supported: the MDM_UNET engine needs 1 <= nframes <= %d", cfg->nframes, kUnetFrames);
+    return 1;
+  }
+  if (cfg->latent_dim != kDModel || cfg->max_batch < 1 ||
       (cfg->precision != CMDI_PRECISION_BF16X3 && cfg->precision != CMDI_PRECISION_BF16 && cfg->precision != CMDI_PRECISION_FP16) ||
-      (!is_unet && (cfg->num_heads * 128 != cfg->latent_dim || cfg->ff_size % 256 != 0 || cfg->nframes + 1 > kAttnKeyPad))) {
-    set_last_error("unsupported model configuration (need latent_dim=512, 4 heads of 128, ff %% 256 == 0, nframes <= 207)");
+      (!is_unet && (cfg->num_heads * 128 != cfg->latent_dim || cfg->ff_size % 256 != 0))) {
+    set_last_error("unsupported model configuration (need latent_dim=512, 4 heads of 128, ff %% 256 == 0, max_batch >= 1)");
     return 1;
   }
   CK(configure_linear2_kernels());

@@ -97,14 +97,16 @@ def build_reference_model(seed: int = 0, text: bool = False, layers: int = 8, la
     return model
 
 
-def build_reference_unet(dim_mults=(2, 2, 2, 2), latent_dim: int = 512, keyframe_conditioned: bool = True, text: bool = False):
-    """MDM_UNET as utils/model_util.py:30-32 builds it for configs/model.py `motion_unet_adagn_xl` (arch='unet', adagn, zero)."""
+def build_reference_unet(dim_mults=(2, 2, 2, 2), latent_dim: int = 512, keyframe_conditioned: bool = True, text: bool = False,
+                         njoints: int = 263, dataset: str = "humanml"):
+    """MDM_UNET as utils/model_util.py:30-32 builds it for configs/model.py `motion_unet_adagn_xl` (arch='unet', adagn, zero).
+    njoints / dataset as utils/model_util.py:62-76 sets them (263 humanml, 251 kit, 764 amass)."""
     import_reference()
     import model.mdm_unet as ref_unet  # noqa: E402
     with contextlib.redirect_stdout(open(os.devnull, "w")):
-        model = ref_unet.MDM_UNET(modeltype="", njoints=263, nfeats=1, num_actions=1, translation=True, pose_rep="rot6d", glob=True,
-                                  glob_rot=True, latent_dim=latent_dim, dim_mults=tuple(dim_mults), data_rep="hml_vec",
-                                  dataset="humanml", cond_mode="no_cond", cond_mask_prob=0.1, adagn=True, zero=True, arch="unet",
+        model = ref_unet.MDM_UNET(modeltype="", njoints=njoints, nfeats=1, num_actions=1, translation=True, pose_rep="rot6d",
+                                  glob=True, glob_rot=True, latent_dim=latent_dim, dim_mults=tuple(dim_mults), data_rep="hml_vec",
+                                  dataset=dataset, cond_mode="no_cond", cond_mask_prob=0.1, adagn=True, zero=True, arch="unet",
                                   keyframe_conditioned=keyframe_conditioned)
     if text:
         model.cond_mode = "text"
