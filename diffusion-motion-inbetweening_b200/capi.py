@@ -24,7 +24,7 @@ EXPORTS = [
     "cmdi_engine_create", "cmdi_engine_destroy", "cmdi_load_weights", "cmdi_set_schedule", "cmdi_model_forward",
     "cmdi_sample", "cmdi_launch_count", "cmdi_last_error", "cmdi_version", "cmdi_test_linear", "cmdi_test_attention",
     "cmdi_test_layernorm", "cmdi_test_step", "cmdi_test_normal", "cmdi_profile_pass", "cmdi_test_layernorm_bwd", "cmdi_test_attention_bwd",
-    "cmdi_test_normal_aten", "cmdi_recover_from_ric",
+    "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp",
 ]
 
 
@@ -102,6 +102,7 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
     lib.cmdi_profile_pass.argtypes = [c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, POINTER(c_int), c_void_p]
     lib.cmdi_test_layernorm_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]
     lib.cmdi_test_attention_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]
+    lib.cmdi_test_input_vjp.argtypes = [c_void_p, POINTER(ForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p]
     _lib = lib
     return lib
 

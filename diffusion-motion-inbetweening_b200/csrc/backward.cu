@@ -33,6 +33,7 @@ __device__ __forceinline__ float bf16_pair_to_f32(const __nv_bfloat16* hi, const
 // ---------------------------------------------------------------------------------------------
 // guidance seed on the frame-major layout [B*L (x2 when cfg), D_pad]
 // ---------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedParams p) {
   const size_t n = (size_t)p.B * p.L * p.D_pad;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -50,7 +51,14 @@ __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedPa
       const float m = p.obs_mask[i] ? 1.f : 0.f;
       const float G = -2.f * (p.x_obs[i] - hat) * m;  // d/dx0_hat of ((x_obs - x0_hat)^2 * M)
       gc = p.cfg ? s * G : G;
-      gu = (1.f - s) * G;
+      gu = F16 ? __fsub_rn(G, __fmul_rn(G, s)) : (1.f - s) * G;
+    }
+    if constexpr (F16) {
+      const int l = (int)((i / p.D_pad) % p.L);
+      __half* seed = reinterpret_cast<__half*>(p.seed_hi);
+      seed[((size_t)b * p.row_period + p.row_lo + l) * p.D_pad + c] = __float2half_rn(gc);
+      if (p.cfg) seed[((size_t)(b + p.B) * p.row_period + p.row_lo + l) * p.D_pad + c] = __float2half_rn(gu);
+      continue;
     }
     __nv_bfloat16 h, l;
     split_bf16(gc, h, l);
@@ -155,7 +163,8 @@ cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t strea
   const size_t n = (size_t)p.B * p.L * p.D_pad;
   size_t grid = (n + 255) / 256;
   if (grid > 132 * 16) grid = 132 * 16;
-  guidance_seed_kernel<<<(unsigned)grid, 256, 0, stream>>>(p);
+  if (p.f16) guidance_seed_kernel<true><<<(unsigned)grid, 256, 0, stream>>>(p);
+  else guidance_seed_kernel<false><<<(unsigned)grid, 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

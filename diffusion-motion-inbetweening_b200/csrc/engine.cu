@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <string>
 #include <vector>
@@ -45,6 +46,9 @@ namespace {
 constexpr int kDModel = 512;
 constexpr int kBnWide = 256;    // QKV, FFN1
 constexpr int kBnNarrow = 128;  // N = 512 / 264 outputs: more tiles per wave
+constexpr const char* kUnetGuidancePrecision =
+    "reconstruction guidance (the denoiser's input-VJP) is implemented for the transformer denoiser and, at "
+    "CMDI_PRECISION_FP16 (condmdi_b200.PRECISION_FP16), for MDM_UNET";
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
@@ -300,7 +304,7 @@ int run_denoiser_chain(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool ha
 // with dup the frame embedding is written for sequences [0,B) and [B,2B)).
 int run_denoiser(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool has_cond, const int* tmap_dev, cudaStream_t s,
                  std::vector<cudaEvent_t>* evs = nullptr, int reps = 1, std::vector<LayerStash>* stash = nullptr) {
-  if (e->unet) return unet_run(e, e->unet, B, dup, n_cond_seqs, has_cond, tmap_dev, s);
+  if (e->unet) return unet_run(e, e->unet, B, dup, n_cond_seqs, has_cond, tmap_dev, s, stash != nullptr);
   if (!stash && chain_eligible(e)) return run_denoiser_chain(e, B, dup, n_cond_seqs, has_cond, tmap_dev, s, evs, reps);
   auto mark = [&]() -> int {
     if (!evs) return 0;
@@ -561,7 +565,14 @@ int run_denoiser_chain(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool ha
   return 0;
 }
 
-int ensure_stash(cmdi_engine* e) {
+int ensure_stash(cmdi_engine* e, cudaStream_t s) {
+  if (e->unet) {
+    // MDM_UNET (fp16 only): its own stash and buffers; re-lays out the dgrad weights after a weight load
+    if (!e->guide_grad) CKI(dev_alloc(e, &e->guide_grad, (size_t)2 * e->frame_rows_pad * e->D_pad));
+    CKI(unet_guidance_init(e, e->unet, s));
+    e->stash_ready = true;
+    return 0;
+  }
   if (e->stash_ready) return 0;
   CK(configure_attention_bwd_tc_kernel());
   e->stash.resize(e->layers);
@@ -593,6 +604,7 @@ int ensure_stash(cmdi_engine* e) {
 // Scratch: xseq / x1 (fp32 + planes) carry the running gradients; qkv_p / attn_p / ffh_p the per-layer ones.
 constexpr int kBackwardLaunchesPerLayer = 8;  // the attention backward is two launches (dQ pass, dK/dV pass)
 int run_backward(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
+  if (e->unet) return unet_backward(e, e->unet, B, cfg, s);
   const int nseq = cfg ? 2 * B : B;
   const int M = nseq * e->S, MF = nseq * e->L;
   GuidanceSeedParams gp{};
@@ -651,6 +663,7 @@ int run_backward(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
   return 0;
 }
 int launches_per_backward(const cmdi_engine* e) {
+  if (e->unet) return unet_launches_per_backward(e->unet);
   return 3 + e->layers * kBackwardLaunchesPerLayer + 1;
 }
 
@@ -953,6 +966,7 @@ extern "C" int cmdi_load_weights(cmdi_engine* e, const cmdi_tensor_desc* tensors
   }
   if (by_name.count("sequence_pos_encoder.pe")) LOAD_F32(e->pe, "sequence_pos_encoder.pe", (size_t)5000 * kDModel);
   if (e->unet && !rc) rc = unet_load_weights(e, e->unet, by_name, missing, s);
+  if (e->unet) e->unet->dgrad_valid = false;  // the guidance's dgrad planes are re-laid out from the new weights
   for (int l = 0; l < e->layers; ++l) {
     LayerW& w = e->lw[l];
     const std::string p = "seqTransEncoder.layers." + std::to_string(l) + ".";
@@ -1209,8 +1223,8 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     set_last_error("imputate / reconstruction_guidance need inpainted_motion and inpainting_mask (editing_util.py:330, :343)");
     return 1;
   }
-  if (a->recon_guidance && e->unet) {
-    set_last_error("reconstruction guidance (the denoiser's input-VJP) is implemented for the transformer denoiser only");
+  if (a->recon_guidance && e->unet && !e->f16) {
+    set_last_error(kUnetGuidancePrecision);
     return 1;
   }
   if (a->recon_guidance) {
@@ -1218,7 +1232,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       set_last_error("reconstruction_guidance needs recon_coef");
       return 1;
     }
-    CKI(ensure_stash(e));
+    CKI(ensure_stash(e, s));
     if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
     CK(cudaMemcpyAsync(e->guide_coef, a->recon_coef, (size_t)e->T * 4, cudaMemcpyHostToDevice, s));
   }
@@ -1557,6 +1571,51 @@ extern "C" int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int
   CK(launch_diffusion_step(sp, s));
   CK(launch_frames_to_ref(e->x_state, B, e->D, e->L, e->D_pad, x_next, s));
   if (pred_xstart) CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, pred_xstart, s));
+  return 0;
+}
+
+// One (CFG: batch-doubled) evaluation of the guided pass and its input-VJP, as a guided sampling step runs them: the
+// seed dL/dx0_hat of sum((inpainted_motion - x0_hat)^2 * M) (M = inpainting_mask), then the backward pass.  grad receives
+// e->guide_grad in the reference layout: (cfg ? 2 : 1) x (B, njoints, 1, nframes), the cond pass's gradient w.r.t. x first.
+// Device pointers only.
+extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                   const uint8_t* inpainting_mask, float* grad, void* stream_) {
+  if (!e || !a || !a->x || !inpainted_motion || !inpainting_mask || !grad || a->host_buffers) {
+    set_last_error("cmdi_test_input_vjp: null argument or host buffers");
+    return 1;
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+  CK(cudaSetDevice(e->device));
+  const int B = a->batch;
+  CKI(check_ready(e, B, false));
+  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
+    set_last_error("cfg needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
+    return 1;
+  }
+  if (a->timestep < 0 || a->timestep >= 5000) {
+    set_last_error("timestep %d outside the positional table", a->timestep);
+    return 1;
+  }
+  if (e->unet && !e->f16) {
+    set_last_error(kUnetGuidancePrecision);
+    return 1;
+  }
+  CKI(ensure_temb(e, s));
+  CKI(ensure_stash(e, s));
+  const size_t n = (size_t)B * e->D * e->L;
+  CK(launch_ref_to_frames(a->x, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
+  CK(launch_ref_to_frames(inpainted_motion, B, e->D, e->L, e->D_pad, e->x_obs, nullptr, nullptr, s));
+  CK(launch_mask_to_frames(inpainting_mask, nullptr, B, e->D, e->L, e->D_pad, e->obs_mask, s));
+  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
+  CKI(prepare_cond(e, B, a->cond_emb, false, s));
+  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+  CK(launch_set_int(e->step_ctr, a->timestep, s));
+  CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
+  CKI(run_backward(e, B, a->cfg != 0, s));
+  const size_t fr = (size_t)B * e->L * e->D_pad;
+  for (int pass = 0; pass < (a->cfg ? 2 : 1); ++pass)
+    CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
+  e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 6;
   return 0;
 }
 

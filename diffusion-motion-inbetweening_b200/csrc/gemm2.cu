@@ -69,7 +69,7 @@ struct Producer {
   }
 };
 
-template <int BLOCK_N, int PART_N, bool F16>
+template <int BLOCK_N, int PART_N, bool F16, bool SUM32>
 __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const EpiStoreMaps& maps, Producer<BLOCK_N>& prod, bool is_producer,
                                                  int col_part, int lane_group, int lane, uint32_t epi_stage_addr) {
   constexpr int kPart0 = epi_part0_cols<BLOCK_N>();
@@ -96,7 +96,7 @@ __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const Ep
       if (is_producer) prod.issue_next();
       if (++stage == num_stages) { stage = 0; phase ^= 1; }
     }
-    epilogue_tile<BLOCK_N, PART_N, F16>(p, maps, acc0, acc1, m_blk, n_blk, lane_group, col_part, lane, epi_stage_addr);
+    epilogue_tile<BLOCK_N, PART_N, F16, SUM32>(p, maps, acc0, acc1, m_blk, n_blk, lane_group, col_part, lane, epi_stage_addr);
   }
 }
 
@@ -107,13 +107,11 @@ __device__ __forceinline__ void mma_and_epilogue(const LinearParams& p, const Ep
 // `num_stages` k-blocks ahead of the MMAs and across tile boundaries (the next tile's operands arrive under the epilogue).
 // Barriers: full[s] (1 arrival + the TMA transaction bytes), empty[s] (one arrival per warp once its wgmmas that read
 // stage s have completed).
-template <int BLOCK_N, bool F16>
-__global__ void __launch_bounds__(kNumThreads, 1)
-linear2_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-               const __grid_constant__ CUtensorMap map_o_hi, const __grid_constant__ CUtensorMap map_o_lo,
-               const __grid_constant__ CUtensorMap map_o_f32,
-               const LinearParams p, const int num_stages, const int num_m_blocks, const int num_n_blocks) {
+template <int BLOCK_N, bool F16, bool SUM32>
+__device__ __forceinline__ void linear2_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo, const CUtensorMap& map_w_hi,
+                                             const CUtensorMap& map_w_lo, const CUtensorMap& map_o_hi, const CUtensorMap& map_o_lo,
+                                             const CUtensorMap& map_o_f32, const LinearParams& p, const int num_stages,
+                                             const int num_m_blocks, const int num_n_blocks) {
   static_assert(BLOCK_N == 128 || BLOCK_N == 192 || BLOCK_N == 256, "BLOCK_N");
   constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   constexpr int kPart0 = epi_part0_cols<BLOCK_N>();
@@ -153,13 +151,37 @@ linear2_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const uint32_t epi_stage_addr = smem_u32(epi_stage + warp_idx * kEpiStageBytes);
   const EpiStoreMaps epi_maps{&map_o_hi, &map_o_lo, &map_o_f32};
   if (col_part == 0)
-    mma_and_epilogue<BLOCK_N, kPart0, F16>(p, epi_maps, prod, is_producer, col_part, lane_group, lane, epi_stage_addr);
+    mma_and_epilogue<BLOCK_N, kPart0, F16, SUM32>(p, epi_maps, prod, is_producer, col_part, lane_group, lane, epi_stage_addr);
   else
-    mma_and_epilogue<BLOCK_N, BLOCK_N - kPart0, F16>(p, epi_maps, prod, false, col_part, lane_group, lane, epi_stage_addr);
+    mma_and_epilogue<BLOCK_N, BLOCK_N - kPart0, F16, SUM32>(p, epi_maps, prod, false, col_part, lane_group, lane, epi_stage_addr);
   if (p.tma_store && lane == 0) tma_store_wait_all();
 }
 
 template <int BLOCK_N, bool F16>
+__global__ void __launch_bounds__(kNumThreads, 1)
+linear2_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+               const __grid_constant__ CUtensorMap map_o_hi, const __grid_constant__ CUtensorMap map_o_lo,
+               const __grid_constant__ CUtensorMap map_o_f32,
+               const LinearParams p, const int num_stages, const int num_m_blocks, const int num_n_blocks) {
+  linear2_body<BLOCK_N, F16, false>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, map_o_hi, map_o_lo, map_o_f32, p, num_stages, num_m_blocks,
+                                    num_n_blocks);
+}
+
+// fp16 operands whose fp16-rounded sum gets an fp32 residual added without a second rounding (epilogue_tile, SUM32): the
+// gradient sums of the UNet's input-VJP.  A kernel of its own, so that linear2_kernel's code is what it was.
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kNumThreads, 1)
+linear2_f16_sum32_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                         const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                         const __grid_constant__ CUtensorMap map_o_hi, const __grid_constant__ CUtensorMap map_o_lo,
+                         const __grid_constant__ CUtensorMap map_o_f32,
+                         const LinearParams p, const int num_stages, const int num_m_blocks, const int num_n_blocks) {
+  linear2_body<BLOCK_N, true, true>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, map_o_hi, map_o_lo, map_o_f32, p, num_stages, num_m_blocks,
+                                    num_n_blocks);
+}
+
+template <int BLOCK_N, bool F16, bool SUM32 = false>
 cudaError_t launch_impl2(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi, const CUtensorMap& w_lo,
                          const LinearParams& p_in, int num_sms, cudaStream_t stream, const LinearStoreMaps* st) {
   LinearParams p = p_in;
@@ -184,6 +206,9 @@ cudaError_t launch_impl2(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const
   int num_stages = (kSmemLimit - fixed) / stage_bytes;
   if (num_stages > kMaxStages) num_stages = kMaxStages;
   const size_t smem = (size_t)fixed + (size_t)num_stages * stage_bytes;
+  if constexpr (SUM32)
+    return launch_kernel(linear2_f16_sum32_kernel<BLOCK_N>, dim3(ctas), dim3(kNumThreads), smem, stream, a_hi, a_lo, w_hi, w_lo,
+                         o_hi, o_lo, o_f32, p, num_stages, num_m_blocks, num_n_blocks);
   return launch_kernel(linear2_kernel<BLOCK_N, F16>, dim3(ctas), dim3(kNumThreads), smem, stream, a_hi, a_lo, w_hi, w_lo,
                        o_hi, o_lo, o_f32, p, num_stages, num_m_blocks, num_n_blocks);
 }
@@ -197,15 +222,20 @@ cudaError_t configure_linear2_kernels() {
   };
   set(linear2_kernel<128, false>); set(linear2_kernel<192, false>); set(linear2_kernel<256, false>);
   set(linear2_kernel<128, true>); set(linear2_kernel<256, true>);
+  set(linear2_f16_sum32_kernel<128>); set(linear2_f16_sum32_kernel<256>);
   return e;
 }
 
 // Tensor maps: A box {64, 128}; W box {64, block_n / 2}.
 cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi, const CUtensorMap& w_lo,
                                const LinearParams& p, int block_n, int num_sms, cudaStream_t stream,
-                               const LinearStoreMaps* st, bool f16) {
+                               const LinearStoreMaps* st, bool f16, bool sum32) {
   if (p.N % 8 != 0 || (p.nsplit != 1 && p.nsplit != 3)) {
     set_last_error("launch_linear_pair: N must be a multiple of 8 and nsplit 1 or 3 (N=%d nsplit=%d)", p.N, p.nsplit);
+    return cudaErrorInvalidValue;
+  }
+  if (sum32 && !f16) {
+    set_last_error("launch_linear_pair: the fp32 residual sum exists for fp16 operands only");
     return cudaErrorInvalidValue;
   }
   if (f16) {
@@ -213,6 +243,10 @@ cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo,
       set_last_error("launch_linear_pair: fp16 operands take one plane (nsplit 1) and block_n 128 or 256 (nsplit=%d block_n=%d)",
                      p.nsplit, block_n);
       return cudaErrorInvalidValue;
+    }
+    if (sum32) {
+      if (block_n == 256) return launch_impl2<256, true, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
+      return launch_impl2<128, true, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
     }
     if (block_n == 256) return launch_impl2<256, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);
     return launch_impl2<128, true>(a_hi, a_lo, w_hi, w_lo, p, num_sms, stream, st);

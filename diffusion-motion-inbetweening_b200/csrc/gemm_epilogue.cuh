@@ -164,7 +164,10 @@ __host__ __device__ constexpr int epi_part0_cols() { return (BLOCK_N == 192) ? 1
 // F16 (CMDI_PRECISION_FP16, CUDA autocast's arithmetic): the bias is rounded to fp16 like autocast's cast of it, the result
 // is rounded to fp16 before and after the activation (convolutions, num_taps > 0: also before the bias), out_f32 receives
 // those fp16 values as fp32 and out_hi one fp16 plane.
-template <int BLOCK_N, int PART_N, bool F16 = false>
+// SUM32 (with F16; the UNet's input-VJP, where autograd adds an fp16 convolution gradient into an fp32 gradient): the
+// residual is added to the fp16-rounded sum in fp32 and the result is NOT rounded again: out_f32 receives the fp32 sum,
+// out_hi its fp16 rounding.
+template <int BLOCK_N, int PART_N, bool F16 = false, bool SUM32 = false>
 __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiStoreMaps& maps, const float (&acc0)[PART_N / 2],
                                               const float (&acc1)[PART_N / 2], int m_blk, int n_blk, int lane_group, int col_part,
                                               int lane, uint32_t stage) {
@@ -299,7 +302,7 @@ __device__ __forceinline__ void epilogue_tile(const LinearParams& p, const EpiSt
       }
     }
     if (ncopies == 0) continue;
-    if constexpr (F16) {
+    if constexpr (F16 && !SUM32) {
 #pragma unroll
       for (int j = 0; j < 64; ++j) f[j] = round_f16(f[j]);
     }

@@ -97,7 +97,8 @@ struct LinearParams {
 cudaError_t configure_linear2_kernels();
 cudaError_t launch_linear_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                                const CUtensorMap& w_lo, const LinearParams& p, int block_n, int num_sms,
-                               cudaStream_t stream, const LinearStoreMaps* st = nullptr, bool f16 = false);
+                               cudaStream_t stream, const LinearStoreMaps* st = nullptr, bool f16 = false,
+                               bool sum32 = false);  // sum32 (fp16 only): epilogue_tile's SUM32 (gemm_epilogue.cuh)
 
 // A chain of linear layers in ONE persistent launch (gemm_chain.cu): the tiles of all phases form one list walked by
 // CTA pairs (one CTA per SM); a tile whose A rows are produced by an earlier phase of the same launch waits on a per-row-pair
@@ -338,6 +339,51 @@ cudaError_t launch_convt_weight_planes(const float* w, int Ci, int Co, __nv_bflo
 cudaError_t launch_small_linear_f16(const float* in, const float* W, const float* bias, float* out, int rows, int N, int K,
                                     cudaStream_t stream);
 
+// ---- the UNet's input-VJP at CMDI_PRECISION_FP16 (reconstruction guidance; the arithmetic of autograd after an autocast
+//      forward, DESIGN.md section 6) ----
+// Backward of GroupNorm -> [AdaGN] -> Mish for one groupnorm_mish launch: dY = GroupNorm'(AdaGN'(Mish'(dO))), recomputed from
+// the stashed convolution output y, in fp32, rounded to fp16 (autograd's cast back into the fp16 convolution output).  dy
+// is written in the halo layout, the halo rows of every sequence as zeros.
+struct GroupNormBwdParams {
+  int C, groups, L;
+  int row_period, row_lo;
+  float eps;
+  const __nv_bfloat16* y;      // fp16 plane [rows, ld_y]: the forward's GroupNorm input (stash)
+  int ld_y;
+  const float* gamma;
+  const float* beta;
+  const float* ada;            // as GroupNormParams::ada (fp16 values), or null
+  int ld_ada;
+  float* dout;                 // fp32 gradient of the Mish output [rows, ld_dout] ...
+  const __nv_bfloat16* dout_h; // ... or an fp16 plane of it
+  int ld_dout;
+  const float* dout_add;       // or null: fp32 [rows, ld_add] added to dout first, the sum written back into dout
+  int ld_add;
+  __nv_bfloat16* dy;           // fp16 plane [rows, ld_dy]
+  int ld_dy;
+};
+cudaError_t configure_groupnorm_bwd_kernel();
+cudaError_t launch_groupnorm_mish_bwd(const GroupNormBwdParams& p, int num_seqs, cudaStream_t stream);
+// dgrad weight planes (fp16) re-laid out from the forward's fp16 planes (launch_conv_weight_planes /
+// launch_convt_weight_planes layouts); dst [N, taps * Kp], tap t's block at columns t * Kp:
+//   kind 0, Conv1d(k):  dst[n, j*Kp + o] = W[o, n, j]               (src [Co, k*Cp]; n < Ci, o < Co valid)
+//   kind 1, Downsample1d (k=3, s=2): N = 2C (even | odd input positions), taps (q, q+1) of the output gradient:
+//           even: [W1^T | 0], odd: [W2^T | W0^T]                    (src [C, 3*Cp])
+//   kind 2, Upsample1d (ConvTranspose k=4, s=2, p=1): dst[n, j*Kp + o] = W[n, o, j], 4 taps  (src: the [2C, 3C] phase planes)
+struct DgradWeightParams {
+  int kind;
+  const __nv_bfloat16* src;
+  int ld_src, Cp_src;
+  int Ci, Co;          // kind 0: the forward's input / output channels (valid extents); kinds 1, 2: Ci = Co = C
+  __nv_bfloat16* dst;
+  int ld_dst, N, taps, Kp;
+};
+cudaError_t launch_dgrad_weight_planes(const DgradWeightParams& p, cudaStream_t stream);
+// guide_grad[(seq*L + l), c] = xg[seq*row_period + row_lo + l, c] * !obs_mask[(seq % B)*L + l, c] for c < D (0 for
+// D <= c < D_pad; obs_mask null: no keyframe input blend): the gradient of the network input's x_t channels
+cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int B, int L, int D, int D_pad, int row_period, int row_lo,
+                                   const uint8_t* obs_mask, float* out, cudaStream_t stream);
+
 // ----------------------------------------------------------------------------------------------
 // backward pieces for reconstruction guidance      (backward.cu)
 // ----------------------------------------------------------------------------------------------
@@ -349,6 +395,10 @@ struct GuidanceSeedParams {
   const uint8_t* obs_mask;   // [B*L, D_pad]
   __nv_bfloat16* seed_hi;    // [B*L (x2), D_pad] dL/d(model output rows)
   __nv_bfloat16* seed_lo;
+  // f16 (MDM_UNET at CMDI_PRECISION_FP16): seed_hi is one fp16 plane [rows, D_pad] in the UNet's halo layout (frame l of
+  // sequence q at row q * row_period + row_lo + l; other rows untouched), the seeds rounded to fp16 like autograd's cast
+  // at the output's `.float()`; the uncond seed is G - s G, the sum autograd forms
+  int f16, row_period, row_lo;
 };
 cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t stream);
 cudaError_t launch_layernorm512_bwd(const float* dy, const float* v, const float* gamma, float eps, int rows, float* dv,

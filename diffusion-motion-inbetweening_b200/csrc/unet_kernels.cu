@@ -255,6 +255,173 @@ __global__ void __launch_bounds__(256) small_linear_f16_kernel(const float* __re
   if (lane == 0) out[(size_t)r * N + n] = round_f16(s + (bias ? round_f16(bias[n]) : 0.f));
 }
 
+// ---------------------------------------------------------------------------------------------
+// Input-VJP (CMDI_PRECISION_FP16 reconstruction guidance): the backward of one groupnorm_mish launch.  Same CTA shape as
+// the forward: the stashed [L, Cg] slab in shared memory, the same two-pass statistics, then with
+//   xhat = (y - mean) rstd,  a = xhat gamma + beta,  b = a fp16(1 + scale) + shift (AdaGN) or a,  o = Mish(b):
+//   g = dO Mish'(b) [fp16(1 + scale)] gamma,  dY = rstd (g - mean(g) - xhat mean(g xhat))     (fp32; dY rounded to fp16)
+// Mish' as PyTorch's mish_backward: tanh(softplus(b)) + b sigmoid(b) (1 - tanh(softplus(b))^2).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float mish_grad_dev(float x) {
+  const float sg = 1.0f / (1.0f + expf(-x));
+  const float ts = tanhf(log1pf(expf(x)));
+  return ts + x * sg * (1.0f - ts * ts);
+}
+
+__global__ void __launch_bounds__(512) groupnorm_mish_bwd_kernel(const GroupNormBwdParams p) {
+  extern __shared__ float slab[];  // [L][Cg]
+  __shared__ float red[16];
+  const int g = blockIdx.x, b = blockIdx.y;
+  const int Cg = p.C / p.groups, L = p.L;
+  const int c0 = g * Cg;
+  const size_t seq0 = (size_t)b * p.row_period;
+  const size_t row0 = seq0 + p.row_lo;
+  const int vec = Cg / 4;
+  const int n4 = L * vec;
+  auto ld_h4 = [](const __nv_bfloat16* base, size_t off) -> float4 {
+    const uint2 h = *reinterpret_cast<const uint2*>(base + off);
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&h.x));
+    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+    return make_float4(a.x, a.y, c.x, c.y);
+  };
+  float sum = 0.f;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+    const int l = i / vec, q = i - l * vec;
+    const float4 v = ld_h4(p.y, (row0 + l) * p.ld_y + c0 + q * 4);
+    reinterpret_cast<float4*>(slab)[i] = v;
+    sum += (v.x + v.y) + (v.z + v.w);
+  }
+  auto block_sum = [&](float v) -> float {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
+    return t;
+  };
+  const float inv_n = 1.0f / (float)(L * Cg);
+  const float mean = block_sum(sum) * inv_n;
+  float sq = 0.f;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+    const float4 v = reinterpret_cast<float4*>(slab)[i];
+    const float a = v.x - mean, bb = v.y - mean, c = v.z - mean, d = v.w - mean;
+    sq += (a * a + bb * bb) + (c * c + d * d);
+  }
+  const float rstd = rsqrtf(block_sum(sq) * inv_n + p.eps);
+  // g and xhat of element j of slab entry i (pass 1 also folds dout_add into dout)
+  auto grad_of = [&](int i, bool first, float (&gg)[4], float (&xh)[4]) {
+    const int l = i / vec, q = i - l * vec;
+    const int c = c0 + q * 4;
+    const size_t row = row0 + l;
+    const float4 v = reinterpret_cast<float4*>(slab)[i];
+    const float4 gm = *reinterpret_cast<const float4*>(p.gamma + c);
+    const float4 bt = *reinterpret_cast<const float4*>(p.beta + c);
+    float4 d4;
+    if (p.dout_h) {
+      d4 = ld_h4(p.dout_h, row * p.ld_dout + c);
+    } else {
+      d4 = *reinterpret_cast<const float4*>(p.dout + row * p.ld_dout + c);
+      if (first && p.dout_add) {
+        const float4 a4 = *reinterpret_cast<const float4*>(p.dout_add + row * p.ld_add + c);
+        d4 = make_float4(__fadd_rn(d4.x, a4.x), __fadd_rn(d4.y, a4.y), __fadd_rn(d4.z, a4.z), __fadd_rn(d4.w, a4.w));
+        *reinterpret_cast<float4*>(p.dout + row * p.ld_dout + c) = d4;
+      }
+    }
+    const float vv[4] = {v.x, v.y, v.z, v.w}, gmv[4] = {gm.x, gm.y, gm.z, gm.w}, btv[4] = {bt.x, bt.y, bt.z, bt.w};
+    const float dv[4] = {d4.x, d4.y, d4.z, d4.w};
+    float s1[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
+    if (p.ada) {
+      const float4 sc = *reinterpret_cast<const float4*>(p.ada + (size_t)b * p.ld_ada + c);
+      const float4 sf = *reinterpret_cast<const float4*>(p.ada + (size_t)b * p.ld_ada + p.C + c);
+      s1[0] = round_f16(1.0f + sc.x); s1[1] = round_f16(1.0f + sc.y); s1[2] = round_f16(1.0f + sc.z); s1[3] = round_f16(1.0f + sc.w);
+      sh[0] = sf.x; sh[1] = sf.y; sh[2] = sf.z; sh[3] = sf.w;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      xh[j] = (vv[j] - mean) * rstd;
+      const float a = (vv[j] - mean) * rstd * gmv[j] + btv[j];  // the forward's expression
+      const float bv = p.ada ? __fadd_rn(__fmul_rn(a, s1[j]), sh[j]) : a;
+      float t = dv[j] * mish_grad_dev(bv);
+      if (p.ada) t = t * s1[j];
+      gg[j] = t * gmv[j];
+    }
+  };
+  float m1 = 0.f, m2 = 0.f;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+    float gg[4], xh[4];
+    grad_of(i, true, gg, xh);
+    m1 += (gg[0] + gg[1]) + (gg[2] + gg[3]);
+    m2 += (gg[0] * xh[0] + gg[1] * xh[1]) + (gg[2] * xh[2] + gg[3] * xh[3]);
+  }
+  m1 = block_sum(m1) * inv_n;  // (block_sum's barriers also order pass 1's dout write-back before pass 2's reads)
+  m2 = block_sum(m2) * inv_n;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+    float gg[4], xh[4];
+    grad_of(i, false, gg, xh);
+    float o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[j] = rstd * (gg[j] - m1 - xh[j] * m2);
+    const int l = i / vec, q = i - l * vec;
+    *reinterpret_cast<uint2*>(p.dy + (row0 + l) * p.ld_dy + c0 + q * 4) = make_uint2(pack_f16x2(o[0], o[1]), pack_f16x2(o[2], o[3]));
+  }
+  // the halo rows of this sequence (the next convolution's zero padding)
+  const int halo = (p.row_period - L) * vec;
+  for (int i = threadIdx.x; i < halo; i += blockDim.x) {
+    const int h = i / vec, q = i - h * vec;
+    const int r = h < p.row_lo ? h : L + h;
+    *reinterpret_cast<uint2*>(p.dy + (seq0 + r) * p.ld_dy + c0 + q * 4) = make_uint2(0u, 0u);
+  }
+}
+
+__global__ void dgrad_weight_planes_kernel(const DgradWeightParams p) {
+  const size_t total = (size_t)p.N * p.taps * p.Kp;
+  const __half* src = reinterpret_cast<const __half*>(p.src);
+  __half* dst = reinterpret_cast<__half*>(p.dst);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % p.Kp);
+    const int t = (int)((i / p.Kp) % p.taps);
+    const int n = (int)(i / ((size_t)p.Kp * p.taps));
+    __half v = __float2half_rn(0.f);
+    if (p.kind == 0) {
+      if (n < p.Ci && k < p.Co) v = src[(size_t)k * p.ld_src + (size_t)t * p.Cp_src + n];
+    } else if (p.kind == 1) {
+      const int C = p.Ci, ci = n % C, odd = n / C;
+      // even input positions 2q: W1^T dOut[q]; odd 2q + 1: W2^T dOut[q] + W0^T dOut[q + 1]
+      const int j = odd ? (t == 0 ? 2 : 0) : (t == 0 ? 1 : -1);
+      if (j >= 0 && k < C) v = src[(size_t)k * p.ld_src + (size_t)j * p.Cp_src + ci];
+    } else {
+      // the forward's phase planes hold W[c, o, 3], W[c, o, 1] in row o (taps 0, 1) and W[c, o, 2], W[c, o, 0] in row C + o
+      // (taps 1, 2)
+      const int C = p.Ci, c = n, o = k;
+      if (c < C && o < C) {
+        const size_t even = (size_t)o * p.ld_src, odd = (size_t)(C + o) * p.ld_src;
+        const size_t at[4] = {odd + 2 * (size_t)C + c, even + (size_t)C + c, odd + (size_t)C + c, even + c};
+        v = src[at[t]];
+      }
+    }
+    dst[(size_t)n * p.ld_dst + (size_t)t * p.Kp + k] = v;
+  }
+}
+
+__global__ void __launch_bounds__(256) unet_input_grad_kernel(const float* __restrict__ xg, int ld, int num_seqs, int B, int L, int D,
+                                                              int D_pad, int row_period, int row_lo, const uint8_t* __restrict__ obs_mask,
+                                                              float* __restrict__ out) {
+  const size_t total = (size_t)num_seqs * L * D_pad;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % D_pad);
+    const size_t fl = i / D_pad;
+    const int l = (int)(fl % L), q = (int)(fl / L);
+    float v = 0.f;
+    if (c < D) {
+      v = xg[((size_t)q * row_period + row_lo + l) * ld + c];
+      if (obs_mask && obs_mask[((size_t)(q % B) * L + l) * D_pad + c]) v = 0.f;  // x = obs_x0 M + x ~M (mdm_unet.py:781)
+    }
+    out[i] = v;
+  }
+}
+
 inline dim3 grid_1d(size_t n, int block) {
   size_t g = (n + block - 1) / block;
   if (g > 132 * 32) g = 132 * 32;
@@ -311,6 +478,33 @@ cudaError_t launch_small_linear_f16(const float* in, const float* W, const float
                                     cudaStream_t stream) {
   const long long warps = (long long)rows * N;
   small_linear_f16_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(in, W, bias, out, rows, N, K);
+  return cudaGetLastError();
+}
+
+cudaError_t configure_groupnorm_bwd_kernel() {
+  return cudaFuncSetAttribute(groupnorm_mish_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 256 * 4);
+}
+
+cudaError_t launch_groupnorm_mish_bwd(const GroupNormBwdParams& p, int num_seqs, cudaStream_t stream) {
+  const int Cg = p.C / p.groups;
+  if (p.C % p.groups || Cg % 4 || (size_t)p.L * Cg * 4 > 224 * 256 * 4 || (p.dout == nullptr) == (p.dout_h == nullptr) ||
+      (p.dout_add && !p.dout)) {
+    set_last_error("launch_groupnorm_mish_bwd: unsupported shape C=%d groups=%d L=%d or gradient inputs", p.C, p.groups, p.L);
+    return cudaErrorInvalidValue;
+  }
+  groupnorm_mish_bwd_kernel<<<dim3(p.groups, num_seqs), 512, (size_t)p.L * Cg * 4, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_dgrad_weight_planes(const DgradWeightParams& p, cudaStream_t stream) {
+  dgrad_weight_planes_kernel<<<grid_1d((size_t)p.N * p.taps * p.Kp, 256), 256, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int B, int L, int D, int D_pad, int row_period, int row_lo,
+                                   const uint8_t* obs_mask, float* out, cudaStream_t stream) {
+  unet_input_grad_kernel<<<grid_1d((size_t)num_seqs * L * D_pad, 256), 256, 0, stream>>>(xg, ld, num_seqs, B, L, D, D_pad, row_period,
+                                                                                        row_lo, obs_mask, out);
   return cudaGetLastError();
 }
 

@@ -239,3 +239,20 @@ class Engine:
                                                _ptr(mask), x_next.data_ptr(), pred.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_test_step")
         return x_next, pred
+
+    def test_input_vjp(self, x, timestep, inpainted_motion, inpainting_mask, cond_emb=None, uncond=False, cfg=False,
+                       text_scale=None, obs_x0=None, obs_mask=None) -> torch.Tensor:
+        """One guided evaluation and its input-VJP (cmdi_test_input_vjp): (cfg ? 2 : 1, B, njoints, 1, nframes), the
+        gradient of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) w.r.t. x through each pass, cond pass first."""
+        dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
+        x = dev(x)
+        B = x.shape[0]
+        cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
+        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
+        grad = torch.empty((2 if cfg else 1,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
+                             _ptr(obs_x0), _ptr(obs_mask))
+        with torch.cuda.device(self.device):
+            capi.check(self.lib.cmdi_test_input_vjp(self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask),
+                                                    grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_input_vjp")
+        return grad

@@ -179,6 +179,11 @@ CMDI_API int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B
                    const float* text_scale, const float* x_t, const float* noise, int impute, int stop_imputation_at,
                    const float* x_obs, const uint8_t* mask, float* x_next, float* pred_xstart, void* stream);
 
+/* one guided evaluation (args as cmdi_model_forward, device pointers) and its input-VJP, as a reconstruction-guided step runs
+ * them: grad receives d/dx of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) through each pass, (cfg ? 2 : 1) x
+ * (B, njoints, 1, nframes), the cond pass first (the sampler adds the two and masks them).  MDM_UNET: CMDI_PRECISION_FP16 only */
+CMDI_API int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
+                        const uint8_t* inpainting_mask, float* grad, void* stream);
 /* backward pieces of reconstruction guidance (fp32 in / out) */
 CMDI_API int cmdi_test_layernorm_bwd(const float* dy, const float* v, const float* gamma, float* dv, int rows, void* stream);
 CMDI_API int cmdi_test_attention_bwd(const float* qkv, const float* dO, float* dqkv, int num_seqs, int S, int H, void* stream);
