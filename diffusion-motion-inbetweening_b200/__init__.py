@@ -16,4 +16,4 @@ from .eval_loop import EvalJob, build_jobs, run_eval_jobs  # noqa: F401
 from .capi import PRECISION_BF16, PRECISION_BF16X3, PRECISION_FP16  # noqa: F401
 
 __version__ = "0.1.0"
-from .motion_process import recover_from_ric, sample_to_joints  # noqa: F401
+from .motion_process import abs3d_to_rel, joints_to_features, recover_from_ric, rel_to_abs3d, sample_to_joints  # noqa: F401

@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcondmdi_b200.so")
-SOURCES = ["gemm2.cu", "gemm_chain.cu", "attention.cu", "elementwise.cu", "unet_kernels.cu", "backward.cu", "attention_bwd_tc.cu", "attention_bwd_simt_test.cu", "tma_host.cu", "capi_test.cu", "engine.cu"]
+SOURCES = ["gemm2.cu", "gemm_chain.cu", "attention.cu", "elementwise.cu", "unet_kernels.cu", "backward.cu", "attention_bwd_tc.cu", "attention_bwd_simt_test.cu", "tma_host.cu", "capi_test.cu", "motion_features.cu", "engine.cu"]
 HEADERS = ["common.cuh", "kernels.h", "gemm_epilogue.cuh", "engine_unet.inc", os.path.join("..", "..", "include", "condmdi_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]

@@ -19,12 +19,13 @@ SAMPLER_DDPM = 0
 SAMPLER_DDIM = 1
 SAMPLER_PLMS = 2
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
+MOTION_ABS3D_TO_REL, MOTION_REL_TO_ABS3D, MOTION_REL_TO_JOINTS, MOTION_ABS3D_TO_JOINTS = 0, 1, 2, 3
 
 EXPORTS = [
     "cmdi_engine_create", "cmdi_engine_destroy", "cmdi_load_weights", "cmdi_set_schedule", "cmdi_model_forward",
     "cmdi_sample", "cmdi_launch_count", "cmdi_last_error", "cmdi_version", "cmdi_test_linear", "cmdi_test_attention",
     "cmdi_test_layernorm", "cmdi_test_step", "cmdi_test_normal", "cmdi_profile_pass", "cmdi_test_layernorm_bwd", "cmdi_test_attention_bwd",
-    "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp",
+    "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp", "cmdi_joints_to_features", "cmdi_convert_motion",
 ]
 
 
@@ -99,6 +100,9 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
     ll = ctypes.c_longlong
     lib.cmdi_recover_from_ric.argtypes = [c_void_p, ll, ll, ll, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                           ll, ll, ll, ll, c_void_p]
+    lib.cmdi_joints_to_features.argtypes = [c_void_p, ll, ll, c_int, c_int, c_int, c_double, c_void_p, ll, ll, ll, c_void_p]
+    lib.cmdi_convert_motion.argtypes = [c_int, c_void_p, ll, ll, ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                        c_void_p, c_void_p, c_int, c_double, c_void_p, ll, ll, ll, c_void_p]
     lib.cmdi_profile_pass.argtypes = [c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, POINTER(c_int), c_void_p]
     lib.cmdi_test_layernorm_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]
     lib.cmdi_test_attention_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]

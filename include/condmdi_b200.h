@@ -209,6 +209,44 @@ CMDI_API int cmdi_recover_from_ric(const float* data, long long stride_seq, long
                           const float* mean, const float* std, int num_seqs, int nframes, int nfeats, int joints_num,
                           int abs_3d, float* out, long long ostride_seq, long long ostride_frame, long long ostride_joint,
                           long long ostride_coord, void* stream);
+/* HumanML3D representation conversions, 22-joint skeleton only (paramUtil.t2m_raw_offsets / t2m_kinematic_chain,
+ * face joints [2, 1, 17, 16], feet [8, 11] / [7, 10]).  One CTA per sequence, one launch on the caller's stream, no host
+ * synchronisation.  Device pointers; strides in elements.  Limits: 2 <= nframes <= 224, joints_num == 22, nfeats == 263.
+ *
+ * cmdi_joints_to_features: extract_features (data_loaders/humanml/scripts/motion_process.py:50-187)
+ *   joints : (num_seqs, nframes, 22, 3) fp32, sequence b / frame f at joints[b*stride_seq + f*stride_frame], the 66
+ *            coordinates of a frame contiguous
+ *   out    : (num_seqs, nframes - 1, 263) de-normalised features, element (b, f, c) at
+ *            out[b*ostride_seq + f*ostride_frame + c*ostride_feat]; contacts compare the squared displacement to feet_thre */
+CMDI_API int cmdi_joints_to_features(const float* joints, long long stride_seq, long long stride_frame, int num_seqs,
+                            int nframes, int joints_num, double feet_thre, float* out, long long ostride_seq,
+                            long long ostride_frame, long long ostride_feat, void* stream);
+
+enum {
+  CMDI_MOTION_ABS3D_TO_REL = 0,    /* dataset.py:1327-1361 abs3d_to_rel                                               */
+  CMDI_MOTION_REL_TO_ABS3D = 1,    /* dataset.py:1364-1401 rel_to_abs3d                                               */
+  CMDI_MOTION_REL_TO_JOINTS = 2,   /* inv_transform + recover_from_ric(abs_3d=False)                                 */
+  CMDI_MOTION_ABS3D_TO_JOINTS = 3  /* inv_transform + recover_from_ric(abs_3d=True) (sample_to_motion, dataset.py:1301) */
+};
+/* cmdi_convert_motion: a normalised (num_seqs, 263, 1, nframes) batch, element (b, c, f) at
+ * in[b*stride_seq + c*stride_feat + f*stride_frame], through
+ *   [x @ inv_proj] (inv_random_projection, dataset.py:536-539; inv_proj [263, 263] row-major or NULL)
+ *   -> x * std_in + mean_in (inv_transform, dataset.py:378-382) -> recover_from_ric (motion_process.py:474-489)
+ * and, for the two representation directions,
+ *   -> extract_features -> duplicate the last row (dataset.py:1214) -> [ABS3D_TO_REL] (x - mean_out) / std_out
+ *                                                                     [REL_TO_ABS3D] channels 0..2 replaced by rot_ang and
+ *      r_pos.xz of recover_root_rot_pos(abs_3d=False) (dataset.py:1276-1279), then (x - mean_out) / std_out
+ * out: the same layout as `in` (ostride_*), or for the *_TO_JOINTS directions positions (num_seqs, 22, 3, nframes) with
+ *      element (b, joint j, coordinate k, f) at out[b*ostride_seq + (3*j + k)*ostride_feat + f*ostride_frame] (mean_out /
+ *      std_out unused).
+ * Statistics are float64 arrays; in_f64 / out_f64 = 1 computes that (de-)normalisation in float64, as the reference does
+ * for float64 statistics, 0 in float32 (the statistics then hold float32 values). */
+CMDI_API int cmdi_convert_motion(int direction, const float* in, long long stride_seq, long long stride_feat,
+                        long long stride_frame, int num_seqs, int nframes, int nfeats, const float* inv_proj,
+                        const double* mean_in, const double* std_in, int in_f64, const double* mean_out,
+                        const double* std_out, int out_f64, double feet_thre, float* out, long long ostride_seq,
+                        long long ostride_feat, long long ostride_frame, void* stream);
+
 /* out[i] = element i of torch.randn(numel, device=this GPU) under generator state (seed, offset); `threads` as
  * cmdi_sample_args.aten_threads */
 CMDI_API int cmdi_test_normal_aten(float* out, long long numel, unsigned long long seed, unsigned long long offset,
