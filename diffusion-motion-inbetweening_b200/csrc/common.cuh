@@ -115,15 +115,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug must surface as a trapped kernel (an error the host sees),
 // never as a hung GPU. ~4e9 cycles is seconds; every legitimate wait here is microseconds.
+// No printf on the timeout path: it compiles to a call to vprintf, and ptxas serialises every wgmma of a kernel that
+// contains a call (C7510), so one diagnostic line would cost every MMA kernel its tensor-core pipelining.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("cmdi: mbarrier timeout block=(%d,%d) thread=%d bar=%u parity=%u\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
 
@@ -280,13 +278,8 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
 // added into acc0 / acc1 with fp32 adds on the CUDA cores.  The tensor cores' own fp32 accumulation rounds toward zero:
 // carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
 // instead, the bias stays at the level of a 64-long sum.
-// One 64-deep k-block of a 128-row x PART_N tile for one warpgroup (A: interleaved 128-row K-major tile, B: PART_N
-// K-major rows; a_plane / b_plane: offsets of the lo planes), with nterms = split ? 3 : 1 bf16 products (lo*hi, hi*lo,
-// hi*hi).  The tensor cores accumulate each 64-column chunk of the k-block in a fresh register fragment, which is then
-// added into acc0 / acc1 with fp32 adds on the CUDA cores.  The tensor cores' own fp32 accumulation rounds toward zero:
-// carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
-// instead, the bias stays at the level of a 64-long sum.  (Measured on H100: double-buffering 32-column chunks so that
-// the adds of one chunk overlap the MMAs of the next is no faster.)
+// A runtime `split` can put the wgmmas behind the term loop's early exit on a divergent path, and ptxas then serialises
+// all of them (C7520): linear_chain_kernel passes a compile-time constant.
 // F16: the operands are single fp16 planes (CMDI_PRECISION_FP16; `split` must be false), same descriptors and swizzle.
 template <int PART_N, bool F16 = false>
 __device__ __forceinline__ void mma_kblock_promoted(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], uint32_t sa, uint32_t sb,

@@ -557,7 +557,7 @@ int run_denoiser_chain(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool ha
     for (int r_ = 0; r_ < reps; ++r_) {
       if (reps > 1)  // profiling repeats one launch back to back: its counters start from zero each time
         CK(cudaMemsetAsync(e->chain_ctr + (size_t)l * 3 * e->max_m_pairs, 0, (size_t)3 * e->max_m_pairs * sizeof(int), s));
-      CK(launch_linear_chain(ct->dev + (size_t)l * kMaxChainPhases, kMaxChainPhases, ct->total_tiles[l], e->num_sms, s,
+      CK(launch_linear_chain(ct->dev + (size_t)l * kMaxChainPhases, kMaxChainPhases, ct->total_tiles[l], e->nsplit, e->num_sms, s,
                              (evs && l == 1) ? e->chain_dbg : nullptr));
     }
     CKI(mark());
@@ -761,7 +761,7 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
   e->cfg = *cfg; e->device = device; e->num_sms = prop.multiProcessorCount; e->nsplit = cfg->precision;
   if (cfg->precision == CMDI_PRECISION_FP16) { e->f16 = true; e->nsplit = 1; }
   // the chained launches spin on counters other CTA pairs bump: every pair must be resident at once
-  if (e->use_chain && linear_chain_max_clusters(e->num_sms) < e->num_sms / 2) e->use_chain = false;
+  if (e->use_chain && linear_chain_max_clusters(e->num_sms, e->nsplit) < e->num_sms / 2) e->use_chain = false;
   e->D = cfg->njoints; e->D_pad = round_up(cfg->njoints, 8); e->L = cfg->nframes; e->S = cfg->nframes + 1;
   e->ff = is_unet ? 256 : cfg->ff_size; e->H = cfg->num_heads; e->layers = is_unet ? 0 : cfg->num_layers; e->maxB = cfg->max_batch;
   if (is_unet) e->S = 2;  // the transformer's sequence buffers are not used: keep them tiny

@@ -64,16 +64,13 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
-// Bounded like mbar_wait: a protocol bug must trap, not hang the GPU.
+// Bounded like mbar_wait: a protocol bug must trap, not hang the GPU (and, like it, without a printf: see mbar_wait).
 __device__ __forceinline__ void wait_counter(const int* ctr, int target) {
   if (ld_acquire_gpu(ctr) >= target) return;
   const long long t0 = clock64();
   while (ld_acquire_gpu(ctr) < target) {
     __nanosleep(32);
-    if (clock64() - t0 > 4000000000LL) {
-      printf("cmdi: chain dependency timeout block=%d counter=%p value=%d target=%d\n", blockIdx.x, ctr, ld_acquire_gpu(ctr), target);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
 
@@ -443,6 +440,7 @@ __device__ __forceinline__ void epilogue_slice(const LinearParams& p, const Chai
 }
 
 // The operand stream of one CTA (thread 0): k-block after k-block of its tiles, one ring stage each.
+template <int NSPLIT>
 struct ChainProducer {
   const ChainPhaseDesc* phases;
   const ChainPhaseInfo* info;
@@ -471,7 +469,7 @@ struct ChainProducer {
       wait_counter(pi.wait_ctr + m_pair, pi.wait_target);
       fence_proxy_async_all();
     }
-    const int nplanes = (pi.p.nsplit == 3) ? 2 : 1;
+    constexpr int nplanes = (NSPLIT == 3) ? 2 : 1;
     mbar_wait(&bars->empty[stage], phase ^ 1);
     uint8_t* da = ring + (size_t)stage * kStageBytes;
     uint8_t* dw = da + 2 * kPlaneBytes;
@@ -484,7 +482,7 @@ struct ChainProducer {
       tma_load_2d(da, &pd.a_hi, &bars->full[stage], kc, m_blk * kBlockM);
       tma_load_2d(dw, &pd.w_hi, &bars->full[stage], kc, n_blk * kBlockN);
       tma_load_2d(dw + kWPlaneBytes / 2, &pd.w_hi, &bars->full[stage], kc, n_blk * kBlockN + kBlockN / 2);
-      if (nplanes == 2) {
+      if constexpr (nplanes == 2) {
         tma_load_2d(da + kPlaneBytes, &pd.a_lo, &bars->full[stage], kc, m_blk * kBlockM);
         tma_load_2d(dw + kWPlaneBytes, &pd.w_lo, &bars->full[stage], kc, n_blk * kBlockN);
         tma_load_2d(dw + kWPlaneBytes + kWPlaneBytes / 2, &pd.w_lo, &bars->full[stage], kc, n_blk * kBlockN + kBlockN / 2);
@@ -497,6 +495,10 @@ struct ChainProducer {
   }
 };
 
+// NSPLIT (1 or 3: the bf16 products per MMA, as LinearParams::nsplit; every phase of a launch has the same) is a
+// template parameter so that mma_kblock_promoted's term loop has a constant trip count: with a runtime count its early
+// exit puts the wgmmas on a divergent path, and ptxas then serialises all of them (C7520).
+template <int NSPLIT>
 __global__ void __launch_bounds__(kNumThreads, 1)
 linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_phases, const int total_tiles, long long* dbg) {
   // dbg (bring-up, CMDI_CHAIN_DBG=1): [gridDim.x][kMaxChainPhases][16] cycle counters per CTA and phase:
@@ -534,7 +536,7 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
     fence_barrier_init();
   }
   __syncthreads();
-  ChainProducer prod{phases, info, ring, bars, cluster_id, num_clusters, rank, my_tiles, 0, 0, 0, 0, 0u, 0};
+  ChainProducer<NSPLIT> prod{phases, info, ring, bars, cluster_id, num_clusters, rank, my_tiles, 0, 0, 0, 0, 0u, 0};
 
   const int j3 = warp_idx >> 2;          // warpgroup = column half of the tile
   const int lane_group = warp_idx & 3;   // rows 32 * lane_group .. + 31 of the CTA's 128
@@ -553,7 +555,6 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
     const int m_blk = 2 * (local / pi.num_n_blocks) + rank;
     const int n_blk = local % pi.num_n_blocks;
     const bool wide = pi.wide != 0;
-    const bool split = pi.p.nsplit == 3;
     load_tile_constants(pi.p, rs, n_blk, j3, wide, lane);
     // ---- mainloop ----
 #pragma unroll
@@ -567,7 +568,7 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
       }
       mbar_wait(&bars->full[stage], phase);
       const uint32_t sa = smem_u32(ring + (size_t)stage * kStageBytes);
-      if (!(pi.p.debug & 2)) mma_kblock_promoted<kPartN>(acc0, acc1, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, split);
+      if (!(pi.p.debug & 2)) mma_kblock_promoted<kPartN>(acc0, acc1, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, NSPLIT == 3);
       // the tensor cores have read this stage: it may be refilled
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars->empty[stage]);
@@ -611,36 +612,42 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
 }  // namespace
 
 cudaError_t configure_linear_chain_kernel() {
-  return cudaFuncSetAttribute(linear_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+  cudaError_t e = cudaFuncSetAttribute(linear_chain_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(linear_chain_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
 }
 
-// how many CTA pairs of this kernel can be resident at once on the current device (they spin on each other's counters:
-// the launch must never exceed this)
-int linear_chain_max_clusters(int num_sms) {
+// how many CTA pairs of the nsplit instance can be resident at once on the current device (they spin on each other's
+// counters: the launch must never exceed this)
+int linear_chain_max_clusters(int num_sms, int nsplit) {
   int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_chain_kernel, kNumThreads, kSmemBytes) != cudaSuccess) {
+  const cudaError_t e = nsplit == 3
+      ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_chain_kernel<3>, kNumThreads, kSmemBytes)
+      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_chain_kernel<1>, kNumThreads, kSmemBytes);
+  if (e != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
   return per_sm * num_sms / 2;
 }
 
-cudaError_t launch_linear_chain(const ChainPhaseDesc* phases_dev, int num_phases, int total_tiles, int num_sms, cudaStream_t stream,
-                                long long* dbg) {
-  if (num_phases < 1 || num_phases > kMaxChainPhases || total_tiles < 1) {
-    set_last_error("launch_linear_chain: bad phase list (%d phases, %d tiles)", num_phases, total_tiles);
+cudaError_t launch_linear_chain(const ChainPhaseDesc* phases_dev, int num_phases, int total_tiles, int nsplit, int num_sms,
+                                cudaStream_t stream, long long* dbg) {
+  if (num_phases < 1 || num_phases > kMaxChainPhases || total_tiles < 1 || (nsplit != 1 && nsplit != 3)) {
+    set_last_error("launch_linear_chain: bad phase list (%d phases, %d tiles, nsplit %d)", num_phases, total_tiles, nsplit);
     return cudaErrorInvalidValue;
   }
-  static int max_clusters = -1;
-  if (max_clusters < 0) max_clusters = linear_chain_max_clusters(num_sms);
+  static int max_clusters[2] = {-1, -1};  // [nsplit == 3]
+  int& max_c = max_clusters[nsplit == 3];
+  if (max_c < 0) max_c = linear_chain_max_clusters(num_sms, nsplit);
   int clusters = num_sms / 2;
   if (clusters > total_tiles) clusters = total_tiles;
-  if (clusters > max_clusters) {
-    set_last_error("launch_linear_chain: %d co-resident CTA pairs needed, the device offers %d", clusters, max_clusters);
+  if (clusters > max_c) {
+    set_last_error("launch_linear_chain: %d co-resident CTA pairs needed, the device offers %d", clusters, max_c);
     return cudaErrorInvalidConfiguration;
   }
-  return launch_kernel(linear_chain_kernel, dim3(2 * clusters), dim3(kNumThreads), (size_t)kSmemBytes, stream, phases_dev,
-                          num_phases, total_tiles, dbg);
+  return launch_kernel(nsplit == 3 ? linear_chain_kernel<3> : linear_chain_kernel<1>, dim3(2 * clusters), dim3(kNumThreads),
+                       (size_t)kSmemBytes, stream, phases_dev, num_phases, total_tiles, dbg);
 }
 
 }  // namespace cmdi

@@ -120,10 +120,11 @@ struct alignas(128) ChainPhaseDesc {
   ChainPhaseInfo info;
 };
 cudaError_t configure_linear_chain_kernel();
-// phases: device array; returns cudaErrorInvalidConfiguration if `num_sms / 2` clusters cannot be co-resident
-cudaError_t launch_linear_chain(const ChainPhaseDesc* phases_dev, int num_phases, int total_tiles, int num_sms,
+// phases: device array, every phase built with info.p.nsplit == nsplit (1 or 3: the kernel instance launched);
+// returns cudaErrorInvalidConfiguration if `num_sms / 2` clusters cannot be co-resident
+cudaError_t launch_linear_chain(const ChainPhaseDesc* phases_dev, int num_phases, int total_tiles, int nsplit, int num_sms,
                                 cudaStream_t stream, long long* dbg = nullptr);
-int linear_chain_max_clusters(int num_sms);
+int linear_chain_max_clusters(int num_sms, int nsplit);
 
 // ----------------------------------------------------------------------------------------------
 // self-attention core: O = softmax(Q K^T / sqrt(dh)) V per (sequence, head)      (attention.cu)
