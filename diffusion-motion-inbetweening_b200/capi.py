@@ -18,6 +18,7 @@ RNG_ENGINE, RNG_TORCH = 0, 1
 SAMPLER_DDPM = 0
 SAMPLER_DDIM = 1
 SAMPLER_PLMS = 2
+SAMPLER_DDIM_REVERSE = 3  # DDIM inversion x_t -> x_{t+1} (ddim_reverse_sample); the loop ascends from skip_timesteps
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
 MOTION_ABS3D_TO_REL, MOTION_REL_TO_ABS3D, MOTION_REL_TO_JOINTS, MOTION_ABS3D_TO_JOINTS = 0, 1, 2, 3
 

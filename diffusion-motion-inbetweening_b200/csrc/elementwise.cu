@@ -7,6 +7,7 @@
 //                          + ClassifierFreeSampleModel combine                     cfg_sampler.py:25-35
 //                          + keyframe imputation blend                             gaussian_diffusion.py:427-435
 //   plms_step              plms_sample (pseudo linear multistep), same combine      gaussian_diffusion.py:1589-1687
+//   ddim_reverse_step      ddim_reverse_sample (DDIM inversion, eta = 0), same combine  gaussian_diffusion.py:1418-1452
 //   layout converters      reference [B,D,1,L] <-> frame-major [B*L, D_pad]
 //
 // The step kernel uses explicit non-contracted fp32 intrinsics (__fmul_rn/__fadd_rn) in the
@@ -360,6 +361,66 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, cons
     if (p.pred_xstart && q.phase != 2) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
   }
   if (q.phase != 2) advance_step(p.step_ptr, t - 1);
+}
+
+// ---------------------------------------------------------------------------------------------
+// DDIM reverse step (ddim_reverse_sample, gaussian_diffusion.py:1418-1452, eta = 0) on frame-major state [B*L, D_pad]:
+// the deterministic encoder x_t -> x_{t+1}.  One thread = 4 consecutive features of one frame.  pred_xstart is the
+// shared combine (p_mean_variance); no noise is drawn.  Advances t -> t + 1.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) ddim_reverse_step_kernel(const StepParams p) {
+  const int t = *p.step_ptr;
+  const float r1 = p.tab.sqrt_recip_acp[t], r2 = p.tab.sqrt_recipm1_acp[t];
+  const float abn = p.tab.acp_next[t];  // _extract_into_tensor(alphas_cumprod_next, t).float() (:1445-1446)
+  const float sq_abn = sqrtf(abn), sq_1m_abn = sqrtf(__fsub_rn(1.0f, abn));
+  const bool do_impute = p.impute && (t >= p.stop_imputation_at);
+  const float guide_c = p.guided ? p.guide_coef[t] : 0.f;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i4 < n4) {
+    const size_t idx = i4 * 4;
+    const int c = (int)(idx % p.D_pad);
+    const int b = (int)(idx / ((size_t)p.L * p.D_pad));
+    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
+    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
+    const bool need_obs = p.guided || do_impute;
+    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
+    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
+    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
+    if (p.guided) {
+      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
+      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
+    }
+    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
+    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
+    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
+    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
+    float xn4[4], x04[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float xn = 0.f, x0 = 0.f;
+      if (c + j < p.D) {
+        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
+        // eps = (sqrt_recip_acp[t] x - x0) / sqrt_recipm1_acp[t] (:1442-1444);
+        // mean_pred = x0 sqrt(ab_next) + sqrt(1 - ab_next) eps (:1449-1450)
+        const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(r1, xtv[j]), x0), r2);
+        xn = __fadd_rn(__fmul_rn(x0, sq_abn), __fmul_rn(sq_1m_abn, eps));
+      }
+      xn4[j] = xn;
+      x04[j] = x0;
+    }
+    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
+    uint32_t h01, l01, h23, l23;
+    split_bf16x2(xn4[0], xn4[1], h01, l01);
+    split_bf16x2(xn4[2], xn4[3], h23, l23);
+    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
+    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
+    if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+  }
+  advance_step(p.step_ptr, t + 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -781,6 +842,12 @@ cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStrea
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   return launch_kernel(plms_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+}
+
+cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream) {
+  if ((p.D_pad & 3) || !p.x_next || !p.x_next_hi || !p.tab.acp_next) return cudaErrorInvalidValue;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  return launch_kernel(ddim_reverse_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p);
 }
 
 cudaError_t launch_ref_to_frames(const float* ref, int B, int D, int L, int D_pad, float* out_f32, __nv_bfloat16* out_hi,

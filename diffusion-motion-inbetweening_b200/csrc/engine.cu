@@ -131,7 +131,7 @@ struct cmdi_engine {
   int T = 0;
   std::vector<double> h_sqrt_acp, h_sqrt_1m_acp;
   std::vector<int> h_tmap;
-  float* tables = nullptr;  // 7 x [T]
+  float* tables = nullptr;  // 8 x [T]
   int* d_tmap = nullptr;
   StepTables tab{};
   // activations
@@ -1038,7 +1038,7 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
   CK(cudaSetDevice(e->device));
   // float64 tables exactly as GaussianDiffusion.__init__ builds them (gaussian_diffusion.py:183-217),
   // cast to fp32 at the point _extract_into_tensor does (.float() after the gather, :2225).
-  std::vector<double> betas(betas_in, betas_in + T), acp(T), acp_prev(T), post_var(T);
+  std::vector<double> betas(betas_in, betas_in + T), acp(T), acp_prev(T), acp_next(T), post_var(T);
   double run = 1.0;
   for (int i = 0; i < T; ++i) {
     if (!(betas[i] > 0 && betas[i] <= 1)) {
@@ -1050,7 +1050,8 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
   }
   // np.cumprod is a sequential product in float64: identical rounding to the loop above
   for (int i = 0; i < T; ++i) acp_prev[i] = i == 0 ? 1.0 : acp[i - 1];
-  std::vector<float> host((size_t)7 * T);
+  for (int i = 0; i < T; ++i) acp_next[i] = i + 1 < T ? acp[i + 1] : 0.0;  // np.append(acp[1:], 0.0) (:194)
+  std::vector<float> host((size_t)8 * T);
   e->h_sqrt_acp.assign(T, 0.0);
   e->h_sqrt_1m_acp.assign(T, 0.0);
   for (int i = 0; i < T; ++i) post_var[i] = betas[i] * (1.0 - acp_prev[i]) / (1.0 - acp[i]);
@@ -1063,6 +1064,7 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
     host[4 * T + i] = (float)std::sqrt(1.0 / acp[i] - 1);                                   // sqrt_recipm1_alphas_cumprod
     host[5 * T + i] = (float)acp[i];
     host[6 * T + i] = (float)acp_prev[i];
+    host[7 * T + i] = (float)acp_next[i];
     e->h_sqrt_acp[i] = std::sqrt(acp[i]);
     e->h_sqrt_1m_acp[i] = std::sqrt(1.0 - acp[i]);
   }
@@ -1084,7 +1086,7 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
   e->T = T;
   e->tab.post_coef1 = e->tables + 0 * T; e->tab.post_coef2 = e->tables + 1 * T; e->tab.post_logvar = e->tables + 2 * T;
   e->tab.sqrt_recip_acp = e->tables + 3 * T; e->tab.sqrt_recipm1_acp = e->tables + 4 * T;
-  e->tab.acp = e->tables + 5 * T; e->tab.acp_prev = e->tables + 6 * T;
+  e->tab.acp = e->tables + 5 * T; e->tab.acp_prev = e->tables + 6 * T; e->tab.acp_next = e->tables + 7 * T;
   for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
   e->graphs.clear();
   return 0;
@@ -1202,11 +1204,28 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CK(cudaSetDevice(e->device));
   const int B = a->batch;
   CKI(check_ready(e, B, true));
-  if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS) {
+  if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
+      a->sampler != CMDI_SAMPLER_DDIM_REVERSE) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
+  // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
+  // nothing and has no q_sample, dump or PLMS history
+  const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
+  if (rev) {
+    const char* bad = a->eta != 0.f ? "eta (the reverse ODE is deterministic: eta must be 0)"
+                      : a->noise_tape ? "noise_tape" : a->init_image ? "init_image" : a->dump_xstart ? "dump_xstart"
+                      : a->plms_order ? "plms_order" : a->plms_old_eps_out ? "plms_old_eps_out" : nullptr;
+    if (bad) {
+      set_last_error("CMDI_SAMPLER_DDIM_REVERSE: %s must be unset", bad);
+      return 1;
+    }
+    if (!a->x_T) {
+      set_last_error("CMDI_SAMPLER_DDIM_REVERSE needs x_T, the state to invert");
+      return 1;
+    }
+  }
   if (plms && (a->plms_order < 2 || a->plms_order > 4)) {
     set_last_error("plms_order %d outside [2, 4]", a->plms_order);
     return 1;
@@ -1242,8 +1261,9 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   }
   const bool host = a->host_buffers != 0;
   const size_t n = (size_t)B * e->D * e->L;
-  const int t0 = e->T - 1 - a->skip_timesteps;
-  const int nsteps = (a->num_steps > 0 && a->num_steps < t0 + 1) ? a->num_steps : t0 + 1;
+  const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
+  const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
+  const int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
   // PLMS: a call without `resume` starts a new eps history at t0; a `resume` call continues the running one
   int hist_t0 = t0;
   if (plms) {
@@ -1295,7 +1315,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CK(launch_set_rng(e->rng, rng, s));
   e->launches += 1;
   // ---- init_image / skip_timesteps: img = q_sample(init_image, t0, img) (:1252-1260) ----
-  if (!a->resume && (a->init_image || a->skip_timesteps)) {
+  if (!rev && !a->resume && (a->init_image || a->skip_timesteps)) {
     const float* init = (const float*)stage_in(a->init_image, e->ref_b, n * 4, host, s, &rc);
     if (rc) return 1;
     if (!init) {
@@ -1345,7 +1365,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;  // first step index: step_ctr[2] (graphs do not depend on it)
     sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
     sp.pred_xstart = e->pred_x0;
-    CK(launch_diffusion_step(sp, st));
+    CK(rev ? launch_ddim_reverse_step(sp, st) : launch_diffusion_step(sp, st));
     return 0;
   };
 
@@ -1453,7 +1473,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   };
 
   int dump_i = 0;
-  auto guided_at = [&](int k) { return a->recon_guidance && (t0 - k) >= a->stop_recguidance_at; };
+  auto guided_at = [&](int k) { return a->recon_guidance && (rev ? t0 + k : t0 - k) >= a->stop_recguidance_at; };
   for (int k = 0; k < nsteps;) {
     if (plms) {
       CKI(plms_step(k));

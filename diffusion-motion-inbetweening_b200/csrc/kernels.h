@@ -191,6 +191,7 @@ struct StepTables {            // device pointers, each [T] fp32, indexed by sam
   const float* sqrt_recipm1_acp;  // sqrt(1/alphas_cumprod - 1)
   const float* acp;               // alphas_cumprod
   const float* acp_prev;          // alphas_cumprod_prev
+  const float* acp_next;          // alphas_cumprod_next (last entry 0)
 };
 struct RngState {
   unsigned long long seed;           // Philox key
@@ -252,6 +253,10 @@ struct PlmsParams {
   float* x_keep;       // [B*L, D_pad] the first step's x_t, kept across its second evaluation
 };
 cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStream_t stream);
+// DDIM reverse step (ddim_reverse_sample, gaussian_diffusion.py:1418-1452, eta = 0): x_t -> x_{t+1} from the same combine
+// inputs as StepParams (its sampler, eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are
+// required).  Advances the step index t -> t + 1, so one captured graph serves every step of an inversion.
+cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream);
 
 // HumanML3D vectors -> joint positions (recover_from_ric), strides in elements; mean/stdv null = already de-normalised
 cudaError_t launch_recover_from_ric(const float* data, long long sb, long long sf, long long sc, const float* mean,

@@ -3,14 +3,15 @@
 Mirrors (same names, argument meaning and error behaviour; paths relative to the reference repository):
     get_named_beta_schedule / betas_for_alpha_bar   diffusion/gaussian_diffusion.py:24-71
     ModelMeanType / ModelVarType / DiffusionConfig  :74-136
-    GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1454-1587, :1589-1804
+    GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1418-1587, :1589-1804
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
-`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` run the WHOLE loop in one native call (`cmdi_sample`): no
-per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
+`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` run the WHOLE loop in one native
+call (`cmdi_sample`): no per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
-`p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` is done by the CUDA kernels in csrc/.
+`p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` / `ddim_reverse_sample` is done by the CUDA
+kernels in csrc/.
 
 Not accelerated (raise NotImplementedError, like the reference does for its own unsupported branches):
 cond_fn / 'gmd' classifier guidance, learned variances, EPSILON/PREVIOUS_X parametrisations,
@@ -154,11 +155,12 @@ class GaussianDiffusion:
         return y
 
     def _run(self, sampler, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image, randomize_class,
-             dump_steps, const_noise, eta, progressive=False, order=2):
+             dump_steps, const_noise, eta, progressive=False, order=2, num_steps=0, want_pred_xstart=False):
         if model_kwargs is None:
             model_kwargs = {}
         y = self._check_supported(cond_fn, const_noise, randomize_class, model_kwargs)
         plms = sampler == capi.SAMPLER_PLMS
+        rev = sampler == capi.SAMPLER_DDIM_REVERSE  # `noise` is the state to invert; skip_timesteps its step index
         if sampler == capi.SAMPLER_DDPM:
             assert cond_fn is None, "only support the case where cond_fn is None"  # gaussian_diffusion.py:685
         elif cond_fn is not None:
@@ -234,9 +236,10 @@ class GaussianDiffusion:
         if tape is not None:
             tape = tape[1:]
         seed, rng_args = 0, {}
-        if plms:
+        if plms or rev:
             # plms_sample_loop_progressive draws nothing after x_T (:1767-1770): a tape contributes tape[0] only, torch's
-            # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine"
+            # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine".
+            # DDIM inversion draws nothing at all: x_T is the caller's state
             tape = None
             if x_T is None:
                 seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -253,7 +256,7 @@ class GaussianDiffusion:
                 rng_args = {}
             else:
                 seed = rng_args.pop("seed")
-        if skip_timesteps and init_image is None:
+        if skip_timesteps and init_image is None and not rev:
             init_image = torch.zeros(tuple(shape), device=device, dtype=torch.float32)
         if init_image is not None:
             init_image = init_image.to(device=device, dtype=torch.float32)
@@ -268,6 +271,11 @@ class GaussianDiffusion:
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
+        if rev:
+            if progressive:
+                return self._reverse_progressive(eng, x_T, skip_timesteps, common)
+            return eng.sample(skip_timesteps=skip_timesteps, num_steps=num_steps, x_T=x_T, want_pred_xstart=want_pred_xstart,
+                              **common)
         if plms:
             common["plms_order"] = int(order)
             if progressive:
@@ -311,6 +319,18 @@ class GaussianDiffusion:
                              x_T=state, want_pred_xstart=True, want_old_eps=True, **common)
             state = res["sample"]
             yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"], "old_eps": res["old_eps"]}
+
+    def _reverse_progressive(self, eng, x_start, skip_timesteps, common):
+        """DDIM inversion as a generator: one native call per step (the step graph is shared), each starting from the
+        previous call's sample, so the samples equal the fused loop's bit for bit.  A caller that stops early has a
+        partial inversion."""
+        state = x_start
+        common = dict(common)
+        common["use_graph"] = 2 if common.get("use_graph", True) else 0
+        for k in range(self.num_timesteps - skip_timesteps):
+            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, x_T=state, want_pred_xstart=True, **common)
+            state = res["sample"]
+            yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
 
     # ------------------------------------------------------------------------------------------
     def p_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
@@ -367,6 +387,43 @@ class GaussianDiffusion:
         _check_plms_order(order)
         return self._run(capi.SAMPLER_PLMS, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image,
                          randomize_class, None, False, 0.0, progressive=True, order=order)
+
+    def ddim_reverse_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
+        """gaussian_diffusion.py:1418-1452: x_t -> x_{t+1} by the reverse DDIM ODE, one native call.  Returns
+        {"sample", "pred_xstart"}.  `t` must hold one step index for the whole batch (the engine's step index is per
+        call)."""
+        assert eta == 0.0, "Reverse ODE only for deterministic path"
+        _check_no_denoised_fn(denoised_fn)
+        ts = torch.as_tensor(t).reshape(-1)
+        if ts.numel() != x.shape[0] or not bool((ts == ts[0]).all()):
+            raise NotImplementedError("ddim_reverse_sample runs one step index for the whole batch: t must be uniform")
+        res = self._run(capi.SAMPLER_DDIM_REVERSE, model, tuple(x.shape), x, None, model_kwargs, None, int(ts[0]), None, False,
+                        None, False, 0.0, num_steps=1, want_pred_xstart=True)
+        return {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
+
+    def ddim_reverse_sample_loop(self, model, x_start, clip_denoised=True, denoised_fn=None, model_kwargs=None, device=None,
+                                 progress=False, eta=0.0):
+        """DDIM inversion of x_start: `for i in range(num_timesteps): x = ddim_reverse_sample(model, x, [i] * B)["sample"]`,
+        the whole loop in one native call.  Returns x_T, the noise ddim_sample_loop(noise=x_T, ...) regenerates x_start
+        from.  (The reference exposes the step only.)"""
+        assert eta == 0.0, "Reverse ODE only for deterministic path"
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DDIM_REVERSE, model, tuple(x_start.shape), x_start, None, model_kwargs, device, 0, None,
+                         False, None, False, 0.0)["sample"]
+
+    def ddim_reverse_sample_loop_progressive(self, model, x_start, clip_denoised=True, denoised_fn=None, model_kwargs=None,
+                                             device=None, progress=False, eta=0.0):
+        """Yields ddim_reverse_sample's {"sample", "pred_xstart"} for t = 0, 1, ..., num_timesteps - 1, one native call per
+        step; stopping early gives a partial inversion.  The configuration is validated at the call."""
+        assert eta == 0.0, "Reverse ODE only for deterministic path"
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DDIM_REVERSE, model, tuple(x_start.shape), x_start, None, model_kwargs, device, 0, None,
+                         False, None, False, 0.0, progressive=True)
+
+
+def _check_no_denoised_fn(denoised_fn) -> None:
+    if denoised_fn is not None:
+        raise NotImplementedError("denoised_fn (a host callback on every x0) is not run by the engine")
 
 
 def _check_plms_order(order) -> None:

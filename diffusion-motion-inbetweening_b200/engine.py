@@ -131,6 +131,8 @@ class Engine:
         H2D/D2H copies happen inside the call and the result is a CPU tensor valid on return.
         sampler=SAMPLER_PLMS: `plms_order` is plms_sample's order; want_old_eps adds result["old_eps"], the eps history
         list after the last step (oldest first), as plms_sample_loop_progressive yields it.
+        sampler=SAMPLER_DDIM_REVERSE: DDIM inversion from the state x_T, ascending from t = skip_timesteps; plms_order
+        is not sent.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         dev = torch.device("cpu") if host_buffers else self.device
@@ -190,7 +192,8 @@ class Engine:
                             _ptr(y_mask), int(imputate), int(stop_imputation_at), _ptr(inpainted_motion),
                             _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
                             dump_arr, n_dump, int(host_buffers),
-                            int(use_graph), _ptr(obs_x0), _ptr(obs_mask), int(plms_order), _ptr(old_eps))
+                            int(use_graph), _ptr(obs_x0), _ptr(obs_mask),
+                            0 if sampler == capi.SAMPLER_DDIM_REVERSE else int(plms_order), _ptr(old_eps))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")

@@ -14,6 +14,7 @@
  *   cmdi_sample             the sampling loop       <- diffusion/gaussian_diffusion.py:1149-1297 (p_sample_loop[_progressive]),
  *                                                      :1454-1587 (ddim_sample_loop[_progressive]),
  *                                                      :1589-1804 (plms_sample_loop[_progressive]),
+ *                                                      :1418-1452 (ddim_reverse_sample, looped),
  *                                                      :352-534 (p_mean_variance), :656-713 (p_sample), :1358-1416 (ddim_sample_with_grad)
  *
  * Conventions
@@ -53,7 +54,12 @@ enum {
 };
 
 /* PLMS: pseudo linear multistep (plms_sample_loop, gaussian_diffusion.py:1589-1804): deterministic, no per-step noise */
-enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2 };
+/* DDIM_REVERSE: DDIM inversion (ddim_reverse_sample, gaussian_diffusion.py:1418-1452, eta = 0), the deterministic
+   encoder x_t -> x_{t+1}.  The loop ascends from t0 = skip_timesteps (the iterations already done, counted upwards);
+   x_T is the start state (e.g. x_0) and is required; num_steps as for the other samplers (0 = up to t = T - 1).
+   eta must be 0 and noise_tape, init_image, dump_xstart, plms_order and plms_old_eps_out unset: the call fails
+   naming the field otherwise.  pred_xstart_out receives the last step's x0. */
+enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3 };
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
 
