@@ -113,6 +113,20 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// non-blocking probe: has the phase with this parity completed?
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t"
+      "}\n"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
 // Bounded wait: a protocol bug must surface as a trapped kernel (an error the host sees),
 // never as a hung GPU. ~4e9 cycles is seconds; every legitimate wait here is microseconds.
 // No printf on the timeout path: it compiles to a call to vprintf, and ptxas serialises every wgmma of a kernel that
@@ -278,47 +292,91 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
 // added into acc0 / acc1 with fp32 adds on the CUDA cores.  The tensor cores' own fp32 accumulation rounds toward zero:
 // carried over a whole K = 1024 reduction, that is a bias of -3.5e-6 relative on positive data.  Added up once per k-block
 // instead, the bias stays at the level of a 64-long sum.
-// A runtime `split` can put the wgmmas behind the term loop's early exit on a divergent path, and ptxas then serialises
-// all of them (C7520): linear_chain_kernel passes a compile-time constant.
 // F16: the operands are single fp16 planes (CMDI_PRECISION_FP16; `split` must be false), same descriptors and swizzle.
+//
+// Pipelined: each 64-column chunk c is cut into its two m64 halves h, the sub-chunks (c, h), each summed in a fresh
+// 32-register fragment; two fragments form a ring, so the tensor cores work on one sub-chunk (a commit group of
+// 4 x nterms MMAs) while the CUDA cores add the previous one into the accumulator (wgmma.wait_group 1).  Every fragment
+// receives the same MMAs in the same order as a chunk's half did before (term 0 for k = 0..3, then term 1, then term 2),
+// and is added once per k-block: the sums are the same bit for bit.
+// The term count is a template parameter: with a runtime count the term loop's early exit leaves ptxas unable to tell
+// which commit group a fragment belongs to, and it then waits for every group before the fragment is read (C7517,
+// C7518) or serialises every wgmma (C7520).  mma_kblock_promoted dispatches a runtime `split` once per k-block.
+//
+// One sub-chunk: issue its MMAs into a fresh fragment (the first one with scale-d = 0: D = A * B, which is what ptxas
+// makes of an MMA onto a zeroed fragment anyway), commit them as one group.
+template <int NTERMS, bool F16>
+__device__ __forceinline__ void mma_subchunk_issue(float (&t)[32], uint32_t sa, uint32_t sb, uint32_t a_plane, uint32_t b_plane,
+                                                   int c, int h) {
+  static_assert(NTERMS == 1 || (NTERMS == 3 && !F16), "1 or 3 bf16 products, fp16 operands: 1");
+  constexpr bool split = NTERMS == 3;
+  wgmma_fence();
+#pragma unroll
+  for (int term = 0; term < NTERMS; ++term) {
+    const uint64_t da = make_desc_kmajor_sw128_interleaved(sa + ((split && term == 0) ? a_plane : 0u));
+    const uint64_t db = make_desc_kmajor_sw128(sb + ((split && term == 1) ? b_plane : 0u) + c * 64 * 128);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t scale_d = (term == 0 && k == 0) ? 0u : 1u;
+      if constexpr (F16)
+        wgmma_m64n64k16_ss_f16(t, desc_advance(da, h * 1024 + k * 32), desc_advance(db, k * 32), scale_d);
+      else
+        wgmma_m64n64k16_ss(t, desc_advance(da, h * 1024 + k * 32), desc_advance(db, k * 32), scale_d);
+    }
+  }
+  wgmma_commit();
+}
+// ... and, once its group has retired, its promotion into columns [32 c, 32 c + 32) of the accumulator of half h
+template <int R>
+__device__ __forceinline__ void mma_subchunk_promote(float (&acc)[R], float (&t)[32], int c) {
+  wgmma_fence_operands(t);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[32 * c + i] += t[i];
+}
+
+// The sub-chunks of a k-block in ring order: (c, 0) in t0, (c, 1) in t1, then c + 1.  Expects sub-chunk (0, 0) issued
+// into t0 already; issues the rest, promotes all but the last, and returns with the last, (PART_N / 64 - 1, 1) in t1,
+// still in flight (its commit group is the newest), so that a caller can issue its next k-block's first sub-chunk before
+// it waits for it.  `between()` runs after every promotion (the chained kernel's TMA thread retries a refill there).
+template <int PART_N, int NTERMS, bool F16, class Between>
+__device__ __forceinline__ void mma_kblock_body(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], float (&t0)[32], float (&t1)[32],
+                                                uint32_t sa, uint32_t sb, uint32_t a_plane, uint32_t b_plane, Between&& between) {
+  static_assert(PART_N % 64 == 0, "64-column chunks");
+#pragma unroll
+  for (int c = 0; c < PART_N / 64; ++c) {
+    mma_subchunk_issue<NTERMS, F16>(t1, sa, sb, a_plane, b_plane, c, 1);
+    wgmma_wait<1>();
+    mma_subchunk_promote(acc0, t0, c);
+    between();
+    if (c + 1 < PART_N / 64) {
+      mma_subchunk_issue<NTERMS, F16>(t0, sa, sb, a_plane, b_plane, c + 1, 0);
+      wgmma_wait<1>();
+      mma_subchunk_promote(acc1, t1, c);
+      between();
+    }
+  }
+}
+
+template <int PART_N, int NTERMS, bool F16>
+__device__ __forceinline__ void mma_kblock_pipelined(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], uint32_t sa, uint32_t sb,
+                                                     uint32_t a_plane, uint32_t b_plane) {
+  float t0[32], t1[32];
+  mma_subchunk_issue<NTERMS, F16>(t0, sa, sb, a_plane, b_plane, 0, 0);
+  mma_kblock_body<PART_N, NTERMS, F16>(acc0, acc1, t0, t1, sa, sb, a_plane, b_plane, [] {});
+  wgmma_wait<0>();
+  mma_subchunk_promote(acc1, t1, PART_N / 64 - 1);
+}
+
 template <int PART_N, bool F16 = false>
 __device__ __forceinline__ void mma_kblock_promoted(float (&acc0)[PART_N / 2], float (&acc1)[PART_N / 2], uint32_t sa, uint32_t sb,
                                                     uint32_t a_plane, uint32_t b_plane, bool split) {
-  static_assert(PART_N % 64 == 0, "64-column chunks");
-  const int nterms = split ? 3 : 1;
-#pragma unroll
-  for (int c = 0; c < PART_N / 64; ++c) {
-    float t0[32], t1[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { t0[i] = 0.f; t1[i] = 0.f; }
-    wgmma_fence_operands(t0);
-    wgmma_fence_operands(t1);
-    wgmma_fence();
-#pragma unroll
-    for (int term = 0; term < 3; ++term) {
-      if (term >= nterms) break;
-      const uint64_t da = make_desc_kmajor_sw128_interleaved(sa + ((split && term == 0) ? a_plane : 0u));
-      const uint64_t db = make_desc_kmajor_sw128(sb + ((split && term == 1) ? b_plane : 0u) + c * 64 * 128);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if constexpr (F16) {
-          wgmma_m64n64k16_ss_f16(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
-          wgmma_m64n64k16_ss_f16(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
-        } else {
-          wgmma_m64n64k16_ss(t0, desc_advance(da, k * 32), desc_advance(db, k * 32), 1u);
-          wgmma_m64n64k16_ss(t1, desc_advance(da, 1024 + k * 32), desc_advance(db, k * 32), 1u);
-        }
-      }
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_operands(t0);
-    wgmma_fence_operands(t1);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      acc0[32 * c + i] += t0[i];
-      acc1[32 * c + i] += t1[i];
-    }
+  if constexpr (F16) {
+    mma_kblock_pipelined<PART_N, 1, true>(acc0, acc1, sa, sb, a_plane, b_plane);
+  } else {
+    if (split)
+      mma_kblock_pipelined<PART_N, 3, false>(acc0, acc1, sa, sb, a_plane, b_plane);
+    else
+      mma_kblock_pipelined<PART_N, 1, false>(acc0, acc1, sa, sb, a_plane, b_plane);
   }
 }
 

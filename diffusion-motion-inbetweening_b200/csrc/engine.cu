@@ -1698,7 +1698,8 @@ extern "C" int cmdi_profile_pass(cmdi_engine* e, int batch, int cfg, int repeats
     std::vector<long long> h((size_t)e->num_sms * kMaxChainPhases * 16);
     CK(cudaMemcpy(h.data(), e->chain_dbg, h.size() * 8, cudaMemcpyDeviceToHost));
     CK(cudaMemset(e->chain_dbg, 0, h.size() * 8));
-    const char* names[16] = {"tiles", "tma_dep_wait", "tma_slot_wait", "mma_operand_wait", "mma_acc_wait", "epi0_acc_wait", "epi0_slices", "epi0_publish",
+    // thread 0 of every CTA (see linear_chain_kernel): mainloop = dep_wait + refill_wait + operand_wait + mma_promote
+    const char* names[16] = {"tiles", "tma_dep_wait", "tma_refill_wait", "w0_operand_wait", "w0_mma_promote", "epi0_acc_wait", "epi0_slices", "epi0_publish",
                              "s_rowstats", "s_stage_free", "s_loads+acc", "s_fold_bias_res", "s_stats_act", "s_f32_store", "s_plane_store", "-"};
     for (int ph = 0; ph < kMaxChainPhases; ++ph) {
       double tiles = 0, acc[16] = {0};
@@ -1706,9 +1707,9 @@ extern "C" int cmdi_profile_pass(cmdi_engine* e, int batch, int cfg, int repeats
         tiles += (double)h[((size_t)b * kMaxChainPhases + ph) * 16];
         for (int k = 1; k < 16; ++k) acc[k] += (double)h[((size_t)b * kMaxChainPhases + ph) * 16 + k];
       }
-      // tiles are counted by both CTAs' TMA threads; the MMA counters exist on leaders only
+      // tiles are counted by both CTAs' TMA threads
       fprintf(stderr, "chain dbg phase %d: %.0f tile visits (%d repeats);  cycles per tile:", ph, tiles, repeats);
-      for (int k = 1; k < 15; ++k) fprintf(stderr, " %s=%.0f", names[k], acc[k] / (tiles > 0 ? tiles : 1) * ((k == 3 || k == 4) ? 2.0 : 1.0));
+      for (int k = 1; k < 15; ++k) fprintf(stderr, " %s=%.0f", names[k], acc[k] / (tiles > 0 ? tiles : 1));
       fprintf(stderr, "\n");
     }
   }

@@ -28,6 +28,8 @@
 // cut into 64-column pairs, two per warp: folded-LayerNorm scale / shift, bias, GELU (branch-free rational erf), hi plane
 // then lo plane through 128-byte-swizzled boxes.  Per-column constants are loaded once per tile into registers and
 // handed out by shuffle.  Shared memory: 2 operand stages x 96 KB (A and W, hi + lo), 8 x 4 KB staging tiles.
+#include <type_traits>
+
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include "kernels.h"
@@ -451,8 +453,9 @@ struct ChainProducer {
   uint32_t phase;
   int issued;  // k-blocks issued so far
 
-  // Issues the next k-block.  A tile's first k-block waits for its dependency counter: blocking, or (blocking = false)
-  // only if it is already satisfied -- returns false then without issuing.
+  // Issues the next k-block.  blocking = false: only if the tile's dependency counter (first k-block) is already
+  // satisfied and both warpgroups have released the stage; returns false then without issuing, and the caller retries
+  // later instead of waiting for the other warpgroup.
   __device__ bool issue_next(bool blocking) {
     if (seq >= my_tiles) return false;
     const int tile = cluster_id + seq * num_clusters;
@@ -470,6 +473,7 @@ struct ChainProducer {
       fence_proxy_async_all();
     }
     constexpr int nplanes = (NSPLIT == 3) ? 2 : 1;
+    if (!blocking && !mbar_test_wait(&bars->empty[stage], phase ^ 1)) return false;
     mbar_wait(&bars->empty[stage], phase ^ 1);
     uint8_t* da = ring + (size_t)stage * kStageBytes;
     uint8_t* dw = da + 2 * kPlaneBytes;
@@ -501,8 +505,9 @@ struct ChainProducer {
 template <int NSPLIT>
 __global__ void __launch_bounds__(kNumThreads, 1)
 linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_phases, const int total_tiles, long long* dbg) {
-  // dbg (bring-up, CMDI_CHAIN_DBG=1): [gridDim.x][kMaxChainPhases][16] cycle counters per CTA and phase:
-  //   0 tiles  1 dependency wait at the tile start  5 warp 0: operand wait  6 its epilogue work  7 its publish wait
+  // dbg (bring-up, CMDI_CHAIN_DBG=1): [gridDim.x][kMaxChainPhases][16] counters per CTA and phase, thread 0:
+  //   0 tiles  1 dependency wait at the tile start  2 blocking refills inside the mainloop  3 operand wait (full barriers)
+  //   4 MMA issue + promotion (the rest of the mainloop)  5 mainloop  6 epilogue  7 publish wait
   long long* dbg_me = dbg ? dbg + (size_t)blockIdx.x * kMaxChainPhases * 16 : nullptr;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -557,25 +562,50 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
     const bool wide = pi.wide != 0;
     load_tile_constants(pi.p, rs, n_blk, j3, wide, lane);
     // ---- mainloop ----
+    // Thread 0 refills stages without blocking: a stage the other warpgroup still reads is retried after the next
+    // sub-chunk's promotion (mma_kblock_body), so neither warpgroup waits for the other inside the k-block loop; thread 0
+    // blocks only for the k-block the MMAs need next.  Every k-block's wgmmas have retired at its end: carrying the
+    // fragment ring across the k-block boundary, over the barrier waits and thread 0's producer branch, makes ptxas
+    // serialise every wgmma of the kernel (C7518).
+    long long dep_wait = 0, issue_wait = 0, operand_wait = 0;  // thread 0's cycles (CMDI_CHAIN_DBG)
+    auto refill = [&] {
+      if (is_producer && prod.issued < consumed + kStages) prod.issue_next(false);
+    };
+    // The k-block loop exists twice, with and without MMAs (CMDI_CHAIN_SKIP=2), chosen once per tile: the same loop with
+    // the MMAs behind a runtime test inside it puts them on a divergent path, and ptxas serialises them (C7520).
+    auto mainloop = [&](auto with_mma) {
+      for (int kb = 0; kb < pi.num_k_blocks; ++kb) {
+        if (is_producer) {
+          // every earlier tile of this CTA is published: blocking on a dependency counter is safe here
+          const long long d0 = clock64();
+          while (prod.issued <= consumed) prod.issue_next(true);
+          (kb > 0 ? issue_wait : dep_wait) += clock64() - d0;
+        }
+        const long long d1 = clock64();
+        mbar_wait(&bars->full[stage], phase);
+        operand_wait += clock64() - d1;
+        const uint32_t sa = smem_u32(ring + (size_t)stage * kStageBytes);
+        if constexpr (decltype(with_mma)::value) {
+          float t0[32], t1[32];
+          mma_subchunk_issue<NSPLIT, false>(t0, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, 0, 0);
+          mma_kblock_body<kPartN, NSPLIT, false>(acc0, acc1, t0, t1, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, refill);
+          wgmma_wait<0>();
+          mma_subchunk_promote(acc1, t1, kPartN / 64 - 1);
+        }
+        // the tensor cores have read this stage: it may be refilled
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->empty[stage]);
+        ++consumed;
+        refill();
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    };
 #pragma unroll
     for (int i = 0; i < kPartN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
-    for (int kb = 0; kb < pi.num_k_blocks; ++kb) {
-      if (is_producer) {
-        // every earlier tile of this CTA is published: blocking on a dependency counter is safe here
-        long long d0 = clock64();
-        while (prod.issued <= consumed) prod.issue_next(true);
-        if (dbg_me && kb == 0) { dbg_me[ph * 16 + 0] += 1; dbg_me[ph * 16 + 1] += clock64() - d0; }
-      }
-      mbar_wait(&bars->full[stage], phase);
-      const uint32_t sa = smem_u32(ring + (size_t)stage * kStageBytes);
-      if (!(pi.p.debug & 2)) mma_kblock_promoted<kPartN>(acc0, acc1, sa, sa + w_off, kPlaneBytes, kWPlaneBytes, NSPLIT == 3);
-      // the tensor cores have read this stage: it may be refilled
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->empty[stage]);
-      ++consumed;
-      if (is_producer && prod.issued < consumed + kStages) prod.issue_next(false);
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-    }
+    if (!(pi.p.debug & 2))
+      mainloop(std::true_type{});
+    else
+      mainloop(std::false_type{});
     long long c1 = clock64();
     // ---- epilogue ----
     load_row_statistics(pi.p, rs, m_blk * kBlockM + lane_group * 32 + lane);
@@ -596,6 +626,7 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
       }
     }
     long long c2 = clock64();
+    refill();  // a stage the other warpgroup was still reading at the end of the mainloop
     // ---- publish: everything this CTA stored for the tile is in memory, then one counter bump ----
     __syncwarp();  // the other lanes' plain stores (row-mapped outputs, partial statistics) before lane 0's wait
     if (lane == 0) tma_store_wait_all();
@@ -605,7 +636,14 @@ linear_chain_kernel(const ChainPhaseDesc* __restrict__ phases, const int num_pha
       __threadfence();
       atomicAdd(pi.done_ctr + (tile - pi.tile_begin) / pi.num_n_blocks, 1);
     }
-    if (dbg_w) { dbg_w[5] += c1 - c0; dbg_w[6] += c2 - c1; dbg_w[7] += clock64() - c2; }
+    if (dbg_w) {
+      dbg_w[0] += 1;
+      dbg_w[1] += dep_wait;
+      dbg_w[2] += issue_wait;
+      dbg_w[3] += operand_wait;
+      dbg_w[4] += (c1 - c0) - dep_wait - issue_wait - operand_wait;
+      dbg_w[5] += c1 - c0; dbg_w[6] += c2 - c1; dbg_w[7] += clock64() - c2;
+    }
   }
 }
 
