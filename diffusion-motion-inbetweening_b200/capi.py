@@ -27,6 +27,7 @@ EXPORTS = [
     "cmdi_sample", "cmdi_launch_count", "cmdi_last_error", "cmdi_version", "cmdi_test_linear", "cmdi_test_attention",
     "cmdi_test_layernorm", "cmdi_test_step", "cmdi_test_normal", "cmdi_profile_pass", "cmdi_test_layernorm_bwd", "cmdi_test_attention_bwd",
     "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp", "cmdi_joints_to_features", "cmdi_convert_motion",
+    "cmdi_test_chain_layer", "cmdi_test_attention_hi", "cmdi_test_attention_bwd_at",
 ]
 
 
@@ -93,6 +94,7 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
     lib.cmdi_test_linear.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_void_p]
     lib.cmdi_test_attention.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
+    lib.cmdi_test_attention_hi.argtypes = lib.cmdi_test_attention.argtypes
     lib.cmdi_test_layernorm.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]
     lib.cmdi_test_step.argtypes = [c_void_p, c_int, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
@@ -107,6 +109,8 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
     lib.cmdi_profile_pass.argtypes = [c_void_p, c_int, c_int, c_int, POINTER(c_float), c_int, POINTER(c_int), c_void_p]
     lib.cmdi_test_layernorm_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]
     lib.cmdi_test_attention_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]
+    lib.cmdi_test_attention_bwd_at.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
+    lib.cmdi_test_chain_layer.argtypes = [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_float, c_void_p]
     lib.cmdi_test_input_vjp.argtypes = [c_void_p, POINTER(ForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p]
     _lib = lib
     return lib

@@ -439,6 +439,10 @@ int get_chain_tables(cmdi_engine* e, int nseq, const ChainTables** out) {
         if (e->chain_res_planes) { p.ln_src_hi = e->xseq_p.hi; p.ln_src_lo = e->xseq_p.lo; }
         else p.ln_src = e->vsum;
       }
+      // v1's planes are FFN2's residual source (v = hi + lo): the lo plane is written at bf16 too, where no GEMM reads it.
+      // (Left unwritten, the residual stream was rounded to bf16 at every sublayer and picked up whatever a guided
+      // call's backward pass had left in the plane: |E - F| 1.75-2.2x the ideal one-MMA error instead of 1.0x.)
+      if (e->chain_res_planes) p.nsplit_out = 3;
       // the fp32 copy of v1 is only ever read back as FFN2's residual source: not written when that reads the planes
       if (!e->chain_res_planes) { p.out_f32 = e->x1; p.ld_f32 = kDModel; }
       p.out_hi = e->x1_p.hi; p.out_lo = e->x1_p.lo; p.ld_bf = kDModel; p.stats_out = e->stats1;
@@ -461,7 +465,7 @@ int get_chain_tables(cmdi_engine* e, int nseq, const ChainTables** out) {
     {
       LinearParams& p = ph[2].info.p;
       p.ld_ln = kDModel; p.ln_partials = e->stats1; p.ln_gamma = w.g1; p.ln_beta = e->beta_b2[l];
-      if (e->chain_res_planes) { p.ln_src_hi = e->x1_p.hi; p.ln_src_lo = e->x1_p.lo; }
+      if (e->chain_res_planes) { p.ln_src_hi = e->x1_p.hi; p.ln_src_lo = e->x1_p.lo; p.nsplit_out = 3; }  // v2: the next out-proj's residual source
       else { p.ln_src = e->x1; p.out_f32 = e->vsum; p.ld_f32 = kDModel; }
       p.out_hi = e->xseq_p.hi; p.out_lo = e->xseq_p.lo; p.ld_bf = kDModel; p.stats_out = e->stats2;
       ph[2].o_hi = e->xseq_p.st32_hi; ph[2].o_lo = e->xseq_p.st32_lo; ph[2].o_f32 = e->vsum_st;

@@ -177,8 +177,12 @@ CMDI_API const char* cmdi_version(void);
    precision: CMDI_PRECISION_*; with CMDI_PRECISION_FP16 A, W and bias are rounded to fp16 and C holds fp16 values */
 CMDI_API int cmdi_test_linear(const float* A, const float* W, const float* bias, const float* residual, float* C, int M, int N,
                      int K, int act, int precision, int block_n, void* stream);
-/* O = softmax(Q K^T / sqrt(128)) V for `num_seqs` sequences of length S and H heads; qkv: [num_seqs*S, 3*H*128] */
+/* O = softmax(Q K^T / sqrt(128)) V for `num_seqs` sequences of length S and H heads; qkv: [num_seqs*S, 3*H*128];
+   O = hi + lo of the output planes (nsplit_out = 3) */
 CMDI_API int cmdi_test_attention(const float* qkv, float* O, int num_seqs, int S, int H, int precision, void* stream);
+/* the same launch with nsplit_out = 1, the engine's setting at CMDI_PRECISION_BF16: the kernel writes the hi plane only
+   and O is that plane */
+CMDI_API int cmdi_test_attention_hi(const float* qkv, float* O, int num_seqs, int S, int H, int precision, void* stream);
 CMDI_API int cmdi_test_layernorm(const float* v, const float* gamma, const float* beta, float* out, int rows, void* stream);
 /* one diffusion-step update on ref-layout tensors (all device): see StepParams in csrc/kernels.h */
 CMDI_API int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B, const float* model_out_c, const float* model_out_u,
@@ -193,6 +197,19 @@ CMDI_API int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, 
 /* backward pieces of reconstruction guidance (fp32 in / out) */
 CMDI_API int cmdi_test_layernorm_bwd(const float* dy, const float* v, const float* gamma, float* dv, int rows, void* stream);
 CMDI_API int cmdi_test_attention_bwd(const float* qkv, const float* dO, float* dqkv, int num_seqs, int S, int H, void* stream);
+/* cmdi_test_attention_bwd (which runs CMDI_PRECISION_BF16X3) at `precision` = CMDI_PRECISION_BF16X3 or CMDI_PRECISION_BF16,
+   the wgmma kernel's nsplit; dqkv = hi + lo of its output planes */
+CMDI_API int cmdi_test_attention_bwd_at(const float* qkv, const float* dO, float* dqkv, int num_seqs, int S, int H, int precision,
+                               void* stream);
+/* One middle encoder layer's chained launch (out-proj + residual LN2'(v2_prev) -> v1; FFN1 with norm1 folded + GELU -> h;
+ * FFN2 + residual LN1(v1) -> v2; the next layer's QKV projection with norm2 folded), phases set up as the engine sets them.
+ * in[16], fp32 device: attn [M,512], v2_prev [M,512] (the previous layer's pre-norm2 sum), prev norm2 weight, bias [512],
+ *   out_proj weight [512,512], bias, norm1 weight, bias, linear1 weight [1024,512], bias, linear2 weight [512,1024], bias,
+ *   norm2 weight, bias, next in_proj weight [1536,512], bias.
+ * out[4], fp32 device: v1 [M,512], h [M,1024], v2 [M,512], qkv [M,1536], read back from the bf16 planes the launch wrote:
+ *   v1 and v2 (residual sources) as hi + lo, h and qkv as hi + lo at CMDI_PRECISION_BF16X3 and hi at CMDI_PRECISION_BF16.
+ * Every lo plane the launch may write or read, except v2_prev's, is prefilled with bf16(stale_lo): results must not depend on it. */
+CMDI_API int cmdi_test_chain_layer(const float* const* in, float* const* out, int M, int precision, float stale_lo, void* stream);
 /* per-launch device times (ms, mean over `repeats` back-to-back launches of each kernel) of one denoiser pass at
  * `batch` (x2 sequences when cfg), in launch order:
  * token_rows, frame_embed, {qkv, attention, out_proj, ln1, ffn1, ffn2, ln2} x num_layers, out_head */
