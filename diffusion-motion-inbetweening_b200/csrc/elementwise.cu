@@ -8,6 +8,7 @@
 //                          + keyframe imputation blend                             gaussian_diffusion.py:427-435
 //   plms_step              plms_sample (pseudo linear multistep), same combine      gaussian_diffusion.py:1589-1687
 //   ddim_reverse_step      ddim_reverse_sample (DDIM inversion, eta = 0), same combine  gaussian_diffusion.py:1418-1452
+//   dpm_solver_step        DPM-Solver++ multistep (Lu et al. 2022), orders 1-3, same combine
 //   layout converters      reference [B,D,1,L] <-> frame-major [B*L, D_pad]
 //
 // The step kernel uses explicit non-contracted fp32 intrinsics (__fmul_rn/__fadd_rn) in the
@@ -421,6 +422,74 @@ __global__ void __launch_bounds__(256) ddim_reverse_step_kernel(const StepParams
     if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
   }
   advance_step(p.step_ptr, t + 1);
+}
+
+// ---------------------------------------------------------------------------------------------
+// DPM-Solver++ multistep step (Lu et al. 2022, data prediction) on frame-major state [B*L, D_pad].  One thread = 4
+// consecutive features of one frame.  m0 = x0 of the shared combine; the update is folded into four per-step
+// coefficients (host-computed in float64 for the running history), x_{s-1} = A x_s + B0 m0 + B1 m1 + B2 m2, where m1 /
+// m2 are the x0 of the previous two loop iterations.  The x0 history is a ring of three [B*L, D_pad] buffers: iteration
+// k = step_ptr[2] - s at slot k % 3, so one kernel serves every step.  No noise is drawn.  Advances s -> s - 1.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p, const DpmParams q) {
+  const int s = *p.step_ptr;
+  const int k = p.step_ptr[2] - s;                      // loop iteration since the history started
+  const int eff = min(min(q.order, k + 1), s + 1);      // effective order: lower while the history fills and at the end
+  const float4 cf = *reinterpret_cast<const float4*>(q.coef + (size_t)s * 4);  // (A, B0, B1, B2)
+  const bool do_impute = p.impute && (s >= p.stop_imputation_at);
+  const float guide_c = p.guided ? p.guide_coef[s] : 0.f;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i4 < n4) {
+    const size_t idx = i4 * 4;
+    const int c = (int)(idx % p.D_pad);
+    const int b = (int)(idx / ((size_t)p.L * p.D_pad));
+    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
+    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
+    const bool need_obs = p.guided || do_impute;
+    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
+    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
+    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
+    if (p.guided) {
+      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
+      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
+    }
+    float* cur = q.x0_hist + (size_t)(k % 3) * q.hist_stride;
+    float4 m1v = make_float4(0.f, 0.f, 0.f, 0.f), m2v = m1v;
+    if (eff >= 2) m1v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 2) % 3) * q.hist_stride + idx);  // k - 1
+    if (eff >= 3) m2v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 1) % 3) * q.hist_stride + idx);  // k - 2
+    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
+    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
+    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
+    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
+    const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w}, m2[4] = {m2v.x, m2v.y, m2v.z, m2v.w};
+    float xn4[4], x04[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float xn = 0.f, x0 = 0.f;
+      if (c + j < p.D) {
+        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
+        xn = __fadd_rn(__fmul_rn(cf.x, xtv[j]), __fmul_rn(cf.y, x0));
+        if (eff >= 2) xn = __fadd_rn(xn, __fmul_rn(cf.z, m1[j]));
+        if (eff >= 3) xn = __fadd_rn(xn, __fmul_rn(cf.w, m2[j]));
+        if (s == 0) xn = x0;  // the last step lands on abar = 1: the sample is x0 (A = 0, B0 = 1)
+      }
+      xn4[j] = xn;
+      x04[j] = x0;
+    }
+    *reinterpret_cast<float4*>(cur + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
+    uint32_t h01, l01, h23, l23;
+    split_bf16x2(xn4[0], xn4[1], h01, l01);
+    split_bf16x2(xn4[2], xn4[3], h23, l23);
+    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
+    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
+    if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+  }
+  advance_step(p.step_ptr, s - 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -842,6 +911,13 @@ cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStrea
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   return launch_kernel(plms_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+}
+
+cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cudaStream_t stream) {
+  if (q.order < 1 || q.order > 3 || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
+    return cudaErrorInvalidValue;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  return launch_kernel(dpm_solver_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream) {

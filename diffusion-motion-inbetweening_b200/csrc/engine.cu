@@ -95,7 +95,8 @@ struct GraphKey {
   float eta;
   const void* tape;
   int t0, uncond, guided, group;
-  int plms_order, plms_phase, guided2;  // PLMS: order, step kind (PlmsStep), guidance of the first step's second evaluation
+  int order, plms_phase, guided2;  // PLMS / DPM-Solver++: order; PLMS: step kind (PlmsStep), guidance of the first step's
+                                   // second evaluation
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -176,11 +177,14 @@ struct cmdi_engine {
   long long* chain_dbg = nullptr;               // CMDI_CHAIN_DBG=1: cycle counters of layer 1's chain during cmdi_profile_pass
   std::map<int, ChainTables> chain_tables;
   UnetModel* unet = nullptr;  // MDM_UNET denoiser (cfg.arch == CMDI_ARCH_UNET): engine_unet.inc
-  // PLMS (allocated by the first PLMS call): the eps history ring [3][maxB*L, D_pad] and the first step's x_t; the host
-  // side of the running history, which a `resume` call continues
-  float *plms_hist = nullptr, *plms_keep = nullptr;
-  bool plms_live = false;
-  int plms_order = 0, plms_B = 0, plms_t_start = 0, plms_steps = 0;
+  // The multistep history of PLMS (eps) and DPM-Solver++ (x0), allocated by the first such call: a ring [3][maxB*L, D_pad],
+  // and the host side of the running history, which a `resume` call continues.  PLMS also keeps its first step's x_t.
+  float *hist = nullptr, *plms_keep = nullptr;
+  bool hist_live = false;
+  int hist_sampler = 0, hist_order = 0, hist_B = 0, hist_t_start = 0, hist_steps = 0;
+  std::vector<double> h_acp;       // alphas_cumprod of the schedule (float64)
+  std::vector<float> h_dpm_coef;   // [T][4] DPM-Solver++ coefficients of the running history
+  float* dpm_coef = nullptr;       // their device copy
   std::map<GraphKey, cudaGraphExec_t> graphs;
   int64_t launches = 0;
 };
@@ -912,6 +916,7 @@ extern "C" int cmdi_engine_destroy(cmdi_engine* e) {
   if (e->tables) cudaFree(e->tables);
   if (e->d_tmap) cudaFree(e->d_tmap);
   if (e->guide_coef) cudaFree(e->guide_coef);
+  if (e->dpm_coef) cudaFree(e->dpm_coef);
   delete e;
   return 0;
 }
@@ -1072,9 +1077,13 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
     e->h_sqrt_acp[i] = std::sqrt(acp[i]);
     e->h_sqrt_1m_acp[i] = std::sqrt(1.0 - acp[i]);
   }
+  e->h_acp = acp;
   if (e->tables) cudaFree(e->tables);
   if (e->d_tmap) cudaFree(e->d_tmap);
-  e->tables = nullptr; e->d_tmap = nullptr;
+  if (e->dpm_coef) cudaFree(e->dpm_coef);
+  e->tables = nullptr; e->d_tmap = nullptr; e->dpm_coef = nullptr;
+  e->hist_live = false;  // a multistep history belongs to the schedule it started on
+  CK(cudaMalloc(&e->dpm_coef, (size_t)4 * T * 4));
   CK(cudaMalloc(&e->tables, host.size() * 4));
   CK(cudaMemcpy(e->tables, host.data(), host.size() * 4, cudaMemcpyHostToDevice));
   e->h_tmap.resize(T);
@@ -1199,6 +1208,52 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
   return 0;
 }
 
+namespace {
+
+// DPM-Solver++ multistep coefficients (Lu et al. 2022, data prediction, solver type `dpmsolver`) of a history started at
+// step index t_start, folded so that step s computes x_{s-1} = A x_s + B0 m0 + B1 m1 + B2 m2 (m0 this step's x0, m1 / m2
+// the previous two steps').  alpha = sqrt(abar), sigma = sqrt(1 - abar), lambda = log alpha - log sigma; the step at s
+// goes from abar_s = acp[s] to abar_u = acp_prev[s], h = lambda_u - lambda_s, phi1 = expm1(-h), r_j = h_j / h:
+//   order 1: x_u = (sigma_u / sigma_s) x_s - alpha_u phi1 m0                               (DDIM at eta = 0)
+//   order 2: ... - alpha_u phi1 D1_0 / 2,  D1_0 = (m0 - m1) / r0
+//   order 3: ... + alpha_u phi2 D1 - alpha_u phi3 D2,  D1_1 = (m1 - m2) / r1, D1 = D1_0 + r0 / (r0 + r1) (D1_0 - D1_1),
+//            D2 = (D1_0 - D1_1) / (r0 + r1), phi2 = phi1 / h + 1, phi3 = phi2 / h - 1/2
+// The step at s uses order min(order, k + 1, s + 1), k = t_start - s.  Float64; rows above t_start are zero.
+void dpm_solver_coefs(const std::vector<double>& acp, int t_start, int order, std::vector<float>* out) {
+  const int T = (int)acp.size();
+  out->assign((size_t)4 * T, 0.f);
+  auto lambda = [&](int i) { return std::log(std::sqrt(acp[i])) - std::log(std::sqrt(1.0 - acp[i])); };
+  for (int s = 0; s <= t_start; ++s) {
+    double A = 0.0, B0 = 1.0, B1 = 0.0, B2 = 0.0;  // s = 0 lands on abar = 1: x = m0
+    if (s > 0) {
+      const int eff = std::min(std::min(order, t_start - s + 1), s + 1);
+      const double alpha_u = std::sqrt(acp[s - 1]);
+      const double h = lambda(s - 1) - lambda(s);
+      const double phi1 = std::expm1(-h);
+      A = std::sqrt(1.0 - acp[s - 1]) / std::sqrt(1.0 - acp[s]);
+      B0 = -alpha_u * phi1;
+      if (eff == 2) {
+        const double r0 = (lambda(s) - lambda(s + 1)) / h;
+        const double c = -0.5 * alpha_u * phi1 / r0;
+        B0 += c;
+        B1 = -c;
+      } else if (eff == 3) {
+        const double r0 = (lambda(s) - lambda(s + 1)) / h, r1 = (lambda(s + 1) - lambda(s + 2)) / h;
+        const double phi2 = phi1 / h + 1.0, phi3 = phi2 / h - 0.5;
+        const double c0 = alpha_u * phi2 * (1.0 + r0 / (r0 + r1)) - alpha_u * phi3 / (r0 + r1);  // on D1_0
+        const double c1 = -alpha_u * phi2 * r0 / (r0 + r1) + alpha_u * phi3 / (r0 + r1);         // on D1_1
+        B0 += c0 / r0;
+        B1 = -c0 / r0 + c1 / r1;
+        B2 = -c1 / r1;
+      }
+    }
+    float* row = out->data() + (size_t)4 * s;
+    row[0] = (float)A; row[1] = (float)B0; row[2] = (float)B1; row[3] = (float)B2;
+  }
+}
+
+}  // namespace
+
 extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
   if (!e || !a || !out) {
     set_last_error("null argument");
@@ -1209,11 +1264,30 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int B = a->batch;
   CKI(check_ready(e, B, true));
   if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
-      a->sampler != CMDI_SAMPLER_DDIM_REVERSE) {
+      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
+  const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER;
+  const bool multistep = plms || dpm;  // samplers with a device-resident history
+  if (dpm) {
+    const char* bad = a->eta != 0.f ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
+                      : a->noise_tape ? "noise_tape (no noise is drawn after x_T)" : a->dump_xstart ? "dump_xstart"
+                      : a->plms_order ? "plms_order" : a->plms_old_eps_out ? "plms_old_eps_out"
+                      : (a->resume && a->init_image) ? "init_image (a resume call continues the running state)" : nullptr;
+    if (bad) {
+      set_last_error("CMDI_SAMPLER_DPM_SOLVER: %s must be unset", bad);
+      return 1;
+    }
+    if (a->dpm_order < 1 || a->dpm_order > 3) {
+      set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
+      return 1;
+    }
+  } else if (a->dpm_order) {
+    set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER field: it must be 0 for sampler %d", a->sampler);
+    return 1;
+  }
   // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
   // nothing and has no q_sample, dump or PLMS history
   const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
@@ -1268,23 +1342,27 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
   const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
   const int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
-  // PLMS: a call without `resume` starts a new eps history at t0; a `resume` call continues the running one
+  // PLMS / DPM-Solver++: a call without `resume` starts a new history at t0; a `resume` call continues the running one
   int hist_t0 = t0;
-  if (plms) {
+  if (multistep) {
+    const int order = plms ? a->plms_order : a->dpm_order;
     if (a->resume) {
-      if (!e->plms_live || e->plms_order != a->plms_order || e->plms_B != B || t0 != e->plms_t_start - e->plms_steps) {
-        set_last_error("PLMS resume at step %d does not continue the running history", t0);
+      if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
+          t0 != e->hist_t_start - e->hist_steps) {
+        set_last_error("%s resume at step %d does not continue the running history", plms ? "PLMS" : "DPM-Solver++", t0);
         return 1;
       }
-      hist_t0 = e->plms_t_start;
+      hist_t0 = e->hist_t_start;
     } else {
-      if (!e->plms_hist) {
-        const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
-        CKI(dev_alloc(e, &e->plms_hist, 3 * slot));
-        CKI(dev_alloc(e, &e->plms_keep, slot));
+      const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
+      if (!e->hist) CKI(dev_alloc(e, &e->hist, 3 * slot));
+      if (plms && !e->plms_keep) CKI(dev_alloc(e, &e->plms_keep, slot));
+      if (dpm) {
+        dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
+        CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
       }
-      e->plms_live = true;
-      e->plms_order = a->plms_order; e->plms_B = B; e->plms_t_start = t0; e->plms_steps = 0;
+      e->hist_live = true;
+      e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
     }
   }
   CKI(ensure_temb(e, s));
@@ -1369,7 +1447,13 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;  // first step index: step_ctr[2] (graphs do not depend on it)
     sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
     sp.pred_xstart = e->pred_x0;
-    CK(rev ? launch_ddim_reverse_step(sp, st) : launch_diffusion_step(sp, st));
+    if (dpm) {
+      DpmParams q{};
+      q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
+      CK(launch_dpm_solver_step(sp, q, st));
+    } else {
+      CK(rev ? launch_ddim_reverse_step(sp, st) : launch_diffusion_step(sp, st));
+    }
     return 0;
   };
 
@@ -1379,7 +1463,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     key.B = B; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
     key.stop_at = a->stop_imputation_at; key.tape_mode = tape != nullptr; key.has_cond = has_cond; key.eta = a->eta;
     key.tape = tape; key.t0 = 0; key.uncond = a->uncond != 0;  // the first step index lives in device memory
-    key.guided = guided; key.group = group;
+    key.guided = guided; key.group = group; key.order = a->dpm_order;
     auto it = e->graphs.find(key);
     if (it != e->graphs.end()) {
       *out_exec = it->second;
@@ -1427,7 +1511,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     sp.pred_xstart = e->pred_x0;
     PlmsParams q{};
     q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
-    q.eps_hist = e->plms_hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
+    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
     const bool guided[2] = {g1, g2};
     for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
       CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided[ev] ? &e->stash : nullptr));
@@ -1440,14 +1524,14 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   };
   auto plms_step = [&](int k) -> int {
     const int t = t0 - k;
-    const int kind = e->plms_steps + k > 0 ? kPlmsSteady : (t > 0 ? kPlmsFirst : kPlmsFirstAtZero);
+    const int kind = e->hist_steps + k > 0 ? kPlmsSteady : (t > 0 ? kPlmsFirst : kPlmsFirstAtZero);
     const bool g1 = a->recon_guidance && t >= a->stop_recguidance_at;
     const bool g2 = kind == kPlmsFirst && a->recon_guidance && t - 1 >= a->stop_recguidance_at;
     GraphKey key{};
     memset(&key, 0, sizeof(key));
     key.B = B; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
     key.stop_at = a->stop_imputation_at; key.has_cond = has_cond; key.uncond = a->uncond != 0;
-    key.guided = g1; key.group = 1; key.plms_order = a->plms_order; key.plms_phase = kind; key.guided2 = g2;
+    key.guided = g1; key.group = 1; key.order = a->plms_order; key.plms_phase = kind; key.guided2 = g2;
     const bool via_graph = a->use_graph && !e->no_graph && (nsteps >= 3 || a->use_graph >= 2 || e->graphs.count(key) != 0);
     if (via_graph) {
       auto it = e->graphs.find(key);
@@ -1498,7 +1582,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       memset(&probe, 0, sizeof(probe));
       probe.B = B; probe.cfg = a->cfg != 0; probe.sampler = a->sampler; probe.impute = a->imputate != 0;
       probe.stop_at = a->stop_imputation_at; probe.tape_mode = tape != nullptr; probe.has_cond = has_cond; probe.eta = a->eta;
-      probe.tape = tape; probe.uncond = a->uncond != 0; probe.guided = guided; probe.group = 1;
+      probe.tape = tape; probe.uncond = a->uncond != 0; probe.guided = guided; probe.group = 1; probe.order = a->dpm_order;
       via_graph = e->graphs.count(probe) != 0;
     }
     if (via_graph) {
@@ -1542,15 +1626,15 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     if (a->pred_xstart_out) CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, a->pred_xstart_out, s));
   }
   e->launches += a->pred_xstart_out ? 2 : 1;
+  if (multistep) e->hist_steps += nsteps;
   if (plms) {
-    e->plms_steps += nsteps;
     if (a->plms_old_eps_out) {
       // the reference's old_eps list after this call's last step: eps of the last min(steps, order - 1) iterations,
       // oldest first
-      const int n_hist = std::min(e->plms_steps, a->plms_order - 1);
+      const int n_hist = std::min(e->hist_steps, a->plms_order - 1);
       for (int j = 0; j < n_hist; ++j) {
-        const int it = e->plms_steps - n_hist + j;
-        const float* src = e->plms_hist + (size_t)(it % 3) * e->maxB * e->L * e->D_pad;
+        const int it = e->hist_steps - n_hist + j;
+        const float* src = e->hist + (size_t)(it % 3) * e->maxB * e->L * e->D_pad;
         float* dst = a->plms_old_eps_out + (size_t)j * n;
         CK(launch_frames_to_ref(src, B, e->D, e->L, e->D_pad, host ? e->ref_b : dst, s));
         if (host) CK(cudaMemcpyAsync(dst, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));

@@ -253,6 +253,17 @@ struct PlmsParams {
   float* x_keep;       // [B*L, D_pad] the first step's x_t, kept across its second evaluation
 };
 cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStream_t stream);
+// DPM-Solver++ multistep step (Lu et al. 2022, data prediction, solver type `dpmsolver`) from the same combine inputs as
+// StepParams (its sampler, eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are required):
+// x_{s-1} = A_s x_s + B0_s m0 + B1_s m1 + B2_s m2, m0 the x0 of this step, m1 / m2 those of the previous two.  The x0
+// history shares PLMS's ring (slot k % 3 for loop iteration k = step_ptr[2] - s); advances s -> s - 1.
+struct DpmParams {
+  int order;           // 1..3; the step at s uses min(order, k + 1, s + 1)
+  float* x0_hist;      // [3][B*L, D_pad]
+  size_t hist_stride;  // elements between slots
+  const float* coef;   // [T][4] (A, B0, B1, B2) per step index, for the running history
+};
+cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cudaStream_t stream);
 // DDIM reverse step (ddim_reverse_sample, gaussian_diffusion.py:1418-1452, eta = 0): x_t -> x_{t+1} from the same combine
 // inputs as StepParams (its sampler, eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are
 // required).  Advances the step index t -> t + 1, so one captured graph serves every step of an inversion.

@@ -4,10 +4,12 @@ Mirrors (same names, argument meaning and error behaviour; paths relative to the
     get_named_beta_schedule / betas_for_alpha_bar   diffusion/gaussian_diffusion.py:24-71
     ModelMeanType / ModelVarType / DiffusionConfig  :74-136
     GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1418-1587, :1589-1804
+                                                    + dpm_solver_sample_loop[_progressive] (DPM-Solver++, not in the reference)
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
-`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` run the WHOLE loop in one native
+`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` / `dpm_solver_sample_loop` run the
+WHOLE loop in one native
 call (`cmdi_sample`): no per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
 `p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` / `ddim_reverse_sample` is done by the CUDA
@@ -160,6 +162,7 @@ class GaussianDiffusion:
             model_kwargs = {}
         y = self._check_supported(cond_fn, const_noise, randomize_class, model_kwargs)
         plms = sampler == capi.SAMPLER_PLMS
+        dpm = sampler == capi.SAMPLER_DPM_SOLVER
         rev = sampler == capi.SAMPLER_DDIM_REVERSE  # `noise` is the state to invert; skip_timesteps its step index
         if sampler == capi.SAMPLER_DDPM:
             assert cond_fn is None, "only support the case where cond_fn is None"  # gaussian_diffusion.py:685
@@ -236,10 +239,10 @@ class GaussianDiffusion:
         if tape is not None:
             tape = tape[1:]
         seed, rng_args = 0, {}
-        if plms or rev:
+        if plms or rev or dpm:
             # plms_sample_loop_progressive draws nothing after x_T (:1767-1770): a tape contributes tape[0] only, torch's
             # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine".
-            # DDIM inversion draws nothing at all: x_T is the caller's state
+            # DPM-Solver++ behaves the same way.  DDIM inversion draws nothing at all: x_T is the caller's state
             tape = None
             if x_T is None:
                 seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -276,10 +279,10 @@ class GaussianDiffusion:
                 return self._reverse_progressive(eng, x_T, skip_timesteps, common)
             return eng.sample(skip_timesteps=skip_timesteps, num_steps=num_steps, x_T=x_T, want_pred_xstart=want_pred_xstart,
                               **common)
-        if plms:
-            common["plms_order"] = int(order)
+        if plms or dpm:
+            common["plms_order" if plms else "dpm_order"] = int(order)
             if progressive:
-                return self._plms_progressive(eng, x_T, init_image, skip_timesteps, common)
+                return self._multistep_progressive(eng, x_T, init_image, skip_timesteps, common)
             return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T, **common)
         if not progressive:
             res = eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T,
@@ -306,19 +309,24 @@ class GaussianDiffusion:
                 _advance_torch_generator(eng.device, inc)
             yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
 
-    def _plms_progressive(self, eng, x_T, init_image, skip_timesteps, common):
-        """plms_sample_loop_progressive's generator: one native call per step, each continuing the eps history the engine
-        keeps on the device, so the samples equal the fused loop's bit for bit.  old_eps holds the values of the
-        reference's history list at that yield (the reference yields one list it keeps mutating)."""
+    def _multistep_progressive(self, eng, x_T, init_image, skip_timesteps, common):
+        """The generator of the multistep samplers (PLMS, DPM-Solver++): one native call per step, each continuing the
+        history the engine keeps on the device, so the samples equal the fused loop's bit for bit.  PLMS also yields
+        old_eps, the values of the reference's history list at that yield (the reference yields one list it keeps
+        mutating)."""
         n = self.num_timesteps - skip_timesteps
         state = x_T
         common = dict(common)
         common["use_graph"] = 2 if common.get("use_graph", True) else 0
+        plms = common["sampler"] == capi.SAMPLER_PLMS
         for k in range(n):
             res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, resume=(k > 0), init_image=init_image if k == 0 else None,
-                             x_T=state, want_pred_xstart=True, want_old_eps=True, **common)
+                             x_T=state, want_pred_xstart=True, want_old_eps=plms, **common)
             state = res["sample"]
-            yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"], "old_eps": res["old_eps"]}
+            step = {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
+            if plms:
+                step["old_eps"] = res["old_eps"]
+            yield step
 
     def _reverse_progressive(self, eng, x_start, skip_timesteps, common):
         """DDIM inversion as a generator: one native call per step (the step graph is shared), each starting from the
@@ -388,6 +396,28 @@ class GaussianDiffusion:
         return self._run(capi.SAMPLER_PLMS, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image,
                          randomize_class, None, False, 0.0, progressive=True, order=order)
 
+    def dpm_solver_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                               model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                               randomize_class=False, cond_fn_with_grad=False, order=2):
+        """DPM-Solver++ multistep (Lu et al. 2022, data prediction) on this object's spaced steps, orders 1-3: one
+        denoiser pass per step, through the same x0 pipeline as DDIM (CFG, keyframe input, imputation, reconstruction
+        guidance).  Order 1 is DDIM at eta = 0.  Deterministic after x_T; the whole loop is one native call and the x0
+        history stays on the device.  (The reference has no such sampler.)"""
+        _check_dpm_order(order)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DPM_SOLVER, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, False, 0.0, order=order)["sample"]
+
+    def dpm_solver_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                           cond_fn=None, model_kwargs=None, device=None, progress=False, skip_timesteps=0,
+                                           init_image=None, randomize_class=False, cond_fn_with_grad=False, order=2):
+        """Yields {"sample", "pred_xstart"} per step of dpm_solver_sample_loop, one native call per step; the samples
+        equal the fused loop's bit for bit.  The configuration is validated at the call."""
+        _check_dpm_order(order)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DPM_SOLVER, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, False, 0.0, progressive=True, order=order)
+
     def ddim_reverse_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
         """gaussian_diffusion.py:1418-1452: x_t -> x_{t+1} by the reverse DDIM ODE, one native call.  Returns
         {"sample", "pred_xstart"}.  `t` must hold one step index for the whole batch (the engine's step index is per
@@ -436,6 +466,12 @@ def _check_plms_order(order) -> None:
         raise NotImplementedError(f"PLMS order {order!r} is not an integer")
     if int(order) == 1:
         raise TypeError("PLMS order 1 fails on the reference's first step ('NoneType' object is not subscriptable)")
+
+
+def _check_dpm_order(order) -> None:
+    """DPM-Solver++'s multistep orders are 1, 2 and 3 (an int; bools and floats are refused)."""
+    if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2, 3):
+        raise ValueError(f"DPM-Solver++ order must be an int in {{1, 2, 3}}, got {order!r}")
 
 
 def space_timesteps(num_timesteps, section_counts):

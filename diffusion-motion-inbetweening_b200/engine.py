@@ -123,7 +123,8 @@ class Engine:
                recon_guidance: bool = False, stop_recguidance_at: int = 0, recon_coef: Optional[Sequence[float]] = None,
                want_pred_xstart: bool = False, dump_steps: Optional[Sequence[int]] = None, host_buffers: bool = False,
                use_graph: bool = True, out: Optional[torch.Tensor] = None, obs_x0: Optional[torch.Tensor] = None,
-               obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False):
+               obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False,
+               dpm_order: int = 2):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -133,6 +134,8 @@ class Engine:
         list after the last step (oldest first), as plms_sample_loop_progressive yields it.
         sampler=SAMPLER_DDIM_REVERSE: DDIM inversion from the state x_T, ascending from t = skip_timesteps; plms_order
         is not sent.
+        sampler=SAMPLER_DPM_SOLVER: DPM-Solver++ multistep of order `dpm_order` (1-3); resume continues its x0 history.
+        dpm_order is sent for this sampler only, plms_order for the others.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         dev = torch.device("cpu") if host_buffers else self.device
@@ -193,7 +196,8 @@ class Engine:
                             _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
                             dump_arr, n_dump, int(host_buffers),
                             int(use_graph), _ptr(obs_x0), _ptr(obs_mask),
-                            0 if sampler == capi.SAMPLER_DDIM_REVERSE else int(plms_order), _ptr(old_eps))
+                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_DPM_SOLVER) else int(plms_order),
+                            _ptr(old_eps), int(dpm_order) if sampler == capi.SAMPLER_DPM_SOLVER else 0)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")

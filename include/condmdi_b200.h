@@ -59,7 +59,13 @@ enum {
    x_T is the start state (e.g. x_0) and is required; num_steps as for the other samplers (0 = up to t = T - 1).
    eta must be 0 and noise_tape, init_image, dump_xstart, plms_order and plms_old_eps_out unset: the call fails
    naming the field otherwise.  pred_xstart_out receives the last step's x0. */
-enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3 };
+/* DPM_SOLVER: DPM-Solver++ multistep (Lu et al. 2022; data prediction, solver type `dpmsolver`) on the spaced steps,
+   orders 1..3 (dpm_order), one denoiser pass per step.  Deterministic after x_T; the step at s uses order
+   min(dpm_order, iterations since the history started + 1, s + 1), and the last step returns x0 as DDIM's does.
+   skip_timesteps / init_image / resume as for DDIM (init_image only on a call that starts a history); eta must be 0 and
+   noise_tape, dump_xstart, plms_order and plms_old_eps_out unset: the call fails naming the field otherwise. */
+enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3,
+       CMDI_SAMPLER_DPM_SOLVER = 4 };
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
 
@@ -158,6 +164,9 @@ typedef struct {
   int32_t plms_order;           /* 2..4 (plms_sample's `order`) */
   float* plms_old_eps_out;      /* NULL, or (min(steps so far, plms_order - 1), B, 263, 1, 196): the reference's old_eps
                                    list after the last step, oldest first (ref layout) */
+  /* CMDI_SAMPLER_DPM_SOLVER only (0 for every other sampler).  The x0 history stays on the device like PLMS's eps
+     history: resume = 1 continues it with the same order and batch. */
+  int32_t dpm_order;            /* 1..3 */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
