@@ -228,6 +228,50 @@ __device__ __forceinline__ float step_x0(float mo, float mu, float ob, unsigned 
   return out;
 }
 
+// x_t and x0 (step_x0) of the 4 consecutive features at idx, the frame-major offset of feature c of a frame of sample
+// b, for the evaluation at step index t_eval.  Operands are read with 16-byte loads, each under the predicate that
+// makes it meaningful: an unguided, un-imputed step never touches x_obs / obs_mask / guide_grad, and only a CFG step
+// reads the uncond half.  Padding features (c + j >= D) get x0 = 0.
+__device__ __forceinline__ void load_step_x0(const StepParams& p, size_t idx, int b, int c, int t_eval, float xt[4], float x0[4]) {
+  const bool do_impute = p.impute && (t_eval >= p.stop_imputation_at);
+  const float guide_c = p.guided ? p.guide_coef[t_eval] : 0.f;
+  const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
+  const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
+  const bool need_obs = p.guided || do_impute;
+  const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
+  const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+  const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
+  float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
+  if (p.guided) {
+    gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
+    if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
+  }
+  const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
+  const float ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
+  const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
+  const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
+  xt[0] = xt4.x; xt[1] = xt4.y; xt[2] = xt4.z; xt[3] = xt4.w;
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    x0[j] = c + j < p.D ? step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c) : 0.f;
+}
+
+// Stores the state after a step for the 4 features at idx: x_next as fp32 and as bf16 planes (hi, and lo where the
+// engine keeps split operands), and pred_xstart.  x_next is null for the pass-through evaluation (sampler 2).
+__device__ __forceinline__ void store_step_state(const StepParams& p, size_t idx, const float xn[4], const float x0[4], bool write_pred) {
+  if (p.x_next) {
+    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn[0], xn[1], xn[2], xn[3]);
+    uint32_t h01, l01, h23, l23;
+    split_bf16x2(xn[0], xn[1], h01, l01);
+    split_bf16x2(xn[2], xn[3], h23, l23);
+    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
+    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
+  }
+  if (p.pred_xstart && write_pred) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x0[0], x0[1], x0[2], x0[3]);
+}
+
 // Bumps the block-arrival counter at step_ptr[1]; the last block to arrive stores `next` as the step index (every
 // block has read the old one by then).
 __device__ __forceinline__ void advance_step(int* step_ptr, int next) {
@@ -266,27 +310,12 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, cons
   const float r1 = p.tab.sqrt_recip_acp[t], r2 = p.tab.sqrt_recipm1_acp[t];
   const float abp = p.tab.acp_prev[t];
   const float sq_abp = sqrtf(abp), sq_1m_abp = sqrtf(__fsub_rn(1.0f, abp));
-  const bool do_impute = p.impute && (t_eval >= p.stop_imputation_at);
-  const float guide_c = p.guided ? p.guide_coef[t_eval] : 0.f;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 < n4) {
     const size_t idx = i4 * 4;
     const int c = (int)(idx % p.D_pad);
     const int b = (int)(idx / ((size_t)p.L * p.D_pad));
-    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
-    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
-    const bool need_obs = p.guided || do_impute;
-    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
-    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
-    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
-    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
-    if (p.guided) {
-      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
-      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
-    }
     float* slot0 = q.eps_hist;
     float* cur = q.eps_hist + (size_t)(k % 3) * q.hist_stride;
     const float* h2 = q.eps_hist + (size_t)((k + 2) % 3) * q.hist_stride;  // iteration k - 1
@@ -301,18 +330,15 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, cons
       e2v = *reinterpret_cast<const float4*>(slot0 + idx);  // eps_0
       xkv = *reinterpret_cast<const float4*>(q.x_keep + idx);
     }
-    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
-    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
-    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
-    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
     const float e2[4] = {e2v.x, e2v.y, e2v.z, e2v.w}, e3[4] = {e3v.x, e3v.y, e3v.z, e3v.w}, e4[4] = {e4v.x, e4v.y, e4v.z, e4v.w};
     const float xk[4] = {xkv.x, xkv.y, xkv.z, xkv.w};
-    float xn4[4], x04[4], ep4[4];
+    float xtv[4], x04[4], xn4[4], ep4[4];
+    load_step_x0(p, idx, b, c, t_eval, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float xn = 0.f, x0 = 0.f, eps = 0.f;
+      const float x0 = x04[j];
+      float xn = 0.f, eps = 0.f;
       if (c + j < p.D) {
-        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
         // _predict_eps_from_xstart at the evaluation's (x, t) (:551-555)
         eps = __fdiv_rn(__fsub_rn(__fmul_rn(r1e, xtv[j]), x0), r2e);
         float ep, x;
@@ -344,22 +370,14 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, cons
         }
       }
       xn4[j] = xn;
-      x04[j] = x0;
       ep4[j] = eps;
     }
     if (q.phase == 0) *reinterpret_cast<float4*>(cur + idx) = make_float4(ep4[0], ep4[1], ep4[2], ep4[3]);
     if (q.phase == 1) {
       *reinterpret_cast<float4*>(slot0 + idx) = make_float4(ep4[0], ep4[1], ep4[2], ep4[3]);
-      *reinterpret_cast<float4*>(q.x_keep + idx) = xt4;
+      *reinterpret_cast<float4*>(q.x_keep + idx) = make_float4(xtv[0], xtv[1], xtv[2], xtv[3]);
     }
-    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
-    uint32_t h01, l01, h23, l23;
-    split_bf16x2(xn4[0], xn4[1], h01, l01);
-    split_bf16x2(xn4[2], xn4[3], h23, l23);
-    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
-    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
-    // pred_xstart is the FIRST evaluation's x0 (:1685)
-    if (p.pred_xstart && q.phase != 2) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+    store_step_state(p, idx, xn4, x04, q.phase != 2);  // pred_xstart is the FIRST evaluation's x0 (:1685)
   }
   if (q.phase != 2) advance_step(p.step_ptr, t - 1);
 }
@@ -374,52 +392,27 @@ __global__ void __launch_bounds__(256) ddim_reverse_step_kernel(const StepParams
   const float r1 = p.tab.sqrt_recip_acp[t], r2 = p.tab.sqrt_recipm1_acp[t];
   const float abn = p.tab.acp_next[t];  // _extract_into_tensor(alphas_cumprod_next, t).float() (:1445-1446)
   const float sq_abn = sqrtf(abn), sq_1m_abn = sqrtf(__fsub_rn(1.0f, abn));
-  const bool do_impute = p.impute && (t >= p.stop_imputation_at);
-  const float guide_c = p.guided ? p.guide_coef[t] : 0.f;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 < n4) {
     const size_t idx = i4 * 4;
     const int c = (int)(idx % p.D_pad);
     const int b = (int)(idx / ((size_t)p.L * p.D_pad));
-    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
-    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
-    const bool need_obs = p.guided || do_impute;
-    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
-    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
-    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
-    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
-    if (p.guided) {
-      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
-      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
-    }
-    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
-    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
-    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
-    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
-    float xn4[4], x04[4];
+    float xtv[4], x04[4], xn4[4];
+    load_step_x0(p, idx, b, c, t, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float xn = 0.f, x0 = 0.f;
+      const float x0 = x04[j];
+      float xn = 0.f;
       if (c + j < p.D) {
-        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
         // eps = (sqrt_recip_acp[t] x - x0) / sqrt_recipm1_acp[t] (:1442-1444);
         // mean_pred = x0 sqrt(ab_next) + sqrt(1 - ab_next) eps (:1449-1450)
         const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(r1, xtv[j]), x0), r2);
         xn = __fadd_rn(__fmul_rn(x0, sq_abn), __fmul_rn(sq_1m_abn, eps));
       }
       xn4[j] = xn;
-      x04[j] = x0;
     }
-    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
-    uint32_t h01, l01, h23, l23;
-    split_bf16x2(xn4[0], xn4[1], h01, l01);
-    split_bf16x2(xn4[2], xn4[3], h23, l23);
-    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
-    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
-    if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+    store_step_state(p, idx, xn4, x04, true);
   }
   advance_step(p.step_ptr, t + 1);
 }
@@ -436,58 +429,33 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p
   const int k = p.step_ptr[2] - s;                      // loop iteration since the history started
   const int eff = min(min(q.order, k + 1), s + 1);      // effective order: lower while the history fills and at the end
   const float4 cf = *reinterpret_cast<const float4*>(q.coef + (size_t)s * 4);  // (A, B0, B1, B2)
-  const bool do_impute = p.impute && (s >= p.stop_imputation_at);
-  const float guide_c = p.guided ? p.guide_coef[s] : 0.f;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i4 < n4) {
     const size_t idx = i4 * 4;
     const int c = (int)(idx % p.D_pad);
     const int b = (int)(idx / ((size_t)p.L * p.D_pad));
-    const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
-    const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
-    const bool need_obs = p.guided || do_impute;
-    const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
-    const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
-    const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
-    float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
-    if (p.guided) {
-      gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
-      if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
-    }
     float* cur = q.x0_hist + (size_t)(k % 3) * q.hist_stride;
     float4 m1v = make_float4(0.f, 0.f, 0.f, 0.f), m2v = m1v;
     if (eff >= 2) m1v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 2) % 3) * q.hist_stride + idx);  // k - 1
     if (eff >= 3) m2v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 1) % 3) * q.hist_stride + idx);  // k - 2
-    const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
-    const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
-    const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
-    const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
     const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w}, m2[4] = {m2v.x, m2v.y, m2v.z, m2v.w};
-    float xn4[4], x04[4];
+    float xtv[4], x04[4], xn4[4];
+    load_step_x0(p, idx, b, c, s, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float xn = 0.f, x0 = 0.f;
+      const float x0 = x04[j];
+      float xn = 0.f;
       if (c + j < p.D) {
-        x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
         xn = __fadd_rn(__fmul_rn(cf.x, xtv[j]), __fmul_rn(cf.y, x0));
         if (eff >= 2) xn = __fadd_rn(xn, __fmul_rn(cf.z, m1[j]));
         if (eff >= 3) xn = __fadd_rn(xn, __fmul_rn(cf.w, m2[j]));
         if (s == 0) xn = x0;  // the last step lands on abar = 1: the sample is x0 (A = 0, B0 = 1)
       }
       xn4[j] = xn;
-      x04[j] = x0;
     }
     *reinterpret_cast<float4*>(cur + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
-    *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
-    uint32_t h01, l01, h23, l23;
-    split_bf16x2(xn4[0], xn4[1], h01, l01);
-    split_bf16x2(xn4[2], xn4[3], h23, l23);
-    *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
-    if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
-    if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+    store_step_state(p, idx, xn4, x04, true);
   }
   advance_step(p.step_ptr, s - 1);
 }
@@ -553,8 +521,6 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
   const float coef1 = p.sampler == 0 ? p.tab.post_coef1[t] : 0.f, coef2 = p.sampler == 0 ? p.tab.post_coef2[t] : 0.f;
   const float logvar = p.sampler == 0 ? p.tab.post_logvar[t] : 0.f;
   const float nonzero = (t != 0) ? 1.0f : 0.0f;
-  const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
-  const bool do_impute = p.impute && (t >= p.stop_imputation_at);
 
   // one thread = 4 consecutive features of one frame (16-byte accesses; D_pad is a multiple of 8)
   {
@@ -563,29 +529,13 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
     const int l = l0 + ll, c = c0 + cq;
     if (l < p.L && c < p.D_pad) {
       const size_t idx = ((size_t)b * p.L + l) * p.D_pad + c;
-      const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
-      const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
-      const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-      const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
-      const bool need_obs = p.guided || do_impute;
-      const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
-      const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
-      float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
-      if (p.guided) {
-        gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
-        if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
-      }
-      const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
-      const float xtv[4] = {xt4.x, xt4.y, xt4.z, xt4.w}, ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
-      const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
-      const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
-      const float guide_c = p.guided ? p.guide_coef[t] : 0.f;
-      float xn4[4], x04[4];
+      float xtv[4], x04[4], xn4[4];
+      load_step_x0(p, idx, b, c, t, xtv, x04);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        float xn = 0.f, x0 = 0.f;
+        const float x0 = x04[j];
+        float xn = 0.f;
         if (c + j < p.D) {
-          x0 = step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c);
           const float xt = xtv[j];
           const float noise = s_noise[cq + j][ll];
           if (p.sampler == 2) {
@@ -608,36 +558,12 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
           }
         }
         xn4[j] = xn;
-        x04[j] = x0;
       }
-      if (p.x_next) {
-        *reinterpret_cast<float4*>(p.x_next + idx) = make_float4(xn4[0], xn4[1], xn4[2], xn4[3]);
-        uint32_t h01, l01, h23, l23;
-        split_bf16x2(xn4[0], xn4[1], h01, l01);
-        split_bf16x2(xn4[2], xn4[3], h23, l23);
-        *reinterpret_cast<uint2*>(p.x_next_hi + idx) = make_uint2(h01, h23);
-        if (p.x_next_lo) *reinterpret_cast<uint2*>(p.x_next_lo + idx) = make_uint2(l01, l23);
-      }
-      if (p.pred_xstart) *reinterpret_cast<float4*>(p.pred_xstart + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+      store_step_state(p, idx, xn4, x04, true);
     }
   }
 
-  // ---- advance the device-side step counter once every block has read it ----
-  if (p.advance) {
-    __shared__ bool is_last;
-    __threadfence();
-    __syncthreads();
-    if (tx == 0 && ty == 0) {
-      const unsigned int total = gridDim.x * gridDim.y * gridDim.z;
-      unsigned int* counter = reinterpret_cast<unsigned int*>(p.step_ptr + 1);
-      const unsigned int prev = atomicAdd(counter, 1u);
-      is_last = (prev == total - 1);
-      if (is_last) {
-        *counter = 0;
-        *p.step_ptr = t - 1;
-      }
-    }
-  }
+  if (p.advance) advance_step(p.step_ptr, t - 1);
 }
 
 // ---------------------------------------------------------------------------------------------

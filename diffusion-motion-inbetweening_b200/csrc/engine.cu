@@ -1252,6 +1252,105 @@ void dpm_solver_coefs(const std::vector<double>& acp, int t_start, int order, st
   }
 }
 
+// The first argument the deterministic samplers (DPM-Solver++, DDIM inversion) have no use for but the caller set, or null.
+const char* field_to_unset(const cmdi_sample_args* a) {
+  const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER, rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
+  if (!dpm && !rev) return nullptr;
+  if (a->eta != 0.f)
+    return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)" : "eta (the reverse ODE is deterministic: eta must be 0)";
+  if (a->noise_tape) return dpm ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
+  if (rev && a->init_image) return "init_image";
+  if (a->dump_xstart) return "dump_xstart";
+  if (a->plms_order) return "plms_order";
+  if (a->plms_old_eps_out) return "plms_old_eps_out";
+  if (dpm && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
+  return nullptr;
+}
+
+// Kernel launches of one evaluation of a sampling step: the denoiser pass, a guided one's backward pass, the step kernel.
+int launches_per_eval(const cmdi_engine* e, bool guided) {
+  return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) : 0);
+}
+
+// What every sampler's step kernel reads and writes: the schedule, the device step counter, the combine inputs (model
+// output, CFG scale, keyframes, guidance gradient) and the state it advances in place.
+StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool guided) {
+  StepParams sp{};
+  sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.B = a->batch; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
+  sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
+  sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
+  sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
+  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
+  sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
+  sp.pred_xstart = e->pred_x0;
+  return sp;
+}
+
+// The step kinds of PLMS (gaussian_diffusion.py:1589-1804).  The first step of a history is the pseudo improved Euler
+// step: evaluation at t, plms_step_kernel phase 1, evaluation at t - 1 (its guidance and imputation predicates tested at
+// t - 1), phase 2; at t = 0 the second evaluation cannot change the result (sample = x0) and is skipped.  Every later
+// step is one evaluation and one Adams-Bashforth kernel.
+enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
+
+// The graph of `group` consecutive steps of this call's configuration with guidance `guided`; for PLMS, of one step of
+// kind `plms_kind` whose second evaluation has guidance `guided2` (both 0 for the other samplers).  The first step index
+// lives in device memory, so t0 stays 0.  PLMS draws no noise: its key leaves eta and the tape at zero.
+// GraphKey is ordered by memcmp and has padding bytes, so the whole struct is zeroed before it is filled.
+GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int plms_kind, bool guided2) {
+  const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
+  GraphKey key;
+  memset(&key, 0, sizeof(key));
+  key.B = a->batch; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
+  key.stop_at = a->stop_imputation_at; key.has_cond = a->cond_emb != nullptr; key.uncond = a->uncond != 0;
+  key.guided = guided; key.group = group; key.order = plms ? a->plms_order : a->dpm_order;
+  if (!plms) {
+    key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
+  }
+  key.plms_phase = plms_kind; key.guided2 = guided2;
+  return key;
+}
+
+// use_graph 1: calls of one or two steps are launched directly unless a step graph of this configuration already exists
+// (capturing and instantiating one costs more than it saves there); use_graph 2 (the *_progressive generators: one
+// native call per step, many calls): always through the step graph.  A noise tape (a test aid) is addressed through a
+// kernel argument: per-step calls with a moving tape pointer would capture a new graph every step, so they are
+// launched directly.
+bool step_uses_graph(int use_graph, bool no_graph, int nsteps, const float* tape, bool key_exists) {
+  return use_graph && !no_graph && (nsteps >= 3 || (use_graph >= 2 && !tape) || key_exists);
+}
+
+// The executable graph of `key`: the cached one, or what `enqueue(stream)` issues, captured on a private stream (so a
+// caller's legacy / default stream is never put into capture mode), instantiated and cached.
+template <class Enqueue>
+int capture_step_graph(cmdi_engine* e, const GraphKey& key, Enqueue enqueue, cudaGraphExec_t* out_exec) {
+  auto it = e->graphs.find(key);
+  if (it != e->graphs.end()) {
+    *out_exec = it->second;
+    return 0;
+  }
+  cudaStream_t cs = nullptr;
+  CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t ex = nullptr;
+  int erc = 0;
+  cudaError_t ce = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
+  if (ce == cudaSuccess) {
+    erc = enqueue(cs);
+    ce = cudaStreamEndCapture(cs, &graph);  // also when enqueueing failed: the stream must leave capture mode
+    if (!erc && ce == cudaSuccess) ce = cudaGraphInstantiate(&ex, graph, 0);
+  }
+  if (graph) cudaGraphDestroy(graph);
+  cudaStreamDestroy(cs);
+  if (erc) return 1;  // enqueue has set the error
+  if (ce != cudaSuccess) {
+    set_last_error("capturing or instantiating a step graph failed: %s", cudaGetErrorString(ce));
+    return 1;
+  }
+  e->graphs[key] = ex;
+  *out_exec = ex;
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
@@ -1271,38 +1370,24 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER;
   const bool multistep = plms || dpm;  // samplers with a device-resident history
-  if (dpm) {
-    const char* bad = a->eta != 0.f ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
-                      : a->noise_tape ? "noise_tape (no noise is drawn after x_T)" : a->dump_xstart ? "dump_xstart"
-                      : a->plms_order ? "plms_order" : a->plms_old_eps_out ? "plms_old_eps_out"
-                      : (a->resume && a->init_image) ? "init_image (a resume call continues the running state)" : nullptr;
-    if (bad) {
-      set_last_error("CMDI_SAMPLER_DPM_SOLVER: %s must be unset", bad);
-      return 1;
-    }
-    if (a->dpm_order < 1 || a->dpm_order > 3) {
-      set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
-      return 1;
-    }
-  } else if (a->dpm_order) {
-    set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER field: it must be 0 for sampler %d", a->sampler);
-    return 1;
-  }
   // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
   // nothing and has no q_sample, dump or PLMS history
   const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  if (rev) {
-    const char* bad = a->eta != 0.f ? "eta (the reverse ODE is deterministic: eta must be 0)"
-                      : a->noise_tape ? "noise_tape" : a->init_image ? "init_image" : a->dump_xstart ? "dump_xstart"
-                      : a->plms_order ? "plms_order" : a->plms_old_eps_out ? "plms_old_eps_out" : nullptr;
-    if (bad) {
-      set_last_error("CMDI_SAMPLER_DDIM_REVERSE: %s must be unset", bad);
-      return 1;
-    }
-    if (!a->x_T) {
-      set_last_error("CMDI_SAMPLER_DDIM_REVERSE needs x_T, the state to invert");
-      return 1;
-    }
+  if (!dpm && a->dpm_order) {
+    set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER field: it must be 0 for sampler %d", a->sampler);
+    return 1;
+  }
+  if (const char* bad = field_to_unset(a)) {
+    set_last_error("%s: %s must be unset", dpm ? "CMDI_SAMPLER_DPM_SOLVER" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+    return 1;
+  }
+  if (dpm && (a->dpm_order < 1 || a->dpm_order > 3)) {
+    set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
+    return 1;
+  }
+  if (rev && !a->x_T) {
+    set_last_error("CMDI_SAMPLER_DDIM_REVERSE needs x_T, the state to invert");
+    return 1;
   }
   if (plms && (a->plms_order < 2 || a->plms_order > 4)) {
     set_last_error("plms_order %d outside [2, 4]", a->plms_order);
@@ -1434,19 +1519,17 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     return 1;
   }
   const bool has_cond = a->cond_emb != nullptr;
-  auto enqueue_step = [&](cudaStream_t st, bool guided) -> int {
-    CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1,
-                     guided ? &e->stash : nullptr));
+  // one evaluation: the denoiser pass and, for a guided one, its backward pass
+  auto enqueue_eval = [&](cudaStream_t st, bool guided) -> int {
+    CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
     if (guided) CKI(run_backward(e, B, a->cfg != 0, st));
-    StepParams sp{};
-    sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.advance = 1; sp.B = B; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
-    sp.sampler = a->sampler; sp.eta = a->eta; sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
-    sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
-    sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
-    sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
+    return 0;
+  };
+  auto enqueue_step = [&](cudaStream_t st, bool guided) -> int {
+    CKI(enqueue_eval(st, guided));
+    StepParams sp = step_params(e, a, guided);
+    sp.advance = 1; sp.sampler = a->sampler; sp.eta = a->eta;
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;  // first step index: step_ctr[2] (graphs do not depend on it)
-    sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
-    sp.pred_xstart = e->pred_x0;
     if (dpm) {
       DpmParams q{};
       q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
@@ -1456,35 +1539,17 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     }
     return 0;
   };
-
-  auto get_exec = [&](bool guided, int group, cudaGraphExec_t* out_exec) -> int {
-    GraphKey key{};
-    memset(&key, 0, sizeof(key));
-    key.B = B; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
-    key.stop_at = a->stop_imputation_at; key.tape_mode = tape != nullptr; key.has_cond = has_cond; key.eta = a->eta;
-    key.tape = tape; key.t0 = 0; key.uncond = a->uncond != 0;  // the first step index lives in device memory
-    key.guided = guided; key.group = group; key.order = a->dpm_order;
-    auto it = e->graphs.find(key);
-    if (it != e->graphs.end()) {
-      *out_exec = it->second;
-      return 0;
+  // one PLMS step of `kind` (PlmsStep): g1 / g2 = guidance of its first / second evaluation
+  auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
+    PlmsParams q{};
+    q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
+    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
+    const bool guided[2] = {g1, g2};
+    for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
+      CKI(enqueue_eval(st, guided[ev]));
+      if (ev == 1) q.phase = 2;
+      CK(launch_plms_step(step_params(e, a, guided[ev]), q, st));
     }
-    // capture on a private stream so a caller's legacy/default stream is never put into capture mode
-    cudaStream_t cs = nullptr;
-    CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-    cudaGraph_t graph = nullptr;
-    CK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    int erc = 0;
-    for (int g = 0; g < group && !erc; ++g) erc = enqueue_step(cs, guided);
-    cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-    cudaStreamDestroy(cs);
-    if (erc) return 1;
-    CK(ce);
-    cudaGraphExec_t ex = nullptr;
-    CK(cudaGraphInstantiate(&ex, graph, 0));
-    cudaGraphDestroy(graph);
-    e->graphs[key] = ex;
-    *out_exec = ex;
     return 0;
   };
   if (e->graphs.size() > 16) {  // bounded cache; cleared before this call takes any handle out of it
@@ -1492,113 +1557,36 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     e->graphs.clear();
   }
   // graphs of `group` consecutive steps (one launch replays that many steps: the per-launch cost of a graph is paid
-  // once per group); single-step graphs serve the remainder and the steps whose pred_xstart is dumped
-  const int group = e->steps_per_graph > 1 ? e->steps_per_graph : 1;
-  cudaGraphExec_t exec1[2] = {nullptr, nullptr}, execg[2] = {nullptr, nullptr};  // [guided]
-
-  // ---- PLMS (gaussian_diffusion.py:1589-1804) ----
-  // The first step of a history is the pseudo improved Euler step: evaluation at t, plms_step_kernel phase 1, evaluation
-  // at t - 1 (its guidance and imputation predicates tested at t - 1), phase 2; at t = 0 the second evaluation cannot
-  // change the result (sample = x0) and is skipped.  Every later step is one evaluation and one Adams-Bashforth kernel.
-  enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
-  auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
-    StepParams sp{};
-    sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.B = B; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
-    sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
-    sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
-    sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
-    sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
-    sp.pred_xstart = e->pred_x0;
-    PlmsParams q{};
-    q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
-    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
-    const bool guided[2] = {g1, g2};
-    for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
-      CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided[ev] ? &e->stash : nullptr));
-      if (guided[ev]) CKI(run_backward(e, B, a->cfg != 0, st));
-      sp.guided = guided[ev];
-      if (ev == 1) q.phase = 2;
-      CK(launch_plms_step(sp, q, st));
-    }
-    return 0;
-  };
-  auto plms_step = [&](int k) -> int {
-    const int t = t0 - k;
-    const int kind = e->hist_steps + k > 0 ? kPlmsSteady : (t > 0 ? kPlmsFirst : kPlmsFirstAtZero);
-    const bool g1 = a->recon_guidance && t >= a->stop_recguidance_at;
-    const bool g2 = kind == kPlmsFirst && a->recon_guidance && t - 1 >= a->stop_recguidance_at;
-    GraphKey key{};
-    memset(&key, 0, sizeof(key));
-    key.B = B; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
-    key.stop_at = a->stop_imputation_at; key.has_cond = has_cond; key.uncond = a->uncond != 0;
-    key.guided = g1; key.group = 1; key.order = a->plms_order; key.plms_phase = kind; key.guided2 = g2;
-    const bool via_graph = a->use_graph && !e->no_graph && (nsteps >= 3 || a->use_graph >= 2 || e->graphs.count(key) != 0);
-    if (via_graph) {
-      auto it = e->graphs.find(key);
-      if (it == e->graphs.end()) {
-        cudaStream_t cs = nullptr;
-        CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t graph = nullptr;
-        CK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-        const int erc = enqueue_plms(cs, kind, g1, g2);
-        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-        cudaStreamDestroy(cs);
-        if (erc) return 1;
-        CK(ce);
-        cudaGraphExec_t ex = nullptr;
-        CK(cudaGraphInstantiate(&ex, graph, 0));
-        cudaGraphDestroy(graph);
-        it = e->graphs.emplace(key, ex).first;
-      }
-      CK(cudaGraphLaunch(it->second, s));
-    } else {
-      CKI(enqueue_plms(s, kind, g1, g2));
-    }
-    const int per_eval = launches_per_pass(e, g1) + 1 + (g1 ? launches_per_backward(e) : 0);
-    e->launches += per_eval;
-    if (kind == kPlmsFirst) e->launches += launches_per_pass(e, g2) + 1 + (g2 ? launches_per_backward(e) : 0);
-    return 0;
-  };
+  // once per group); single-step graphs serve the remainder and the steps whose pred_xstart is dumped.  A PLMS graph
+  // is one step.
+  const int group = !plms && e->steps_per_graph > 1 ? e->steps_per_graph : 1;
 
   int dump_i = 0;
+  // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
   auto guided_at = [&](int k) { return a->recon_guidance && (rev ? t0 + k : t0 - k) >= a->stop_recguidance_at; };
   for (int k = 0; k < nsteps;) {
-    if (plms) {
-      CKI(plms_step(k));
-      ++k;
-      continue;
-    }
-    // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
     const bool guided = guided_at(k);
+    // PLMS: the kind of this step and the guidance of a first step's second evaluation, at t - 1
+    const int kind = !plms || e->hist_steps + k > 0 ? kPlmsSteady : (t0 - k > 0 ? kPlmsFirst : kPlmsFirstAtZero);
+    const bool guided2 = kind == kPlmsFirst && guided_at(k + 1);
+    auto enqueue = [&](cudaStream_t st, int steps) -> int {
+      if (plms) return enqueue_plms(st, kind, guided, guided2);
+      for (int g = 0; g < steps; ++g) CKI(enqueue_step(st, guided));
+      return 0;
+    };
     int run = 1;
-    // use_graph 1: calls of one or two steps are launched directly unless a step graph of this configuration already
-    // exists (capturing and instantiating one costs more than it saves there); use_graph 2 (the *_progressive
-    // generators: one native call per step, many calls): always through the step graph
-    // (a noise tape -- test aid -- is addressed through a kernel argument: per-step calls with a moving tape pointer
-    //  would capture a new graph every step, so they are launched directly)
-    bool via_graph = a->use_graph && !e->no_graph && (nsteps >= 3 || (a->use_graph >= 2 && !tape));
-    if (a->use_graph && !e->no_graph && !via_graph) {
-      GraphKey probe{};
-      memset(&probe, 0, sizeof(probe));
-      probe.B = B; probe.cfg = a->cfg != 0; probe.sampler = a->sampler; probe.impute = a->imputate != 0;
-      probe.stop_at = a->stop_imputation_at; probe.tape_mode = tape != nullptr; probe.has_cond = has_cond; probe.eta = a->eta;
-      probe.tape = tape; probe.uncond = a->uncond != 0; probe.guided = guided; probe.group = 1; probe.order = a->dpm_order;
-      via_graph = e->graphs.count(probe) != 0;
-    }
-    if (via_graph) {
+    GraphKey key = step_graph_key(a, guided, 1, kind, guided2);
+    if (step_uses_graph(a->use_graph, e->no_graph, nsteps, tape, e->graphs.count(key) != 0)) {
       const bool dump_in_group = a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] < k + group;
-      if (group > 1 && k + group <= nsteps && !dump_in_group && guided_at(k + group - 1) == guided) {
-        if (!execg[guided]) CKI(get_exec(guided, group, &execg[guided]));
-        CK(cudaGraphLaunch(execg[guided], s));
-        run = group;
-      } else {
-        if (!exec1[guided]) CKI(get_exec(guided, 1, &exec1[guided]));
-        CK(cudaGraphLaunch(exec1[guided], s));
-      }
+      if (group > 1 && k + group <= nsteps && !dump_in_group && guided_at(k + group - 1) == guided) key.group = run = group;
+      cudaGraphExec_t exec = nullptr;
+      CKI(capture_step_graph(e, key, [&](cudaStream_t cs) { return enqueue(cs, run); }, &exec));
+      CK(cudaGraphLaunch(exec, s));
     } else {
-      CKI(enqueue_step(s, guided));
+      CKI(enqueue(s, 1));
     }
-    e->launches += (long long)run * (launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) : 0));
+    e->launches += (long long)run * launches_per_eval(e, guided);
+    if (kind == kPlmsFirst) e->launches += launches_per_eval(e, guided2);
     k += run;
     if (a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] == k - 1) {
       if (host) {

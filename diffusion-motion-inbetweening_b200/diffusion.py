@@ -274,71 +274,48 @@ class GaussianDiffusion:
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
+        if plms or dpm:
+            common["plms_order" if plms else "dpm_order"] = int(order)
+        if progressive:
+            return self._step_generator(eng, x_T, init_image, skip_timesteps, tape, common)
         if rev:
-            if progressive:
-                return self._reverse_progressive(eng, x_T, skip_timesteps, common)
             return eng.sample(skip_timesteps=skip_timesteps, num_steps=num_steps, x_T=x_T, want_pred_xstart=want_pred_xstart,
                               **common)
         if plms or dpm:
-            common["plms_order" if plms else "dpm_order"] = int(order)
-            if progressive:
-                return self._multistep_progressive(eng, x_T, init_image, skip_timesteps, common)
             return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T, **common)
-        if not progressive:
-            res = eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T,
-                             noise_tape=None if tape is None else tape, want_pred_xstart=False, dump_steps=dump_steps, **common)
-            return res
-        return self._progressive(eng, x_T, init_image, skip_timesteps, tape, common)
+        return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T,
+                          noise_tape=None if tape is None else tape, want_pred_xstart=False, dump_steps=dump_steps, **common)
 
-    def _progressive(self, eng, x_T, init_image, skip_timesteps, tape, common):
-        """Generator form: one native call per step (slower than the fused loop; kept for API parity)."""
-        n = self.num_timesteps - skip_timesteps
-        state = x_T
+    def _step_generator(self, eng, x_T, init_image, skip_timesteps, tape, common):
+        """Generator form of every sampler: one native call per step (slower than the fused loop; kept for API parity),
+        each starting from the previous call's sample and replaying the same step graph.  The multistep samplers
+        (PLMS, DPM-Solver++) continue the history the engine keeps on the device, and DDIM inversion draws nothing, so
+        their samples equal the fused loop's bit for bit; a caller that stops an inversion early has a partial one.
+        PLMS also yields old_eps, the values of the reference's history list at that yield (the reference yields one
+        list it keeps mutating)."""
         common = dict(common)
+        common["use_graph"] = 2 if common.get("use_graph", True) else 0  # one native call per step, same step graph every time
+        plms = common["sampler"] == capi.SAMPLER_PLMS
+        torch_rng = common.get("rng_mode", capi.RNG_ENGINE) == capi.RNG_TORCH
         off0, inc = common.pop("aten_offset", 0), common.get("aten_increment", 0)
-        for k in range(n):
-            if common.get("rng_mode", capi.RNG_ENGINE) == capi.RNG_TORCH:
-                common["aten_offset"] = off0 + k * inc  # each one-step call starts at its own draw of the stream
-            common["use_graph"] = 2 if common.get("use_graph", True) else 0  # one native call per step, same step graph every time
-            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, resume=(k > 0), init_image=init_image if k == 0 else None,
-                             x_T=state, noise_tape=None if tape is None else tape[k:], want_pred_xstart=True, **common)
+        state = x_T
+        for k in range(self.num_timesteps - skip_timesteps):
+            call = {}
+            if common["sampler"] != capi.SAMPLER_DDIM_REVERSE:  # an inversion has no q_sample and no history to resume
+                call.update(resume=(k > 0), init_image=init_image if k == 0 else None)
+            if torch_rng:
+                call["aten_offset"] = off0 + k * inc  # each one-step call starts at its own draw of the stream
+            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, x_T=state, want_pred_xstart=True, want_old_eps=plms,
+                             noise_tape=None if tape is None else tape[k:], **call, **common)
             state = res["sample"]
-            if common.get("rng_mode", capi.RNG_ENGINE) == capi.RNG_TORCH:
+            if torch_rng:
                 # torch's generator moves one randn_like at a time, as the reference's loop moves it: a caller that
                 # breaks out of the generator early leaves it where the reference would
                 _advance_torch_generator(eng.device, inc)
-            yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
-
-    def _multistep_progressive(self, eng, x_T, init_image, skip_timesteps, common):
-        """The generator of the multistep samplers (PLMS, DPM-Solver++): one native call per step, each continuing the
-        history the engine keeps on the device, so the samples equal the fused loop's bit for bit.  PLMS also yields
-        old_eps, the values of the reference's history list at that yield (the reference yields one list it keeps
-        mutating)."""
-        n = self.num_timesteps - skip_timesteps
-        state = x_T
-        common = dict(common)
-        common["use_graph"] = 2 if common.get("use_graph", True) else 0
-        plms = common["sampler"] == capi.SAMPLER_PLMS
-        for k in range(n):
-            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, resume=(k > 0), init_image=init_image if k == 0 else None,
-                             x_T=state, want_pred_xstart=True, want_old_eps=plms, **common)
-            state = res["sample"]
             step = {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
             if plms:
                 step["old_eps"] = res["old_eps"]
             yield step
-
-    def _reverse_progressive(self, eng, x_start, skip_timesteps, common):
-        """DDIM inversion as a generator: one native call per step (the step graph is shared), each starting from the
-        previous call's sample, so the samples equal the fused loop's bit for bit.  A caller that stops early has a
-        partial inversion."""
-        state = x_start
-        common = dict(common)
-        common["use_graph"] = 2 if common.get("use_graph", True) else 0
-        for k in range(self.num_timesteps - skip_timesteps):
-            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, x_T=state, want_pred_xstart=True, **common)
-            state = res["sample"]
-            yield {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
 
     # ------------------------------------------------------------------------------------------
     def p_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,

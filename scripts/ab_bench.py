@@ -9,6 +9,10 @@ prints steps/s, the clocks bench.py sampled and the per-kernel ms per step of it
     the two builds' sample.npy files are compared byte for byte;
   - one profile pass per build with CMDI_CHAIN_DBG=1, which prints the chained kernel's cycles per tile (warp 0:
     epi0_acc_wait = mainloop, epi0_slices = epilogue, epi0_publish = publish wait);
+  - the samplers bench.py does not drive (its workload is DDPM): SAMPLER_SNIPPET runs short loops of DDIM eta = 1 with
+    CFG + imputation, PLMS order 4 down to t = 0, DPM-Solver++ order 3 (fused, and the generator, which resumes the
+    history), DDIM inversion and a reconstruction-guided loop under each build, same seeds; every tensor is compared
+    byte for byte and every launch count exactly;
   - with --full, the whole bench.py (configs[2..4] and the eager PyTorch baseline) and scripts/bench_unet_precision.py
     once per build.
 Prints the card's name, power limit and max SM clock first.  Writes nothing in the tree: dumps go to a temporary
@@ -38,6 +42,61 @@ eng = m.engine_for(torch.device("cuda", 0), max_batch=bench.B, precision=C.capi.
 eng.profile_pass(bench.B)
 print("--- warm pass ---", file=sys.stderr, flush=True)
 eng.profile_pass(bench.B)
+"""
+
+
+SAMPLER_SNIPPET = r"""
+import sys, numpy as np, torch
+sys.path.insert(0, sys.argv[1])
+import condmdi_b200 as C
+from oracle import condmdi_oracle as O
+dev = torch.device("cuda", 0)
+gi = O.golden_inputs()
+B, D, L = gi["x"].shape[0], gi["x"].shape[1], gi["x"].shape[3]
+shape = (B, D, 1, L)
+m = C.MDM(cond_mode="text", cond_mask_prob=0.1)
+m.load_state_dict(O.random_state_dict(seed=7, text=True), strict=False)
+m = m.to(dev)
+m.encode_text = lambda texts: gi["cond"].to(dev)
+w = C.ClassifierFreeSampleModel(m)
+eng = m.engine_for(dev, max_batch=B)
+x_obs, x_T = gi["x_obs"].to(dev), gi["x"].to(dev)
+y = {"text": ["a", "b"], "text_scale": gi["text_scale"].to(dev), "mask": gi["y_mask"].to(dev), "lengths": gi["lengths"],
+     "imputate": 1, "stop_imputation_at": 1, "replacement_distribution": "conditional", "inpainted_motion": x_obs,
+     "inpainting_mask": gi["kf_mask"].to(dev)}
+y_guided = dict(y, reconstruction_guidance=True, reconstruction_weight=20.0, gradient_schedule=None, diffusion_steps=1000,
+                stop_recguidance_at=2)
+d = C.create_gaussian_diffusion(timestep_respacing="ddim50")
+d.rng, d.engine_seed = "engine", 5
+out, counts = {}, {}
+
+def record(name, fn):
+    n0 = eng.launch_count
+    res = fn()
+    torch.cuda.synchronize()
+    counts[name] = eng.launch_count - n0
+    steps = res if isinstance(res, list) else [{"sample": res}]
+    for i, st in enumerate(steps):
+        for k, v in st.items():
+            for j, t in enumerate(v if isinstance(v, (list, tuple)) else [v]):
+                out[f"{name}.{i}.{k}.{j}"] = t.cpu().numpy()
+
+kw = dict(model_kwargs={"y": y}, init_image=x_obs)
+record("ddim_eta1", lambda: d.ddim_sample_loop(w, shape, eta=1.0, skip_timesteps=44, **kw))
+record("ddim_eta1_gen", lambda: list(d.ddim_sample_loop_progressive(w, shape, eta=1.0, skip_timesteps=46, **kw)))
+record("plms4", lambda: d.plms_sample_loop(w, shape, noise=x_T, order=4, skip_timesteps=43, **kw))
+record("plms4_gen", lambda: list(d.plms_sample_loop_progressive(w, shape, noise=x_T, order=4, skip_timesteps=45, **kw)))
+record("plms_first_at_zero", lambda: d.plms_sample_loop(w, shape, noise=x_T, order=4, skip_timesteps=49, **kw))
+record("dpm3", lambda: d.dpm_solver_sample_loop(w, shape, noise=x_T, order=3, skip_timesteps=44, **kw))
+record("dpm3_gen", lambda: list(d.dpm_solver_sample_loop_progressive(w, shape, noise=x_T, order=3, skip_timesteps=45, **kw)))
+record("inversion", lambda: d.ddim_reverse_sample_loop(w, x_obs, model_kwargs={"y": y}))
+record("inversion_gen", lambda: list(d.ddim_reverse_sample_loop_progressive(w, x_obs, model_kwargs={"y": y}))[-3:])
+kw["model_kwargs"] = {"y": y_guided}
+record("guided_ddim", lambda: d.ddim_sample_loop(w, shape, noise=x_T, skip_timesteps=45, **kw))
+record("guided_plms", lambda: d.plms_sample_loop(w, shape, noise=x_T, order=3, skip_timesteps=45, **kw))
+record("guided_dpm_gen", lambda: list(d.dpm_solver_sample_loop_progressive(w, shape, noise=x_T, order=2, skip_timesteps=45, **kw)))
+np.savez(sys.argv[2], **out)
+print("launch counts:", counts)
 """
 
 
@@ -137,6 +196,9 @@ def compare(arms, args, res, tmp):
         res["chain_dbg"][arm] = lines
         print(f"chain dbg {arm}:", *lines, sep="\n  ", flush=True)
 
+    res["samplers"] = samplers(arms, tmp)
+    print("samplers (A vs B):", json.dumps(res["samplers"]), flush=True)
+
     if args.full:
         res["full"] = {}
         for arm, lib in arms.items():
@@ -147,6 +209,21 @@ def compare(arms, args, res, tmp):
             out = run([sys.executable, os.path.join("scripts", "bench_unet_precision.py")], lib).stdout.strip().splitlines()
             res["full"][arm]["bench_unet_precision"] = json.loads(out[-1])
             print(f"bench_unet_precision {arm}:", out[-1], flush=True)
+
+
+def samplers(arms, tmp):
+    import numpy as np
+
+    counts, dumps = {}, {}
+    for arm, lib in arms.items():
+        path = os.path.join(tmp, arm, "samplers.npz")
+        r_ = run([sys.executable, "-c", SAMPLER_SNIPPET, ROOT, path], lib)
+        counts[arm] = r_.stdout.strip().splitlines()[-1]
+        dumps[arm] = np.load(path)
+    a, b = dumps["A"], dumps["B"]
+    differ = sorted(set(a.files) ^ set(b.files)) + [k for k in a.files if k in b.files and a[k].tobytes() != b[k].tobytes()]
+    return {"tensors": len(a.files), "tensors_that_differ": differ, "launch_counts_equal": counts["A"] == counts["B"],
+            "launch_counts": counts}
 
 
 if __name__ == "__main__":
