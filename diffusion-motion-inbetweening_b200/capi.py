@@ -20,6 +20,8 @@ SAMPLER_DDIM = 1
 SAMPLER_PLMS = 2
 SAMPLER_DDIM_REVERSE = 3  # DDIM inversion x_t -> x_{t+1} (ddim_reverse_sample); the loop ascends from skip_timesteps
 SAMPLER_DPM_SOLVER = 4  # DPM-Solver++ multistep, orders 1-3 (dpm_order)
+SAMPLER_UNIPC = 5  # UniPC predictor-corrector, orders 1-3 (unipc_order, unipc_variant, unipc_corrector)
+UNIPC_BH1, UNIPC_BH2 = 1, 2  # unipc_variant
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
 MOTION_ABS3D_TO_REL, MOTION_REL_TO_ABS3D, MOTION_REL_TO_JOINTS, MOTION_ABS3D_TO_JOINTS = 0, 1, 2, 3
 
@@ -58,7 +60,8 @@ class SampleArgs(Structure):
                 ("stop_recguidance_at", c_int32), ("recon_coef", POINTER(c_float)), ("pred_xstart_out", c_void_p),
                 ("dump_xstart", c_void_p), ("dump_steps", POINTER(c_int32)), ("n_dump", c_int32),
                 ("host_buffers", c_int32), ("use_graph", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p),
-                ("plms_order", c_int32), ("plms_old_eps_out", c_void_p), ("dpm_order", c_int32)]
+                ("plms_order", c_int32), ("plms_old_eps_out", c_void_p), ("dpm_order", c_int32),
+                ("unipc_order", c_int32), ("unipc_variant", c_int32), ("unipc_corrector", c_int32)]
 
 
 class LibraryMissing(RuntimeError):

@@ -9,6 +9,7 @@
 //   plms_step              plms_sample (pseudo linear multistep), same combine      gaussian_diffusion.py:1589-1687
 //   ddim_reverse_step      ddim_reverse_sample (DDIM inversion, eta = 0), same combine  gaussian_diffusion.py:1418-1452
 //   dpm_solver_step        DPM-Solver++ multistep (Lu et al. 2022), orders 1-3, same combine
+//   unipc_step             UniPC predictor-corrector (Zhao et al. 2023), orders 1-3, same combine
 //   layout converters      reference [B,D,1,L] <-> frame-major [B*L, D_pad]
 //
 // The step kernel uses explicit non-contracted fp32 intrinsics (__fmul_rn/__fadd_rn) in the
@@ -461,6 +462,67 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p
 }
 
 // ---------------------------------------------------------------------------------------------
+// UniPC step (Zhao et al. 2023, multistep, data prediction) on frame-major state [B*L, D_pad].  One thread = 4
+// consecutive features of one frame.  The pass evaluated the uncorrected state x_s; m0 = its x0 (shared combine).  The
+// kernel corrects (UniC) x_s^c = Ac x_{s+1}^c + C0 m0 + C1 m1 + C2 m2 + C3 m3 when a predictor step led into s, then
+// predicts (UniP) x_{s-1} = A x_s^c + B0 m0 + B1 m1 + B2 m2; m_j is the x0 of iteration k - j.  The coefficients are
+// host-computed in float64 for the running history, 12 per step index.  The x0 history is the ring of three buffers
+// DPM-Solver++ uses: iteration k at slot k % 3, so m3 (iteration k - 3) sits in this step's own slot and is read before
+// m0 overwrites it.  x_s^c replaces x_{s+1}^c in q.xc.  No noise is drawn.  Advances s -> s - 1.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) unipc_step_kernel(const StepParams p, const UnipcParams q) {
+  const int s = *p.step_ptr;
+  const int k = p.step_ptr[2] - s;                                  // loop iteration since the history started
+  const int pe = min(min(q.order, k + 1), s + 1);                   // predictor order of s -> s - 1
+  const int ce = (q.corrector && k > 0 && s > 0) ? min(min(q.order, k), s + 2) : 0;  // order of the predictor into s
+  const int nh = max(pe - 1, ce);                                   // history planes the two updates read
+  const float4* row = reinterpret_cast<const float4*>(q.coef + (size_t)s * 12);
+  const float4 cp = row[0];                                         // (A, B0, B1, B2)
+  const float4 cc = ce ? row[1] : make_float4(0.f, 0.f, 0.f, 0.f);  // (Ac, C0, C1, C2)
+  const float c3 = ce >= 3 ? row[2].x : 0.f;                        // C3
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  const size_t i4 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i4 < n4) {
+    const size_t idx = i4 * 4;
+    const int c = (int)(idx % p.D_pad);
+    const int b = (int)(idx / ((size_t)p.L * p.D_pad));
+    float* cur = q.x0_hist + (size_t)(k % 3) * q.hist_stride;
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 m1v = nh >= 1 ? *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 2) % 3) * q.hist_stride + idx) : z4;
+    const float4 m2v = nh >= 2 ? *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 1) % 3) * q.hist_stride + idx) : z4;
+    const float4 m3v = nh >= 3 ? *reinterpret_cast<const float4*>(cur + idx) : z4;  // k - 3, before m0 overwrites it
+    const float4 xcv = ce ? *reinterpret_cast<const float4*>(q.xc + idx) : z4;
+    const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w}, m2[4] = {m2v.x, m2v.y, m2v.z, m2v.w};
+    const float m3[4] = {m3v.x, m3v.y, m3v.z, m3v.w}, xcp[4] = {xcv.x, xcv.y, xcv.z, xcv.w};
+    float xtv[4], x04[4], xn4[4], xc4[4];
+    load_step_x0(p, idx, b, c, s, xtv, x04);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float x0 = x04[j];
+      float xn = 0.f, xc = 0.f;
+      if (c + j < p.D) {
+        xc = xtv[j];  // nothing to correct: x_s^c = x_s
+        if (ce) {
+          xc = __fadd_rn(__fadd_rn(__fmul_rn(cc.x, xcp[j]), __fmul_rn(cc.y, x0)), __fmul_rn(cc.z, m1[j]));
+          if (ce >= 2) xc = __fadd_rn(xc, __fmul_rn(cc.w, m2[j]));
+          if (ce >= 3) xc = __fadd_rn(xc, __fmul_rn(c3, m3[j]));
+        }
+        xn =__fadd_rn(__fmul_rn(cp.x, xc), __fmul_rn(cp.y, x0));
+        if (pe >= 2) xn = __fadd_rn(xn, __fmul_rn(cp.z, m1[j]));
+        if (pe >= 3) xn = __fadd_rn(xn, __fmul_rn(cp.w, m2[j]));
+        if (s == 0) xn = x0;  // the last step lands on abar = 1: the sample is x0 (A = 0, B0 = 1)
+      }
+      xn4[j] = xn;
+      xc4[j] = xc;
+    }
+    *reinterpret_cast<float4*>(cur + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+    if (q.xc) *reinterpret_cast<float4*>(q.xc + idx) = make_float4(xc4[0], xc4[1], xc4[2], xc4[3]);
+    store_step_state(p, idx, xn4, x04, true);
+  }
+  advance_step(p.step_ptr, s - 1);
+}
+
+// ---------------------------------------------------------------------------------------------
 // diffusion step. grid: (ceil(L/32), ceil(D_pad/32), B); block 32x8. Each block owns a 32(l) x 32(c)
 // tile: frame-major operands are read/written with c fastest, the reference-layout noise tape with
 // l fastest, through a padded smem tile.
@@ -844,6 +906,13 @@ cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cuda
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
   return launch_kernel(dpm_solver_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+}
+
+cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStream_t stream) {
+  if (q.order < 1 || q.order > 3 || (q.corrector && !q.xc) || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
+    return cudaErrorInvalidValue;
+  const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
+  return launch_kernel(unipc_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream) {

@@ -95,8 +95,9 @@ struct GraphKey {
   float eta;
   const void* tape;
   int t0, uncond, guided, group;
-  int order, plms_phase, guided2;  // PLMS / DPM-Solver++: order; PLMS: step kind (PlmsStep), guidance of the first step's
-                                   // second evaluation
+  int order, plms_phase, guided2;  // PLMS / DPM-Solver++ / UniPC: order; PLMS: step kind (PlmsStep), guidance of the first
+                                   // step's second evaluation
+  int variant, corrector;          // UniPC
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -177,14 +178,19 @@ struct cmdi_engine {
   long long* chain_dbg = nullptr;               // CMDI_CHAIN_DBG=1: cycle counters of layer 1's chain during cmdi_profile_pass
   std::map<int, ChainTables> chain_tables;
   UnetModel* unet = nullptr;  // MDM_UNET denoiser (cfg.arch == CMDI_ARCH_UNET): engine_unet.inc
-  // The multistep history of PLMS (eps) and DPM-Solver++ (x0), allocated by the first such call: a ring [3][maxB*L, D_pad],
-  // and the host side of the running history, which a `resume` call continues.  PLMS also keeps its first step's x_t.
-  float *hist = nullptr, *plms_keep = nullptr;
+  // The multistep history of PLMS (eps), DPM-Solver++ and UniPC (x0), allocated by the first such call: a ring
+  // [3][maxB*L, D_pad], and the host side of the running history, which a `resume` call continues.  hist_keep
+  // [maxB*L, D_pad] (allocated by the first PLMS call or UniPC call with the corrector) holds PLMS's first step's x_t or
+  // UniPC's corrected state.
+  float *hist = nullptr, *hist_keep = nullptr;
   bool hist_live = false;
   int hist_sampler = 0, hist_order = 0, hist_B = 0, hist_t_start = 0, hist_steps = 0;
+  int hist_variant = 0, hist_corrector = 0;  // UniPC
   std::vector<double> h_acp;       // alphas_cumprod of the schedule (float64)
   std::vector<float> h_dpm_coef;   // [T][4] DPM-Solver++ coefficients of the running history
   float* dpm_coef = nullptr;       // their device copy
+  std::vector<float> h_unipc_coef; // [T][12] UniPC coefficients of the running history
+  float* unipc_coef = nullptr;     // their device copy (allocated by the first UniPC call on a schedule)
   std::map<GraphKey, cudaGraphExec_t> graphs;
   int64_t launches = 0;
 };
@@ -917,6 +923,7 @@ extern "C" int cmdi_engine_destroy(cmdi_engine* e) {
   if (e->d_tmap) cudaFree(e->d_tmap);
   if (e->guide_coef) cudaFree(e->guide_coef);
   if (e->dpm_coef) cudaFree(e->dpm_coef);
+  if (e->unipc_coef) cudaFree(e->unipc_coef);
   delete e;
   return 0;
 }
@@ -1081,7 +1088,8 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
   if (e->tables) cudaFree(e->tables);
   if (e->d_tmap) cudaFree(e->d_tmap);
   if (e->dpm_coef) cudaFree(e->dpm_coef);
-  e->tables = nullptr; e->d_tmap = nullptr; e->dpm_coef = nullptr;
+  if (e->unipc_coef) cudaFree(e->unipc_coef);
+  e->tables = nullptr; e->d_tmap = nullptr; e->dpm_coef = nullptr; e->unipc_coef = nullptr;
   e->hist_live = false;  // a multistep history belongs to the schedule it started on
   CK(cudaMalloc(&e->dpm_coef, (size_t)4 * T * 4));
   CK(cudaMalloc(&e->tables, host.size() * 4));
@@ -1252,18 +1260,120 @@ void dpm_solver_coefs(const std::vector<double>& acp, int t_start, int order, st
   }
 }
 
-// The first argument the deterministic samplers (DPM-Solver++, DDIM inversion) have no use for but the caller set, or null.
+// Solves the n x n system M x = v (n <= 3) in float64 by Gaussian elimination with partial pivoting; M and v are overwritten.
+void solve_small(int n, double M[3][3], double v[3], double x[3]) {
+  for (int c = 0; c < n; ++c) {
+    int piv = c;
+    for (int r = c + 1; r < n; ++r)
+      if (std::fabs(M[r][c]) > std::fabs(M[piv][c])) piv = r;
+    std::swap(M[c], M[piv]);
+    std::swap(v[c], v[piv]);
+    for (int r = c + 1; r < n; ++r) {
+      const double f = M[r][c] / M[c][c];
+      for (int j = c; j < n; ++j) M[r][j] -= f * M[c][j];
+      v[r] -= f * v[c];
+    }
+  }
+  for (int r = n - 1; r >= 0; --r) {
+    double acc = v[r];
+    for (int j = r + 1; j < n; ++j) acc -= M[r][j] * x[j];
+    x[r] = acc / M[r][r];
+  }
+}
+
+// One UniPC update (Zhao et al. 2023, multistep, data prediction) of order p from step index u (state x, x0 history
+// m_u, m_{u+1}, ..., m_{u+p-1}) to step index t, folded to x_t = ratio x + w[0] m_t + w[1] m_u + ... + w[p] m_{u+p-1}
+// (w[0] = 0 for the predictor UniP; m_t = x0 at the predicted x_t for the corrector UniC).  alpha = sqrt(abar),
+// sigma = sqrt(1 - abar), lambda = log alpha - log sigma:
+//   h = lambda_t - lambda_u, hh = -h, h_phi_1 = expm1(hh), B_h = hh (bh1) or expm1(hh) (bh2),
+//   r_k = (lambda_{u+k} - lambda_u) / h, rks = [r_1 .. r_{p-1}, 1], D1_k = (m_{u+k} - m_u) / r_k,
+//   R row i = rks^i, b_i = h_phi_{i+1} (i+1)! / B_h (h_phi_1 / hh - 1, then h_phi / hh - 1 / (i+2)! per row)
+//   UniP: x_t = ratio x - alpha_t h_phi_1 m_u - alpha_t B_h sum_k rho_k D1_k, rho = [0.5] (p = 2) or
+//         solve(R[:-1, :-1], b[:-1]) (p = 3)
+//   UniC: the same with sum_k rho_k D1_k + rho_{p-1} (m_t - m_u), rho = [0.5] (p = 1) or solve(R, b)
+// ratio = sigma_t / sigma_u.  At p = 1 the predictor's ratio and w[1] are formed exactly as dpm_solver_coefs forms A and B0.
+struct UniFold {
+  double ratio;
+  double w[4];
+};
+UniFold unipc_fold(const std::vector<double>& acp, int t, int u, int p, int variant, bool predictor) {
+  auto lambda = [&](int i) { return std::log(std::sqrt(acp[i])) - std::log(std::sqrt(1.0 - acp[i])); };
+  const double h = lambda(t) - lambda(u);
+  const double hh = -h;
+  const double h_phi_1 = std::expm1(hh);
+  const double B_h = variant == CMDI_UNIPC_BH1 ? hh : std::expm1(hh);
+  double rks[3], R[3][3], b[3], rho[3] = {0.0, 0.0, 0.0};
+  for (int k = 1; k < p; ++k) rks[k - 1] = (lambda(u + k) - lambda(u)) / h;
+  rks[p - 1] = 1.0;
+  double h_phi_k = h_phi_1 / hh - 1.0, fact = 1.0;
+  for (int i = 0; i < p; ++i) {
+    for (int j = 0; j < p; ++j) R[i][j] = std::pow(rks[j], i);
+    b[i] = h_phi_k * fact / B_h;
+    fact *= i + 2;
+    h_phi_k = h_phi_k / hh - 1.0 / fact;
+  }
+  if (predictor ? p == 2 : p == 1) rho[0] = 0.5;
+  else if (predictor ? p == 3 : p > 1) solve_small(predictor ? p - 1 : p, R, b, rho);
+  const double alpha_t = std::sqrt(acp[t]);
+  UniFold f{};
+  f.ratio = std::sqrt(1.0 - acp[t]) / std::sqrt(1.0 - acp[u]);
+  f.w[1] = -alpha_t * h_phi_1;
+  if (!predictor) {
+    const double c = alpha_t * B_h * rho[p - 1];  // on m_t - m_u
+    f.w[0] -= c;
+    f.w[1] += c;
+  }
+  for (int k = 1; k < p; ++k) {
+    const double c = alpha_t * B_h * rho[k - 1] / rks[k - 1];  // on D1_k
+    f.w[1] += c;
+    f.w[k + 1] -= c;
+  }
+  return f;
+}
+
+// UniPC coefficients of a history started at step index t_start, 12 per step index s:
+// (A, B0, B1, B2) of the predictor s -> s - 1 (order min(order, k + 1, s + 1), k = t_start - s) and
+// (Ac, C0, C1, C2, C3) of the correction at s (the order of the predictor into s, min(order, k, s + 2); none without
+// the corrector, at k = 0 and at s = 0, whose sample is m0), then three zeros.  Float64; rows above t_start are zero.
+void unipc_coefs(const std::vector<double>& acp, int t_start, int order, int variant, bool corrector, std::vector<float>* out) {
+  const int T = (int)acp.size();
+  out->assign((size_t)12 * T, 0.f);
+  for (int s = 0; s <= t_start; ++s) {
+    const int k = t_start - s;
+    float* row = out->data() + (size_t)12 * s;
+    if (s == 0) {
+      row[1] = 1.f;  // s = 0 lands on abar = 1: x = m0
+    } else {
+      const int pe = std::min(std::min(order, k + 1), s + 1);
+      const UniFold f = unipc_fold(acp, s - 1, s, pe, variant, true);
+      row[0] = (float)f.ratio;
+      for (int j = 1; j <= pe; ++j) row[j] = (float)f.w[j];
+    }
+    const int ce = (corrector && k > 0 && s > 0) ? std::min(std::min(order, k), s + 2) : 0;
+    if (ce) {
+      const UniFold f = unipc_fold(acp, s, s + 1, ce, variant, false);
+      row[4] = (float)f.ratio;
+      for (int j = 0; j <= ce; ++j) row[5 + j] = (float)f.w[j];
+    }
+  }
+}
+
+// The first argument the deterministic samplers (DPM-Solver++, UniPC, DDIM inversion) have no use for but the caller
+// set, or null.
 const char* field_to_unset(const cmdi_sample_args* a) {
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER, rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  if (!dpm && !rev) return nullptr;
+  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
+  if (!dpm && !rev && !unipc) return nullptr;
   if (a->eta != 0.f)
-    return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)" : "eta (the reverse ODE is deterministic: eta must be 0)";
-  if (a->noise_tape) return dpm ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
+    return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
+           : unipc ? "eta (UniPC is deterministic after x_T: eta must be 0)"
+                   : "eta (the reverse ODE is deterministic: eta must be 0)";
+  if (a->noise_tape) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
   if (rev && a->init_image) return "init_image";
   if (a->dump_xstart) return "dump_xstart";
   if (a->plms_order) return "plms_order";
   if (a->plms_old_eps_out) return "plms_old_eps_out";
-  if (dpm && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
+  if ((dpm || unipc) && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
   return nullptr;
 }
 
@@ -1302,7 +1412,9 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   memset(&key, 0, sizeof(key));
   key.B = a->batch; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
   key.stop_at = a->stop_imputation_at; key.has_cond = a->cond_emb != nullptr; key.uncond = a->uncond != 0;
-  key.guided = guided; key.group = group; key.order = plms ? a->plms_order : a->dpm_order;
+  key.guided = guided; key.group = group;
+  key.order = plms ? a->plms_order : a->sampler == CMDI_SAMPLER_UNIPC ? a->unipc_order : a->dpm_order;
+  key.variant = a->unipc_variant; key.corrector = a->unipc_corrector;
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
@@ -1363,13 +1475,14 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int B = a->batch;
   CKI(check_ready(e, B, true));
   if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
-      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER) {
+      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER && a->sampler != CMDI_SAMPLER_UNIPC) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER;
-  const bool multistep = plms || dpm;  // samplers with a device-resident history
+  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
+  const bool multistep = plms || dpm || unipc;  // samplers with a device-resident history
   // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
   // nothing and has no q_sample, dump or PLMS history
   const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
@@ -1377,12 +1490,30 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER field: it must be 0 for sampler %d", a->sampler);
     return 1;
   }
+  if (!unipc && (a->unipc_order || a->unipc_variant || a->unipc_corrector)) {
+    set_last_error("%s is a CMDI_SAMPLER_UNIPC field: it must be 0 for sampler %d",
+                   a->unipc_order ? "unipc_order" : a->unipc_variant ? "unipc_variant" : "unipc_corrector", a->sampler);
+    return 1;
+  }
   if (const char* bad = field_to_unset(a)) {
-    set_last_error("%s: %s must be unset", dpm ? "CMDI_SAMPLER_DPM_SOLVER" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+    set_last_error("%s: %s must be unset",
+                   dpm ? "CMDI_SAMPLER_DPM_SOLVER" : unipc ? "CMDI_SAMPLER_UNIPC" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
     return 1;
   }
   if (dpm && (a->dpm_order < 1 || a->dpm_order > 3)) {
     set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
+    return 1;
+  }
+  if (unipc && (a->unipc_order < 1 || a->unipc_order > 3)) {
+    set_last_error("unipc_order %d outside [1, 3]", a->unipc_order);
+    return 1;
+  }
+  if (unipc && a->unipc_variant != CMDI_UNIPC_BH1 && a->unipc_variant != CMDI_UNIPC_BH2) {
+    set_last_error("unipc_variant %d is neither CMDI_UNIPC_BH1 (1) nor CMDI_UNIPC_BH2 (2)", a->unipc_variant);
+    return 1;
+  }
+  if (unipc && a->unipc_corrector != 0 && a->unipc_corrector != 1) {
+    set_last_error("unipc_corrector %d is neither 0 nor 1", a->unipc_corrector);
     return 1;
   }
   if (rev && !a->x_T) {
@@ -1427,27 +1558,36 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
   const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
   const int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
-  // PLMS / DPM-Solver++: a call without `resume` starts a new history at t0; a `resume` call continues the running one
+  // PLMS / DPM-Solver++ / UniPC: a call without `resume` starts a new history at t0; a `resume` call continues the
+  // running one
   int hist_t0 = t0;
   if (multistep) {
-    const int order = plms ? a->plms_order : a->dpm_order;
+    const int order = plms ? a->plms_order : unipc ? a->unipc_order : a->dpm_order;
     if (a->resume) {
       if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
+          e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
           t0 != e->hist_t_start - e->hist_steps) {
-        set_last_error("%s resume at step %d does not continue the running history", plms ? "PLMS" : "DPM-Solver++", t0);
+        set_last_error("%s resume at step %d does not continue the running history",
+                       plms ? "PLMS" : unipc ? "UniPC" : "DPM-Solver++", t0);
         return 1;
       }
       hist_t0 = e->hist_t_start;
     } else {
       const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
       if (!e->hist) CKI(dev_alloc(e, &e->hist, 3 * slot));
-      if (plms && !e->plms_keep) CKI(dev_alloc(e, &e->plms_keep, slot));
+      if ((plms || (unipc && a->unipc_corrector)) && !e->hist_keep) CKI(dev_alloc(e, &e->hist_keep, slot));
       if (dpm) {
         dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
         CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
       }
+      if (unipc) {
+        if (!e->unipc_coef) CK(cudaMalloc(&e->unipc_coef, (size_t)12 * e->T * 4));
+        unipc_coefs(e->h_acp, t0, order, a->unipc_variant, a->unipc_corrector != 0, &e->h_unipc_coef);
+        CK(cudaMemcpyAsync(e->unipc_coef, e->h_unipc_coef.data(), e->h_unipc_coef.size() * 4, cudaMemcpyHostToDevice, s));
+      }
       e->hist_live = true;
       e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
+      e->hist_variant = a->unipc_variant; e->hist_corrector = a->unipc_corrector;
     }
   }
   CKI(ensure_temb(e, s));
@@ -1534,6 +1674,12 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       DpmParams q{};
       q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
       CK(launch_dpm_solver_step(sp, q, st));
+    } else if (unipc) {
+      UnipcParams q{};
+      q.order = a->unipc_order; q.corrector = a->unipc_corrector;
+      q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad;
+      q.xc = a->unipc_corrector ? e->hist_keep : nullptr; q.coef = e->unipc_coef;
+      CK(launch_unipc_step(sp, q, st));
     } else {
       CK(rev ? launch_ddim_reverse_step(sp, st) : launch_diffusion_step(sp, st));
     }
@@ -1543,7 +1689,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
     PlmsParams q{};
     q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
-    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->plms_keep;
+    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->hist_keep;
     const bool guided[2] = {g1, g2};
     for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
       CKI(enqueue_eval(st, guided[ev]));

@@ -264,6 +264,21 @@ struct DpmParams {
   const float* coef;   // [T][4] (A, B0, B1, B2) per step index, for the running history
 };
 cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cudaStream_t stream);
+// UniPC step (Zhao et al. 2023, multistep, data prediction) from the same combine inputs as StepParams (its sampler,
+// eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are required).  After the pass at s on the
+// uncorrected x_s: x_s^c = Ac x_{s+1}^c + C0 m0 + C1 m1 + C2 m2 + C3 m3 (when a predictor step led into s and the
+// corrector is on; x_s^c = x_s otherwise), then x_{s-1} = A x_s^c + B0 m0 + B1 m1 + B2 m2, m_j the x0 of iteration
+// k - j.  The x0 history is DPM-Solver++'s ring (slot k % 3 for loop iteration k = step_ptr[2] - s); advances s -> s - 1.
+struct UnipcParams {
+  int order;           // 1..3; the predictor at s uses min(order, k + 1, s + 1), the correction at s the order of the
+                       // predictor into s, min(order, k, s + 2) (none at k = 0 or s = 0)
+  int corrector;       // 0: UniP only (q.xc may be null)
+  float* x0_hist;      // [3][B*L, D_pad]
+  size_t hist_stride;  // elements between slots
+  float* xc;           // [B*L, D_pad] the corrected state: x_{s+1}^c in, x_s^c out
+  const float* coef;   // [T][12] (A, B0, B1, B2, Ac, C0, C1, C2, C3, 0, 0, 0) per step index, for the running history
+};
+cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStream_t stream);
 // DDIM reverse step (ddim_reverse_sample, gaussian_diffusion.py:1418-1452, eta = 0): x_t -> x_{t+1} from the same combine
 // inputs as StepParams (its sampler, eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are
 // required).  Advances the step index t -> t + 1, so one captured graph serves every step of an inversion.

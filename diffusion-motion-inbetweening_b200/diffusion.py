@@ -5,11 +5,12 @@ Mirrors (same names, argument meaning and error behaviour; paths relative to the
     ModelMeanType / ModelVarType / DiffusionConfig  :74-136
     GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1418-1587, :1589-1804
                                                     + dpm_solver_sample_loop[_progressive] (DPM-Solver++, not in the reference)
+                                                    + unipc_sample_loop[_progressive] (UniPC, not in the reference)
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
-`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` / `dpm_solver_sample_loop` run the
-WHOLE loop in one native
+`p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` / `dpm_solver_sample_loop` /
+`unipc_sample_loop` run the WHOLE loop in one native
 call (`cmdi_sample`): no per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
 `p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` / `ddim_reverse_sample` is done by the CUDA
@@ -157,12 +158,14 @@ class GaussianDiffusion:
         return y
 
     def _run(self, sampler, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image, randomize_class,
-             dump_steps, const_noise, eta, progressive=False, order=2, num_steps=0, want_pred_xstart=False):
+             dump_steps, const_noise, eta, progressive=False, order=2, num_steps=0, want_pred_xstart=False,
+             variant="bh2", corrector=True):
         if model_kwargs is None:
             model_kwargs = {}
         y = self._check_supported(cond_fn, const_noise, randomize_class, model_kwargs)
         plms = sampler == capi.SAMPLER_PLMS
         dpm = sampler == capi.SAMPLER_DPM_SOLVER
+        unipc = sampler == capi.SAMPLER_UNIPC
         rev = sampler == capi.SAMPLER_DDIM_REVERSE  # `noise` is the state to invert; skip_timesteps its step index
         if sampler == capi.SAMPLER_DDPM:
             assert cond_fn is None, "only support the case where cond_fn is None"  # gaussian_diffusion.py:685
@@ -239,10 +242,10 @@ class GaussianDiffusion:
         if tape is not None:
             tape = tape[1:]
         seed, rng_args = 0, {}
-        if plms or rev or dpm:
+        if plms or rev or dpm or unipc:
             # plms_sample_loop_progressive draws nothing after x_T (:1767-1770): a tape contributes tape[0] only, torch's
             # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine".
-            # DPM-Solver++ behaves the same way.  DDIM inversion draws nothing at all: x_T is the caller's state
+            # DPM-Solver++ and UniPC behave the same way.  DDIM inversion draws nothing at all: x_T is the caller's state
             tape = None
             if x_T is None:
                 seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -276,12 +279,15 @@ class GaussianDiffusion:
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
         if plms or dpm:
             common["plms_order" if plms else "dpm_order"] = int(order)
+        if unipc:
+            common.update(unipc_order=int(order), unipc_variant=capi.UNIPC_BH1 if variant == "bh1" else capi.UNIPC_BH2,
+                          unipc_corrector=bool(corrector))
         if progressive:
             return self._step_generator(eng, x_T, init_image, skip_timesteps, tape, common)
         if rev:
             return eng.sample(skip_timesteps=skip_timesteps, num_steps=num_steps, x_T=x_T, want_pred_xstart=want_pred_xstart,
                               **common)
-        if plms or dpm:
+        if plms or dpm or unipc:
             return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T, **common)
         return eng.sample(skip_timesteps=skip_timesteps, init_image=init_image, x_T=x_T,
                           noise_tape=None if tape is None else tape, want_pred_xstart=False, dump_steps=dump_steps, **common)
@@ -289,7 +295,8 @@ class GaussianDiffusion:
     def _step_generator(self, eng, x_T, init_image, skip_timesteps, tape, common):
         """Generator form of every sampler: one native call per step (slower than the fused loop; kept for API parity),
         each starting from the previous call's sample and replaying the same step graph.  The multistep samplers
-        (PLMS, DPM-Solver++) continue the history the engine keeps on the device, and DDIM inversion draws nothing, so
+        (PLMS, DPM-Solver++, UniPC) continue the history the engine keeps on the device (UniPC's corrected state
+        included), and DDIM inversion draws nothing, so
         their samples equal the fused loop's bit for bit; a caller that stops an inversion early has a partial one.
         PLMS also yields old_eps, the values of the reference's history list at that yield (the reference yields one
         list it keeps mutating)."""
@@ -395,6 +402,34 @@ class GaussianDiffusion:
         return self._run(capi.SAMPLER_DPM_SOLVER, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
                          init_image, randomize_class, None, False, 0.0, progressive=True, order=order)
 
+    def unipc_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                          model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                          randomize_class=False, cond_fn_with_grad=False, order=2, variant="bh2", corrector=True):
+        """UniPC (Zhao et al. 2023; multistep, data prediction) on this object's spaced steps, orders 1-3, variant
+        "bh1" or "bh2": one denoiser pass per step, through the same x0 pipeline as DDIM (CFG, keyframe input,
+        imputation, reconstruction guidance).  With corrector=True each pass's x0 also corrects the state it was
+        evaluated at (UniC), which raises the order by one at no extra pass.  Order 1 without the corrector is DDIM at
+        eta = 0.  Deterministic after x_T; the whole loop is one native call and the x0 history and corrected state stay
+        on the device.  (The reference has no such sampler.)"""
+        _check_unipc_args(order, variant, corrector)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_UNIPC, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, False, 0.0, order=order, variant=variant,
+                         corrector=corrector)["sample"]
+
+    def unipc_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                                      model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                                      randomize_class=False, cond_fn_with_grad=False, order=2, variant="bh2",
+                                      corrector=True):
+        """Yields {"sample", "pred_xstart"} per step of unipc_sample_loop, one native call per step: "sample" is the
+        state the next pass evaluates (uncorrected), "pred_xstart" this pass's x0.  The samples equal the fused loop's
+        bit for bit.  The configuration is validated at the call."""
+        _check_unipc_args(order, variant, corrector)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_UNIPC, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, False, 0.0, progressive=True, order=order, variant=variant,
+                         corrector=corrector)
+
     def ddim_reverse_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
         """gaussian_diffusion.py:1418-1452: x_t -> x_{t+1} by the reverse DDIM ODE, one native call.  Returns
         {"sample", "pred_xstart"}.  `t` must hold one step index for the whole batch (the engine's step index is per
@@ -449,6 +484,17 @@ def _check_dpm_order(order) -> None:
     """DPM-Solver++'s multistep orders are 1, 2 and 3 (an int; bools and floats are refused)."""
     if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2, 3):
         raise ValueError(f"DPM-Solver++ order must be an int in {{1, 2, 3}}, got {order!r}")
+
+
+def _check_unipc_args(order, variant, corrector) -> None:
+    """UniPC's multistep orders are 1, 2 and 3 (an int; bools and floats are refused), its variants "bh1" and "bh2",
+    and corrector a bool."""
+    if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2, 3):
+        raise ValueError(f"UniPC order must be an int in {{1, 2, 3}}, got {order!r}")
+    if not isinstance(variant, str) or variant not in ("bh1", "bh2"):
+        raise ValueError(f"UniPC variant must be 'bh1' or 'bh2', got {variant!r}")
+    if not isinstance(corrector, (bool, np.bool_)):
+        raise ValueError(f"UniPC corrector must be a bool, got {corrector!r}")
 
 
 def space_timesteps(num_timesteps, section_counts):

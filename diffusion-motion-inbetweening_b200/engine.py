@@ -124,7 +124,7 @@ class Engine:
                want_pred_xstart: bool = False, dump_steps: Optional[Sequence[int]] = None, host_buffers: bool = False,
                use_graph: bool = True, out: Optional[torch.Tensor] = None, obs_x0: Optional[torch.Tensor] = None,
                obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False,
-               dpm_order: int = 2):
+               dpm_order: int = 2, unipc_order: int = 2, unipc_variant: int = capi.UNIPC_BH2, unipc_corrector: bool = True):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -136,6 +136,9 @@ class Engine:
         is not sent.
         sampler=SAMPLER_DPM_SOLVER: DPM-Solver++ multistep of order `dpm_order` (1-3); resume continues its x0 history.
         dpm_order is sent for this sampler only, plms_order for the others.
+        sampler=SAMPLER_UNIPC: UniPC of order `unipc_order` (1-3), variant `unipc_variant` (UNIPC_BH1 / UNIPC_BH2), with
+        or without the corrector; resume continues its x0 history and corrected state.  The unipc_* fields are sent
+        for this sampler only.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         dev = torch.device("cpu") if host_buffers else self.device
@@ -189,6 +192,7 @@ class Engine:
         if want_old_eps and sampler == capi.SAMPLER_PLMS:
             n_old = min(plms_steps, int(plms_order) - 1)  # the length of the reference's list after that many steps
             old_eps = torch.empty((max(n_old, 1),) + shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
+        unipc = sampler == capi.SAMPLER_UNIPC
         a = capi.SampleArgs(batch, sampler, float(eta), int(skip_timesteps), int(num_steps), int(resume), _ptr(init_image), _ptr(x_T), _ptr(noise_tape),
                             int(seed) & (2 ** 64 - 1), int(sample_offset), int(rng_mode), int(aten_offset), int(aten_increment),
                             int(aten_threads), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale),
@@ -196,8 +200,11 @@ class Engine:
                             _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
                             dump_arr, n_dump, int(host_buffers),
                             int(use_graph), _ptr(obs_x0), _ptr(obs_mask),
-                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_DPM_SOLVER) else int(plms_order),
-                            _ptr(old_eps), int(dpm_order) if sampler == capi.SAMPLER_DPM_SOLVER else 0)
+                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_DPM_SOLVER, capi.SAMPLER_UNIPC)
+                            else int(plms_order),
+                            _ptr(old_eps), int(dpm_order) if sampler == capi.SAMPLER_DPM_SOLVER else 0,
+                            int(unipc_order) if unipc else 0, int(unipc_variant) if unipc else 0,
+                            int(unipc_corrector) if unipc else 0)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")

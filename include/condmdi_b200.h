@@ -64,8 +64,16 @@ enum {
    min(dpm_order, iterations since the history started + 1, s + 1), and the last step returns x0 as DDIM's does.
    skip_timesteps / init_image / resume as for DDIM (init_image only on a call that starts a history); eta must be 0 and
    noise_tape, dump_xstart, plms_order and plms_old_eps_out unset: the call fails naming the field otherwise. */
+/* UNIPC: UniPC (Zhao et al. 2023; multistep, data prediction) on the spaced steps, orders 1..3 (unipc_order), variant
+   bh1 or bh2 (unipc_variant), with or without the UniC corrector (unipc_corrector), one denoiser pass per step.  The
+   pass at s evaluates the uncorrected state; its x0 then corrects the state of s (with the order of the predictor
+   step into s) and predicts s - 1 with order min(unipc_order, iterations since the history started + 1, s + 1).  The
+   corrected state stays on the device; the last step returns x0 as DDIM's does.  skip_timesteps / init_image / resume
+   as for DPM_SOLVER; eta must be 0 and noise_tape, dump_xstart, plms_order, plms_old_eps_out and dpm_order unset: the
+   call fails naming the field otherwise. */
 enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3,
-       CMDI_SAMPLER_DPM_SOLVER = 4 };
+       CMDI_SAMPLER_DPM_SOLVER = 4, CMDI_SAMPLER_UNIPC = 5 };
+enum { CMDI_UNIPC_BH1 = 1, CMDI_UNIPC_BH2 = 2 };  /* unipc_variant: B(h) = h or e^h - 1 */
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
 
@@ -167,6 +175,11 @@ typedef struct {
   /* CMDI_SAMPLER_DPM_SOLVER only (0 for every other sampler).  The x0 history stays on the device like PLMS's eps
      history: resume = 1 continues it with the same order and batch. */
   int32_t dpm_order;            /* 1..3 */
+  /* CMDI_SAMPLER_UNIPC only (all 0 for every other sampler).  The x0 history and the corrected state stay on the device:
+     resume = 1 continues them with the same order, variant, corrector and batch. */
+  int32_t unipc_order;          /* 1..3 */
+  int32_t unipc_variant;        /* CMDI_UNIPC_BH1 / CMDI_UNIPC_BH2 */
+  int32_t unipc_corrector;      /* 0 / 1 */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
