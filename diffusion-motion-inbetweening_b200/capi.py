@@ -21,6 +21,7 @@ SAMPLER_PLMS = 2
 SAMPLER_DDIM_REVERSE = 3  # DDIM inversion x_t -> x_{t+1} (ddim_reverse_sample); the loop ascends from skip_timesteps
 SAMPLER_DPM_SOLVER = 4  # DPM-Solver++ multistep, orders 1-3 (dpm_order)
 SAMPLER_UNIPC = 5  # UniPC predictor-corrector, orders 1-3 (unipc_order, unipc_variant, unipc_corrector)
+SAMPLER_DPM_SOLVER_SDE = 6  # SDE-DPM-Solver++ multistep, orders 1-2 (dpm_order); DDPM's per-step draws
 UNIPC_BH1, UNIPC_BH2 = 1, 2  # unipc_variant
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
 MOTION_ABS3D_TO_REL, MOTION_REL_TO_ABS3D, MOTION_REL_TO_JOINTS, MOTION_ABS3D_TO_JOINTS = 0, 1, 2, 3

@@ -523,6 +523,105 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const StepParams p, con
 }
 
 // ---------------------------------------------------------------------------------------------
+// The per-step noise of sample b at step index t for the 32(c) x 32(l) tile at (c0, l0), in the reference layout
+// [b][c][l] (l contiguous), into s_noise[c - c0][l - l0]; block 32x8.  tape_t0 is the call's first step index, so
+// (tape_t0 - t) numbers this step's draw within the call.  Three sources: the noise tape, the torch.randn_like stream
+// (draw number (tape_t0 - t) after aten_offset) and the engine generator (stream t + 1, keyed by the global sample
+// index).  The caller synchronises the block before reading the tile.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void fill_noise_tile(const StepParams& p, int t, int tape_t0, int b, int l0, int c0,
+                                                float (&s_noise)[32][33]) {
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  RngState rng{};
+  if (!p.noise_ref && p.rng) rng = *p.rng;
+  if (!p.noise_ref && rng.mode == 1) {
+    // torch.randn_like stream: draw number (tape_t0 - t) of this loop, element index in the (B, D, 1, L) layout
+    const unsigned long long off = rng.aten_offset + (unsigned long long)(tape_t0 - t) * rng.aten_increment;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = c0 + ty + i * 8, l = l0 + tx;
+      float nz = 0.f;
+      if (c < p.D && l < p.L) nz = aten_normal(rng.seed, off, rng.aten_threads, ((size_t)b * p.D + c) * p.L + l);
+      s_noise[ty + i * 8][tx] = nz;
+    }
+  } else if (!p.noise_ref && (p.L & 3) == 0) {
+    // engine generator: one Philox call yields the 4 consecutive frames of a quad (l0 and L are multiples of 4)
+    const int q = ty * 32 + tx;          // 256 quads = 32 features x 8 frame-quads
+    const int cl = q >> 3, lq = (q & 7) * 4;
+    const int c = c0 + cl, l = l0 + lq;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (c < p.D && l < p.L) philox_normal4(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, ((size_t)c * p.L + l) >> 2, v);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s_noise[cl][lq + j] = v[j];
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = c0 + ty + i * 8, l = l0 + tx;
+      float nz = 0.f;
+      if (c < p.D && l < p.L) {
+        const size_t e = (size_t)c * p.L + l;
+        nz = p.noise_ref ? p.noise_ref[((size_t)(tape_t0 - t) * p.B + b) * p.D * p.L + e]
+                         : philox_normal(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, e);
+      }
+      s_noise[ty + i * 8][tx] = nz;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// SDE-DPM-Solver++ multistep step (Lu et al. 2022, "DPM-Solver++", the SDE solver in data prediction, midpoint form)
+// on frame-major state [B*L, D_pad], with diffusion_step_kernel's grid, block and noise tile.  m0 = x0 of the shared
+// combine; the update is folded into four per-step coefficients (host-computed in float64 for the running history),
+// x_{s-1} = A x_s + B0 m0 + B1 m1 + Cn z, where m1 is the x0 of the previous loop iteration and z this step's draw.
+// The x0 history is DPM-Solver++'s ring (iteration k = step_ptr[2] - s at slot k % 3).  The draw is numbered from the
+// call's first step (step_ptr[3], or the tape_t0 argument), as p_sample_loop's draws are; the last step (s = 0)
+// returns m0 and reads no noise.  Advances s -> s - 1.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) dpm_solver_sde_step_kernel(const StepParams p, const DpmParams q) {
+  griddep_launch_dependents();
+  griddep_wait();
+  __shared__ float s_noise[32][33];
+  const int b = blockIdx.z;
+  const int l0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int s = *p.step_ptr;
+  const int k = p.step_ptr[2] - s;                      // loop iteration since the history started
+  const int call_t0 = p.tape_t0 >= 0 ? p.tape_t0 : p.step_ptr[3];
+  const int eff = min(min(q.order, k + 1), s + 1);      // effective order: lower while the history fills and at the end
+  if (s > 0) fill_noise_tile(p, s, call_t0, b, l0, c0, s_noise);
+  __syncthreads();
+  const float4 cf = *reinterpret_cast<const float4*>(q.coef + (size_t)s * 4);  // (A, B0, B1, Cn)
+  {
+    const int tid = ty * 32 + tx;
+    const int ll = tid >> 3, cq = (tid & 7) * 4;
+    const int l = l0 + ll, c = c0 + cq;
+    if (l < p.L && c < p.D_pad) {
+      const size_t idx = ((size_t)b * p.L + l) * p.D_pad + c;
+      float* cur = q.x0_hist + (size_t)(k % 3) * q.hist_stride;
+      float4 m1v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (eff >= 2) m1v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 2) % 3) * q.hist_stride + idx);  // k - 1
+      const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w};
+      float xtv[4], x04[4], xn4[4];
+      load_step_x0(p, idx, b, c, s, xtv, x04);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float x0 = x04[j];
+        float xn = 0.f;
+        if (c + j < p.D) {
+          xn = __fadd_rn(__fmul_rn(cf.x, xtv[j]), __fmul_rn(cf.y, x0));
+          if (eff >= 2) xn = __fadd_rn(xn, __fmul_rn(cf.z, m1[j]));
+          xn = s != 0 ? __fadd_rn(xn, __fmul_rn(cf.w, s_noise[cq + j][ll])) : x0;  // s = 0 lands on abar = 1: x = m0
+        }
+        xn4[j] = xn;
+      }
+      *reinterpret_cast<float4*>(cur + idx) = make_float4(x04[0], x04[1], x04[2], x04[3]);
+      store_step_state(p, idx, xn4, x04, true);
+    }
+  }
+  advance_step(p.step_ptr, s - 1);
+}
+
+// ---------------------------------------------------------------------------------------------
 // diffusion step. grid: (ceil(L/32), ceil(D_pad/32), B); block 32x8. Each block owns a 32(l) x 32(c)
 // tile: frame-major operands are read/written with c fastest, the reference-layout noise tape with
 // l fastest, through a padded smem tile.
@@ -540,42 +639,7 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
 
   // ---- noise tile (reference layout [b][c][l], l contiguous) ----
   const bool want_noise = p.sampler != 2;  // the reference draws noise at every step, including t == 0
-  if (want_noise) {
-    RngState rng{};
-    if (!p.noise_ref && p.rng) rng = *p.rng;
-    if (!p.noise_ref && rng.mode == 1) {
-      // torch.randn_like stream: draw number (tape_t0 - t) of this loop, element index in the (B, D, 1, L) layout
-      const unsigned long long off = rng.aten_offset + (unsigned long long)(tape_t0 - t) * rng.aten_increment;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = c0 + ty + i * 8, l = l0 + tx;
-        float nz = 0.f;
-        if (c < p.D && l < p.L) nz = aten_normal(rng.seed, off, rng.aten_threads, ((size_t)b * p.D + c) * p.L + l);
-        s_noise[ty + i * 8][tx] = nz;
-      }
-    } else if (!p.noise_ref && (p.L & 3) == 0) {
-      // engine generator: one Philox call yields the 4 consecutive frames of a quad (l0 and L are multiples of 4)
-      const int q = ty * 32 + tx;          // 256 quads = 32 features x 8 frame-quads
-      const int cl = q >> 3, lq = (q & 7) * 4;
-      const int c = c0 + cl, l = l0 + lq;
-      float v[4] = {0.f, 0.f, 0.f, 0.f};
-      if (c < p.D && l < p.L) philox_normal4(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, ((size_t)c * p.L + l) >> 2, v);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s_noise[cl][lq + j] = v[j];
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = c0 + ty + i * 8, l = l0 + tx;
-        float nz = 0.f;
-        if (c < p.D && l < p.L) {
-          const size_t e = (size_t)c * p.L + l;
-          nz = p.noise_ref ? p.noise_ref[((size_t)(tape_t0 - t) * p.B + b) * p.D * p.L + e]
-                           : philox_normal(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, e);
-        }
-        s_noise[ty + i * 8][tx] = nz;
-      }
-    }
-  }
+  if (want_noise) fill_noise_tile(p, t, tape_t0, b, l0, c0, s_noise);
   __syncthreads();
 
   // ---- per-step scalars (fp32, gathered exactly like _extract_into_tensor(...).float()) ----
@@ -708,9 +772,9 @@ __global__ void axpby_kernel(const float* __restrict__ x, const float* __restric
     out[i] = __fadd_rn(__fmul_rn(a, x[i]), __fmul_rn(b, y[i]));
 }
 
-__global__ void set_int_kernel(int* p, int v) {
+__global__ void set_int_kernel(int* p, int v, int next) {
   p[0] = v;
-  p[1] = 0;  // block-arrival counter used by diffusion_step_kernel
+  p[1] = next;  // after the step index: the block-arrival counter (0); after the history's first step: the call's
 }
 
 // LayerNorm folded into the linear layer that consumes it: Wf[n,k] = W[n,k] * gamma[k] (fp32, split into planes by
@@ -908,6 +972,13 @@ cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cuda
   return launch_kernel(dpm_solver_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
+cudaError_t launch_dpm_solver_sde_step(const StepParams& p, const DpmParams& q, cudaStream_t stream) {
+  if (q.order < 1 || q.order > 2 || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
+    return cudaErrorInvalidValue;
+  dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
+  return launch_kernel(dpm_solver_sde_step_kernel, grid, block, 0, stream, p, q);
+}
+
 cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStream_t stream) {
   if (q.order < 1 || q.order > 3 || (q.corrector && !q.xc) || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
     return cudaErrorInvalidValue;
@@ -974,8 +1045,8 @@ cudaError_t launch_recover_from_ric(const float* data, long long sb, long long s
   return cudaGetLastError();
 }
 
-cudaError_t launch_set_int(int* p, int v, cudaStream_t stream) {
-  set_int_kernel<<<1, 1, 0, stream>>>(p, v);
+cudaError_t launch_set_int(int* p, int v, cudaStream_t stream, int next) {
+  set_int_kernel<<<1, 1, 0, stream>>>(p, v, next);
   return cudaGetLastError();
 }
 

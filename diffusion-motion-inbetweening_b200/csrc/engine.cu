@@ -146,7 +146,7 @@ struct cmdi_engine {
   CUtensorMap xseq_st{}, x1_st{};  // fp32 TMA-store targets: xseq (backward pass), x1 (v1 of the chained forward path)
   uint8_t* obs_mask = nullptr;
   float *cond_emb = nullptr, *cond_proj = nullptr, *text_scale = nullptr;
-  int* step_ctr = nullptr;  // [2]: step index, block-arrival counter
+  int* step_ctr = nullptr;  // [4]: step index, block-arrival counter, first step of the running history, of the call
   RngState* rng = nullptr;  // generator state of the running loop (device-resident: step graphs do not depend on it)
   float *ref_a = nullptr, *ref_b = nullptr;  // reference-layout staging [maxB, D, L]
   uint8_t *ref_mask = nullptr, *ymask = nullptr;
@@ -178,7 +178,7 @@ struct cmdi_engine {
   long long* chain_dbg = nullptr;               // CMDI_CHAIN_DBG=1: cycle counters of layer 1's chain during cmdi_profile_pass
   std::map<int, ChainTables> chain_tables;
   UnetModel* unet = nullptr;  // MDM_UNET denoiser (cfg.arch == CMDI_ARCH_UNET): engine_unet.inc
-  // The multistep history of PLMS (eps), DPM-Solver++ and UniPC (x0), allocated by the first such call: a ring
+  // The multistep history of PLMS (eps), DPM-Solver++ (ODE and SDE) and UniPC (x0), allocated by the first such call: a ring
   // [3][maxB*L, D_pad], and the host side of the running history, which a `resume` call continues.  hist_keep
   // [maxB*L, D_pad] (allocated by the first PLMS call or UniPC call with the corrector) holds PLMS's first step's x_t or
   // UniPC's corrected state.
@@ -187,7 +187,7 @@ struct cmdi_engine {
   int hist_sampler = 0, hist_order = 0, hist_B = 0, hist_t_start = 0, hist_steps = 0;
   int hist_variant = 0, hist_corrector = 0;  // UniPC
   std::vector<double> h_acp;       // alphas_cumprod of the schedule (float64)
-  std::vector<float> h_dpm_coef;   // [T][4] DPM-Solver++ coefficients of the running history
+  std::vector<float> h_dpm_coef;   // [T][4] DPM-Solver++ (or SDE-DPM-Solver++) coefficients of the running history
   float* dpm_coef = nullptr;       // their device copy
   std::vector<float> h_unipc_coef; // [T][12] UniPC coefficients of the running history
   float* unipc_coef = nullptr;     // their device copy (allocated by the first UniPC call on a schedule)
@@ -1260,6 +1260,40 @@ void dpm_solver_coefs(const std::vector<double>& acp, int t_start, int order, st
   }
 }
 
+// SDE-DPM-Solver++ multistep coefficients (Lu et al. 2022, the SDE solver in data prediction, midpoint form) of a
+// history started at step index t_start, folded so that step s computes x_{s-1} = A x_s + B0 m0 + B1 m1 + Cn z (m0 this
+// step's x0, m1 the previous step's, z a standard normal draw).  With alpha, sigma, lambda and h as above and
+// e = -expm1(-2h) = 1 - e^{-2h}:
+//   order 1: A = (sigma_u / sigma_s) e^{-h}, B0 = alpha_u e, Cn = sigma_u sqrt(e)   (the DDPM posterior step)
+//   order 2: B0 += alpha_u e / (2 r0), B1 = -alpha_u e / (2 r0), r0 = (lambda_s - lambda_{s+1}) / h
+// The step at s uses order min(order, k + 1, s + 1), k = t_start - s; the row of s = 0 is (0, 1, 0, 0).  Float64; rows
+// above t_start are zero.
+void dpm_solver_sde_coefs(const std::vector<double>& acp, int t_start, int order, std::vector<float>* out) {
+  const int T = (int)acp.size();
+  out->assign((size_t)4 * T, 0.f);
+  auto lambda = [&](int i) { return std::log(std::sqrt(acp[i])) - std::log(std::sqrt(1.0 - acp[i])); };
+  for (int s = 0; s <= t_start; ++s) {
+    double A = 0.0, B0 = 1.0, B1 = 0.0, Cn = 0.0;  // s = 0 lands on abar = 1: x = m0
+    if (s > 0) {
+      const int eff = std::min(std::min(order, t_start - s + 1), s + 1);
+      const double alpha_u = std::sqrt(acp[s - 1]), sigma_u = std::sqrt(1.0 - acp[s - 1]);
+      const double h = lambda(s - 1) - lambda(s);
+      const double e = -std::expm1(-2.0 * h);
+      A = sigma_u / std::sqrt(1.0 - acp[s]) * std::exp(-h);
+      B0 = alpha_u * e;
+      Cn = sigma_u * std::sqrt(e);
+      if (eff == 2) {
+        const double r0 = (lambda(s) - lambda(s + 1)) / h;
+        const double c = 0.5 * alpha_u * e / r0;
+        B0 += c;
+        B1 = -c;
+      }
+    }
+    float* row = out->data() + (size_t)4 * s;
+    row[0] = (float)A; row[1] = (float)B0; row[2] = (float)B1; row[3] = (float)Cn;
+  }
+}
+
 // Solves the n x n system M x = v (n <= 3) in float64 by Gaussian elimination with partial pivoting; M and v are overwritten.
 void solve_small(int n, double M[3][3], double v[3], double x[3]) {
   for (int c = 0; c < n; ++c) {
@@ -1358,22 +1392,23 @@ void unipc_coefs(const std::vector<double>& acp, int t_start, int order, int var
   }
 }
 
-// The first argument the deterministic samplers (DPM-Solver++, UniPC, DDIM inversion) have no use for but the caller
-// set, or null.
+// The first argument the samplers added to the reference's (DPM-Solver++ as ODE and SDE, UniPC, DDIM inversion) have no
+// use for but the caller set, or null.
 const char* field_to_unset(const cmdi_sample_args* a) {
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER, rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
-  if (!dpm && !rev && !unipc) return nullptr;
+  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC, sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
+  if (!dpm && !rev && !unipc && !sde) return nullptr;
   if (a->eta != 0.f)
     return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
            : unipc ? "eta (UniPC is deterministic after x_T: eta must be 0)"
-                   : "eta (the reverse ODE is deterministic: eta must be 0)";
-  if (a->noise_tape) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
+           : sde ? "eta (the SDE solver's noise is fixed by the schedule: eta must be 0)"
+                 : "eta (the reverse ODE is deterministic: eta must be 0)";
+  if (a->noise_tape && !sde) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
   if (rev && a->init_image) return "init_image";
   if (a->dump_xstart) return "dump_xstart";
   if (a->plms_order) return "plms_order";
   if (a->plms_old_eps_out) return "plms_old_eps_out";
-  if ((dpm || unipc) && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
+  if ((dpm || unipc || sde) && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
   return nullptr;
 }
 
@@ -1404,7 +1439,8 @@ enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
 
 // The graph of `group` consecutive steps of this call's configuration with guidance `guided`; for PLMS, of one step of
 // kind `plms_kind` whose second evaluation has guidance `guided2` (both 0 for the other samplers).  The first step index
-// lives in device memory, so t0 stays 0.  PLMS draws no noise: its key leaves eta and the tape at zero.
+// lives in device memory, so t0 stays 0.  PLMS draws no noise: its key leaves eta and the tape at zero.  The order is
+// plms_order, unipc_order or (DPM-Solver++, ODE and SDE) dpm_order; the sampler field tells the two DPM-Solver++ apart.
 // GraphKey is ordered by memcmp and has padding bytes, so the whole struct is zeroed before it is filled.
 GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int plms_kind, bool guided2) {
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
@@ -1475,19 +1511,23 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int B = a->batch;
   CKI(check_ready(e, B, true));
   if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
-      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER && a->sampler != CMDI_SAMPLER_UNIPC) {
+      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER && a->sampler != CMDI_SAMPLER_UNIPC &&
+      a->sampler != CMDI_SAMPLER_DPM_SOLVER_SDE) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER;
   const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
-  const bool multistep = plms || dpm || unipc;  // samplers with a device-resident history
+  // SDE-DPM-Solver++: DPM-Solver++'s x0 history, with DDPM's per-step draws
+  const bool sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
+  const bool multistep = plms || dpm || unipc || sde;  // samplers with a device-resident history
   // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
   // nothing and has no q_sample, dump or PLMS history
   const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  if (!dpm && a->dpm_order) {
-    set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER field: it must be 0 for sampler %d", a->sampler);
+  if (!dpm && !sde && a->dpm_order) {
+    set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER / CMDI_SAMPLER_DPM_SOLVER_SDE field: it must be 0 for sampler %d",
+                   a->sampler);
     return 1;
   }
   if (!unipc && (a->unipc_order || a->unipc_variant || a->unipc_corrector)) {
@@ -1497,11 +1537,16 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   }
   if (const char* bad = field_to_unset(a)) {
     set_last_error("%s: %s must be unset",
-                   dpm ? "CMDI_SAMPLER_DPM_SOLVER" : unipc ? "CMDI_SAMPLER_UNIPC" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+                   dpm ? "CMDI_SAMPLER_DPM_SOLVER" : unipc ? "CMDI_SAMPLER_UNIPC" : sde ? "CMDI_SAMPLER_DPM_SOLVER_SDE"
+                                                                                     : "CMDI_SAMPLER_DDIM_REVERSE", bad);
     return 1;
   }
   if (dpm && (a->dpm_order < 1 || a->dpm_order > 3)) {
     set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
+    return 1;
+  }
+  if (sde && (a->dpm_order < 1 || a->dpm_order > 2)) {
+    set_last_error("dpm_order %d outside [1, 2] (CMDI_SAMPLER_DPM_SOLVER_SDE)", a->dpm_order);
     return 1;
   }
   if (unipc && (a->unipc_order < 1 || a->unipc_order > 3)) {
@@ -1558,8 +1603,8 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
   const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
   const int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
-  // PLMS / DPM-Solver++ / UniPC: a call without `resume` starts a new history at t0; a `resume` call continues the
-  // running one
+  // PLMS / DPM-Solver++ / UniPC / SDE-DPM-Solver++: a call without `resume` starts a new history at t0; a `resume` call
+  // continues the running one
   int hist_t0 = t0;
   if (multistep) {
     const int order = plms ? a->plms_order : unipc ? a->unipc_order : a->dpm_order;
@@ -1568,7 +1613,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
           e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
           t0 != e->hist_t_start - e->hist_steps) {
         set_last_error("%s resume at step %d does not continue the running history",
-                       plms ? "PLMS" : unipc ? "UniPC" : "DPM-Solver++", t0);
+                       plms ? "PLMS" : unipc ? "UniPC" : sde ? "SDE-DPM-Solver++" : "DPM-Solver++", t0);
         return 1;
       }
       hist_t0 = e->hist_t_start;
@@ -1576,8 +1621,9 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
       if (!e->hist) CKI(dev_alloc(e, &e->hist, 3 * slot));
       if ((plms || (unipc && a->unipc_corrector)) && !e->hist_keep) CKI(dev_alloc(e, &e->hist_keep, slot));
-      if (dpm) {
-        dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
+      if (dpm || sde) {  // one history runs at a time: the SDE table takes the same buffer
+        if (dpm) dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
+        else dpm_solver_sde_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
         CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
       }
       if (unipc) {
@@ -1650,7 +1696,9 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CKI(prepare_cond(e, B, a->cond_emb, host, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, t0, s));
-  CK(launch_set_int(e->step_ctr + 2, hist_t0, s));
+  // [2]: the history's first step (the call's for the single-step samplers), [3]: the call's first step, from which the
+  // per-step draws of SDE-DPM-Solver++ are numbered (they differ on a resume)
+  CK(launch_set_int(e->step_ctr + 2, hist_t0, s, t0));
   e->launches += 2;
 
   const float* tape = a->noise_tape;
@@ -1669,11 +1717,12 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     CKI(enqueue_eval(st, guided));
     StepParams sp = step_params(e, a, guided);
     sp.advance = 1; sp.sampler = a->sampler; sp.eta = a->eta;
-    sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;  // first step index: step_ctr[2] (graphs do not depend on it)
-    if (dpm) {
+    // first step index: step_ctr[2] (DDPM / DDIM) or step_ctr[3] (SDE-DPM-Solver++); graphs do not depend on it
+    sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
+    if (dpm || sde) {
       DpmParams q{};
       q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
-      CK(launch_dpm_solver_step(sp, q, st));
+      CK(dpm ? launch_dpm_solver_step(sp, q, st) : launch_dpm_solver_sde_step(sp, q, st));
     } else if (unipc) {
       UnipcParams q{};
       q.order = a->unipc_order; q.corrector = a->unipc_corrector;

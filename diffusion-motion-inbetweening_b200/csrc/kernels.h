@@ -203,8 +203,9 @@ struct RngState {
 };
 struct StepParams {
   StepTables tab;
-  int* step_ptr;            // device [3]: current step t (decremented by the kernel's last block when advance != 0),
-                            // block-arrival counter, first step index of the call
+  int* step_ptr;            // device [4]: current step t (decremented by the kernel's last block when advance != 0),
+                            // block-arrival counter, first step index of the running history (of the call for the
+                            // single-step samplers), first step index of the call
   int advance;
   int B, L, D, D_pad;
   int sampler;              // 0 = ancestral DDPM (p_sample), 1 = DDIM (ddim_sample_with_grad, cond_fn=None),
@@ -264,6 +265,12 @@ struct DpmParams {
   const float* coef;   // [T][4] (A, B0, B1, B2) per step index, for the running history
 };
 cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cudaStream_t stream);
+// SDE-DPM-Solver++ multistep step (Lu et al. 2022, the SDE solver in data prediction, orders 1..2) with
+// launch_diffusion_step's grid and per-step noise (noise_ref / rng; StepParams' sampler, eta and advance are not read;
+// x_next / x_next_hi are required): x_{s-1} = A_s x_s + B0_s m0 + B1_s m1 + Cn_s z, q.coef rows (A, B0, B1, Cn).  The
+// x0 history is DPM-Solver++'s ring; the draw z is number (first step of the call - s), the call's first step read
+// from step_ptr[3] when tape_t0 < 0.  Advances s -> s - 1.
+cudaError_t launch_dpm_solver_sde_step(const StepParams& p, const DpmParams& q, cudaStream_t stream);
 // UniPC step (Zhao et al. 2023, multistep, data prediction) from the same combine inputs as StepParams (its sampler,
 // eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are required).  After the pass at s on the
 // uncorrected x_s: x_s^c = Ac x_{s+1}^c + C0 m0 + C1 m1 + C2 m2 + C3 m3 (when a predictor step led into s and the
@@ -306,7 +313,8 @@ cudaError_t launch_axpby(const float* x, const float* y, float a, float b, float
 // standard normal fill (Philox4x32-10 + Box-Muller), value at flat index i of sample s depends on (seed, stream_id, s, i) only
 cudaError_t launch_fill_normal_ref(float* out, int B, size_t per_sample, unsigned long long seed,
                                    unsigned long long stream_id, unsigned long long sample_offset, cudaStream_t stream);
-cudaError_t launch_set_int(int* p, int v, cudaStream_t stream);
+// p[0] = v, p[1] = next
+cudaError_t launch_set_int(int* p, int v, cudaStream_t stream, int next = 0);
 
 // LayerNorm folded into its consumer: Wf = W * gamma (fp32 [N,K]), c[n] = sum_k Wf[n,k], d[n] = sum_k W[n,k] beta[k] + bias[n]
 cudaError_t launch_add_vectors(const float* a, const float* b, float* out, int n, cudaStream_t stream);

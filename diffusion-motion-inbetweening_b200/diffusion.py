@@ -6,11 +6,13 @@ Mirrors (same names, argument meaning and error behaviour; paths relative to the
     GaussianDiffusion  (sampling half)              :139-241, :311-349, :1149-1297, :1418-1587, :1589-1804
                                                     + dpm_solver_sample_loop[_progressive] (DPM-Solver++, not in the reference)
                                                     + unipc_sample_loop[_progressive] (UniPC, not in the reference)
+                                                    + dpm_solver_sde_sample_loop[_progressive] (SDE-DPM-Solver++,
+                                                      not in the reference)
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
 `p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` / `dpm_solver_sample_loop` /
-`unipc_sample_loop` run the WHOLE loop in one native
+`unipc_sample_loop` / `dpm_solver_sde_sample_loop` run the WHOLE loop in one native
 call (`cmdi_sample`): no per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
 `p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` / `ddim_reverse_sample` is done by the CUDA
@@ -245,12 +247,14 @@ class GaussianDiffusion:
         if plms or rev or dpm or unipc:
             # plms_sample_loop_progressive draws nothing after x_T (:1767-1770): a tape contributes tape[0] only, torch's
             # generator has moved by the one randn(*shape) above, and the engine generator draws x_T when rng="engine".
-            # DPM-Solver++ and UniPC behave the same way.  DDIM inversion draws nothing at all: x_T is the caller's state
+            # DPM-Solver++ and UniPC behave the same way.  DDIM inversion draws nothing at all: x_T is the caller's state.
+            # (SDE-DPM-Solver++ draws like p_sample_loop: the branch below.)
             tape = None
             if x_T is None:
                 seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         elif tape is None:
-            n_draws = self.num_timesteps - skip_timesteps  # one randn_like per loop iteration (:696, :1407)
+            # one randn_like per loop iteration (:696, :1407); SDE-DPM-Solver++ draws the same way
+            n_draws = self.num_timesteps - skip_timesteps
             rng_args = _torch_stream_args(device, int(np.prod(shape)), n_draws, lazy=progressive) if self.rng == "torch" else None
             if rng_args is None:
                 if x_T is not None and noise is None:
@@ -277,7 +281,7 @@ class GaussianDiffusion:
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
-        if plms or dpm:
+        if plms or dpm or sampler == capi.SAMPLER_DPM_SOLVER_SDE:
             common["plms_order" if plms else "dpm_order"] = int(order)
         if unipc:
             common.update(unipc_order=int(order), unipc_variant=capi.UNIPC_BH1 if variant == "bh1" else capi.UNIPC_BH2,
@@ -295,8 +299,8 @@ class GaussianDiffusion:
     def _step_generator(self, eng, x_T, init_image, skip_timesteps, tape, common):
         """Generator form of every sampler: one native call per step (slower than the fused loop; kept for API parity),
         each starting from the previous call's sample and replaying the same step graph.  The multistep samplers
-        (PLMS, DPM-Solver++, UniPC) continue the history the engine keeps on the device (UniPC's corrected state
-        included), and DDIM inversion draws nothing, so
+        (PLMS, DPM-Solver++ as ODE and SDE, UniPC) continue the history the engine keeps on the device (UniPC's
+        corrected state included), and DDIM inversion draws nothing, so
         their samples equal the fused loop's bit for bit; a caller that stops an inversion early has a partial one.
         PLMS also yields old_eps, the values of the reference's history list at that yield (the reference yields one
         list it keeps mutating)."""
@@ -402,6 +406,32 @@ class GaussianDiffusion:
         return self._run(capi.SAMPLER_DPM_SOLVER, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
                          init_image, randomize_class, None, False, 0.0, progressive=True, order=order)
 
+    def dpm_solver_sde_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                                   model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                                   randomize_class=False, cond_fn_with_grad=False, const_noise=False, order=2):
+        """SDE-DPM-Solver++ multistep (Lu et al. 2022; the SDE solver in data prediction, midpoint form) on this object's
+        spaced steps, orders 1-2: one denoiser pass per step, through the same x0 pipeline as p_sample_loop (CFG,
+        keyframe input, imputation, reconstruction guidance).  Stochastic, with p_sample_loop's noise: one randn(*shape)
+        for x_T, then one randn_like per step including the last, from the same source (`rng`, `noise_tape`).  Order 1 is
+        p_sample_loop's posterior step; order 2 is second-order accurate in the step size.  The whole loop is one native
+        call and the x0 history stays on the device.  (The reference has no such sampler.)"""
+        _check_sde_order(order)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DPM_SOLVER_SDE, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, const_noise, 0.0, order=order)["sample"]
+
+    def dpm_solver_sde_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                               cond_fn=None, model_kwargs=None, device=None, progress=False,
+                                               skip_timesteps=0, init_image=None, randomize_class=False,
+                                               cond_fn_with_grad=False, const_noise=False, order=2):
+        """Yields {"sample", "pred_xstart"} per step of dpm_solver_sde_sample_loop, one native call per step; the samples
+        equal the fused loop's bit for bit, and torch's generator moves one randn_like per yielded step, as
+        p_sample_loop_progressive moves it.  The configuration is validated at the call."""
+        _check_sde_order(order)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_DPM_SOLVER_SDE, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, const_noise, 0.0, progressive=True, order=order)
+
     def unipc_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
                           model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
                           randomize_class=False, cond_fn_with_grad=False, order=2, variant="bh2", corrector=True):
@@ -484,6 +514,12 @@ def _check_dpm_order(order) -> None:
     """DPM-Solver++'s multistep orders are 1, 2 and 3 (an int; bools and floats are refused)."""
     if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2, 3):
         raise ValueError(f"DPM-Solver++ order must be an int in {{1, 2, 3}}, got {order!r}")
+
+
+def _check_sde_order(order) -> None:
+    """SDE-DPM-Solver++'s multistep orders are 1 and 2 (an int; bools and floats are refused)."""
+    if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2):
+        raise ValueError(f"SDE-DPM-Solver++ order must be an int in {{1, 2}}, got {order!r}")
 
 
 def _check_unipc_args(order, variant, corrector) -> None:

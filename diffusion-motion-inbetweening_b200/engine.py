@@ -135,7 +135,9 @@ class Engine:
         sampler=SAMPLER_DDIM_REVERSE: DDIM inversion from the state x_T, ascending from t = skip_timesteps; plms_order
         is not sent.
         sampler=SAMPLER_DPM_SOLVER: DPM-Solver++ multistep of order `dpm_order` (1-3); resume continues its x0 history.
-        dpm_order is sent for this sampler only, plms_order for the others.
+        sampler=SAMPLER_DPM_SOLVER_SDE: SDE-DPM-Solver++ of order `dpm_order` (1-2), with DDPM's per-step draws
+        (noise_tape, seed / rng_mode); resume continues its x0 history.
+        dpm_order is sent for these two samplers only, plms_order for the others.
         sampler=SAMPLER_UNIPC: UniPC of order `unipc_order` (1-3), variant `unipc_variant` (UNIPC_BH1 / UNIPC_BH2), with
         or without the corrector; resume continues its x0 history and corrected state.  The unipc_* fields are sent
         for this sampler only.
@@ -193,6 +195,7 @@ class Engine:
             n_old = min(plms_steps, int(plms_order) - 1)  # the length of the reference's list after that many steps
             old_eps = torch.empty((max(n_old, 1),) + shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
         unipc = sampler == capi.SAMPLER_UNIPC
+        dpm = sampler in (capi.SAMPLER_DPM_SOLVER, capi.SAMPLER_DPM_SOLVER_SDE)
         a = capi.SampleArgs(batch, sampler, float(eta), int(skip_timesteps), int(num_steps), int(resume), _ptr(init_image), _ptr(x_T), _ptr(noise_tape),
                             int(seed) & (2 ** 64 - 1), int(sample_offset), int(rng_mode), int(aten_offset), int(aten_increment),
                             int(aten_threads), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale),
@@ -200,9 +203,8 @@ class Engine:
                             _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
                             dump_arr, n_dump, int(host_buffers),
                             int(use_graph), _ptr(obs_x0), _ptr(obs_mask),
-                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_DPM_SOLVER, capi.SAMPLER_UNIPC)
-                            else int(plms_order),
-                            _ptr(old_eps), int(dpm_order) if sampler == capi.SAMPLER_DPM_SOLVER else 0,
+                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_UNIPC) or dpm else int(plms_order),
+                            _ptr(old_eps), int(dpm_order) if dpm else 0,
                             int(unipc_order) if unipc else 0, int(unipc_variant) if unipc else 0,
                             int(unipc_corrector) if unipc else 0)
         with torch.cuda.device(self.device):

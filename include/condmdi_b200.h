@@ -71,8 +71,15 @@ enum {
    corrected state stays on the device; the last step returns x0 as DDIM's does.  skip_timesteps / init_image / resume
    as for DPM_SOLVER; eta must be 0 and noise_tape, dump_xstart, plms_order, plms_old_eps_out and dpm_order unset: the
    call fails naming the field otherwise. */
+/* DPM_SOLVER_SDE: SDE-DPM-Solver++ (Lu et al. 2022; the SDE multistep solver in data prediction, midpoint form) on the
+   spaced steps, orders 1..2 (dpm_order), one denoiser pass per step.  Stochastic like DDPM, with DDPM's noise contract:
+   one draw per step including the last (tape, CMDI_RNG_TORCH stream or engine generator, numbered from the call's
+   first step), whose value the last step does not use.  Order 1 is the DDPM posterior step.  The step at s uses order
+   min(dpm_order, iterations since the history started + 1, s + 1); the last step returns x0.  skip_timesteps /
+   init_image / resume as for DPM_SOLVER; eta must be 0 and dump_xstart, plms_order, plms_old_eps_out and the unipc_*
+   fields unset: the call fails naming the field otherwise. */
 enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3,
-       CMDI_SAMPLER_DPM_SOLVER = 4, CMDI_SAMPLER_UNIPC = 5 };
+       CMDI_SAMPLER_DPM_SOLVER = 4, CMDI_SAMPLER_UNIPC = 5, CMDI_SAMPLER_DPM_SOLVER_SDE = 6 };
 enum { CMDI_UNIPC_BH1 = 1, CMDI_UNIPC_BH2 = 2 };  /* unipc_variant: B(h) = h or e^h - 1 */
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
@@ -172,9 +179,9 @@ typedef struct {
   int32_t plms_order;           /* 2..4 (plms_sample's `order`) */
   float* plms_old_eps_out;      /* NULL, or (min(steps so far, plms_order - 1), B, 263, 1, 196): the reference's old_eps
                                    list after the last step, oldest first (ref layout) */
-  /* CMDI_SAMPLER_DPM_SOLVER only (0 for every other sampler).  The x0 history stays on the device like PLMS's eps
-     history: resume = 1 continues it with the same order and batch. */
-  int32_t dpm_order;            /* 1..3 */
+  /* CMDI_SAMPLER_DPM_SOLVER and CMDI_SAMPLER_DPM_SOLVER_SDE only (0 for every other sampler).  The x0 history stays on
+     the device like PLMS's eps history: resume = 1 continues it with the same sampler, order and batch. */
+  int32_t dpm_order;            /* 1..3 (DPM_SOLVER), 1..2 (DPM_SOLVER_SDE) */
   /* CMDI_SAMPLER_UNIPC only (all 0 for every other sampler).  The x0 history and the corrected state stay on the device:
      resume = 1 continues them with the same order, variant, corrector and batch. */
   int32_t unipc_order;          /* 1..3 */
