@@ -18,10 +18,11 @@ from .diffusion import GaussianDiffusion, from_reference_diffusion
 _LOOPS = ("p_sample_loop", "p_sample_loop_progressive", "ddim_sample_loop", "ddim_sample_loop_progressive",
           "plms_sample_loop", "plms_sample_loop_progressive")
 # loops the reference lacks: DDIM inversion (it has the step, ddim_reverse_sample, which install() leaves as it is) and
-# the DPM-Solver++, UniPC and SDE-DPM-Solver++ multistep samplers
+# the DPM-Solver++, UniPC and SDE-DPM-Solver++ multistep samplers, and RePaint resampling
 _ADDED_LOOPS = ("ddim_reverse_sample_loop", "ddim_reverse_sample_loop_progressive", "dpm_solver_sample_loop",
                 "dpm_solver_sample_loop_progressive", "unipc_sample_loop", "unipc_sample_loop_progressive",
-                "dpm_solver_sde_sample_loop", "dpm_solver_sde_sample_loop_progressive")
+                "dpm_solver_sde_sample_loop", "dpm_solver_sde_sample_loop_progressive", "repaint_sample_loop",
+                "repaint_sample_loop_progressive")
 
 
 def accelerate(ref_diffusion):
@@ -34,8 +35,8 @@ def accelerate(ref_diffusion):
 def install(ref_diffusion, fallback_to_reference: bool = False):
     """Replace the six sampling loops (DDPM, DDIM, PLMS and their progressive forms) of a reference diffusion object by
     the engine's, in place, and add the engine's DDIM inversion loops (ddim_reverse_sample_loop[_progressive]),
-    DPM-Solver++ loops (dpm_solver_sample_loop[_progressive]), UniPC loops (unipc_sample_loop[_progressive]) and
-    SDE-DPM-Solver++ loops (dpm_solver_sde_sample_loop[_progressive]).
+    DPM-Solver++ loops (dpm_solver_sample_loop[_progressive]), UniPC loops (unipc_sample_loop[_progressive]),
+    SDE-DPM-Solver++ loops (dpm_solver_sde_sample_loop[_progressive]) and RePaint loops (repaint_sample_loop[_progressive]).
 
     Configurations the engine does not implement raise NotImplementedError.  With fallback_to_reference=True those
     (and only those) are forwarded to the reference's original PyTorch loop instead -- an explicit opt-in for

@@ -22,6 +22,7 @@ SAMPLER_DDIM_REVERSE = 3  # DDIM inversion x_t -> x_{t+1} (ddim_reverse_sample);
 SAMPLER_DPM_SOLVER = 4  # DPM-Solver++ multistep, orders 1-3 (dpm_order)
 SAMPLER_UNIPC = 5  # UniPC predictor-corrector, orders 1-3 (unipc_order, unipc_variant, unipc_corrector)
 SAMPLER_DPM_SOLVER_SDE = 6  # SDE-DPM-Solver++ multistep, orders 1-2 (dpm_order); DDPM's per-step draws
+SAMPLER_REPAINT = 7  # RePaint resampling around DDPM (repaint_jump_length, repaint_jump_n_sample); one draw per walk op
 UNIPC_BH1, UNIPC_BH2 = 1, 2  # unipc_variant
 ARCH_TRANS_ENC, ARCH_UNET = 0, 1
 MOTION_ABS3D_TO_REL, MOTION_REL_TO_ABS3D, MOTION_REL_TO_JOINTS, MOTION_ABS3D_TO_JOINTS = 0, 1, 2, 3
@@ -62,7 +63,8 @@ class SampleArgs(Structure):
                 ("dump_xstart", c_void_p), ("dump_steps", POINTER(c_int32)), ("n_dump", c_int32),
                 ("host_buffers", c_int32), ("use_graph", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p),
                 ("plms_order", c_int32), ("plms_old_eps_out", c_void_p), ("dpm_order", c_int32),
-                ("unipc_order", c_int32), ("unipc_variant", c_int32), ("unipc_corrector", c_int32)]
+                ("unipc_order", c_int32), ("unipc_variant", c_int32), ("unipc_corrector", c_int32),
+                ("repaint_jump_length", c_int32), ("repaint_jump_n_sample", c_int32)]
 
 
 class LibraryMissing(RuntimeError):

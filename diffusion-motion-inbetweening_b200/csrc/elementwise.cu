@@ -693,6 +693,97 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
 }
 
 // ---------------------------------------------------------------------------------------------
+// RePaint resampling (Lugmayr et al. 2022, "time travel"): one op of the walk (engine.cu, repaint_walk) at the position
+// s = step_ptr[0], on frame-major state [B*L, D_pad], with diffusion_step_kernel's grid, block and noise tile.
+//   phase 0  denoise at s: p_sample at s with diffusion_step_kernel's DDPM arithmetic (x0 through load_step_x0, so
+//            CFG, keyframe input, imputation and guidance as in DDPM; at s = 0 the sample is x0); s -> s - 1
+//   phase 1  undo into u = s + 1: x <- a_u x + b_u z, one forward step of the spaced chain (non-contracted fp32,
+//            multiply then add); pred_xstart is left as it is; s -> s + 1
+// Every op takes one draw.  d = step_ptr[5] is the op's index in the walk started at t0 = step_ptr[2], and step_ptr[4]
+// the index of the call's first op, so the draw is number d - step_ptr[4] of the call (tape slice, torch.randn_like
+// stream).  The engine generator gives the first denoise op at s p_sample_loop's stream for step s (s + 1) and every
+// other op the stream kWalkStream + 1 + d, which no step reaches.  The first visit of s is op (t0 - s) + 2 j (r - 1) n_s,
+// n_s the number of jump points t >= s (t % j == 0, t + j <= t0).  fill_noise_tile numbers the draw (tape_t0 - t) and
+// keys the stream t + 1, so it is called with t = key and tape_t0 = key + draw number.
+// ---------------------------------------------------------------------------------------------
+constexpr int kWalkStream = 1 << 30;
+
+// advance_step for a walk op: the last block to arrive also moves the walk index step_ptr[5] to the next op.  (A copy,
+// not an option of advance_step, so the six step kernels that use advance_step compile as before.)
+__device__ __forceinline__ void advance_walk(int* step_ptr, int next) {
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0 && threadIdx.y == 0) {
+    const unsigned int total = gridDim.x * gridDim.y * gridDim.z;
+    unsigned int* counter = reinterpret_cast<unsigned int*>(step_ptr + 1);
+    if (atomicAdd(counter, 1u) == total - 1) {
+      *counter = 0;
+      *step_ptr = next;
+      step_ptr[5] += 1;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) repaint_step_kernel(const StepParams p, const RepaintParams q) {
+  griddep_launch_dependents();
+  griddep_wait();
+  __shared__ float s_noise[32][33];
+  const int b = blockIdx.z;
+  const int l0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int s = *p.step_ptr;
+  const int t0 = p.step_ptr[2], d = p.step_ptr[5];
+  const int j = q.jump_length;
+  const bool denoise = q.phase == 0;
+  const bool first = denoise && d == t0 - s + 2 * j * (q.jump_n_sample - 1) * max(0, t0 / j - (s + j - 1) / j);
+  const int key = first ? s : kWalkStream + d;
+  fill_noise_tile(p, key, key + (d - p.step_ptr[4]), b, l0, c0, s_noise);
+  __syncthreads();
+
+  // per-op scalars: DDPM's (gathered like _extract_into_tensor(...).float()) or the undo row of s + 1
+  float coef1 = 0.f, coef2 = 0.f, logvar = 0.f, ua = 0.f, ub = 0.f;
+  if (denoise) {
+    coef1 = p.tab.post_coef1[s]; coef2 = p.tab.post_coef2[s]; logvar = p.tab.post_logvar[s];
+  } else {
+    ua = q.undo_coef[(size_t)(s + 1) * 4]; ub = q.undo_coef[(size_t)(s + 1) * 4 + 1];
+  }
+  const float nonzero = (s != 0) ? 1.0f : 0.0f;
+  {
+    const int tid = ty * 32 + tx;
+    const int ll = tid >> 3, cq = (tid & 7) * 4;
+    const int l = l0 + ll, c = c0 + cq;
+    if (l < p.L && c < p.D_pad) {
+      const size_t idx = ((size_t)b * p.L + l) * p.D_pad + c;
+      float xtv[4], x04[4] = {0.f, 0.f, 0.f, 0.f}, xn4[4];
+      if (denoise) {
+        load_step_x0(p, idx, b, c, s, xtv, x04);
+      } else {
+        const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+        xtv[0] = xt4.x; xtv[1] = xt4.y; xtv[2] = xt4.z; xtv[3] = xt4.w;
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        float xn = 0.f;
+        if (c + jj < p.D) {
+          const float noise = s_noise[cq + jj][ll];
+          if (denoise) {
+            // diffusion_step_kernel's DDPM branch: mean = coef1*x0 + coef2*x_t; sample = mean + nonzero*exp(0.5*logvar)*z
+            const float mean = __fadd_rn(__fmul_rn(coef1, x04[jj]), __fmul_rn(coef2, xtv[jj]));
+            const float sd = expf(__fmul_rn(0.5f, logvar));
+            xn = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sd), noise));
+          } else {
+            xn = __fadd_rn(__fmul_rn(ua, xtv[jj]), __fmul_rn(ub, noise));
+          }
+        }
+        xn4[jj] = xn;
+      }
+      store_step_state(p, idx, xn4, x04, denoise);
+    }
+  }
+  advance_walk(p.step_ptr, denoise ? s - 1 : s + 1);
+}
+
+// ---------------------------------------------------------------------------------------------
 // layout converters (32x32 smem tile transposes)
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) ref_to_frames_kernel(const float* __restrict__ ref, int B, int D, int L, int D_pad,
@@ -977,6 +1068,14 @@ cudaError_t launch_dpm_solver_sde_step(const StepParams& p, const DpmParams& q, 
     return cudaErrorInvalidValue;
   dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
   return launch_kernel(dpm_solver_sde_step_kernel, grid, block, 0, stream, p, q);
+}
+
+cudaError_t launch_repaint_step(const StepParams& p, const RepaintParams& q, cudaStream_t stream) {
+  if (q.phase < 0 || q.phase > 1 || q.jump_length < 1 || q.jump_n_sample < 1 || (p.D_pad & 3) || !p.x_next ||
+      !p.x_next_hi || !q.undo_coef)
+    return cudaErrorInvalidValue;
+  dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
+  return launch_kernel(repaint_step_kernel, grid, block, 0, stream, p, q);
 }
 
 cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStream_t stream) {

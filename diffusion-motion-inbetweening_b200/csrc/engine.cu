@@ -98,7 +98,14 @@ struct GraphKey {
   int order, plms_phase, guided2;  // PLMS / DPM-Solver++ / UniPC: order; PLMS: step kind (PlmsStep), guidance of the first
                                    // step's second evaluation
   int variant, corrector;          // UniPC
+  int jump_length, jump_n_sample;  // RePaint
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
+};
+
+// One op of a RePaint walk: denoise at p (the position moves p -> p - 1) or undo into p (p - 1 -> p).
+struct WalkOp {
+  int p;
+  bool undo;
 };
 
 }  // namespace
@@ -146,7 +153,8 @@ struct cmdi_engine {
   CUtensorMap xseq_st{}, x1_st{};  // fp32 TMA-store targets: xseq (backward pass), x1 (v1 of the chained forward path)
   uint8_t* obs_mask = nullptr;
   float *cond_emb = nullptr, *cond_proj = nullptr, *text_scale = nullptr;
-  int* step_ctr = nullptr;  // [4]: step index, block-arrival counter, first step of the running history, of the call
+  int* step_ctr = nullptr;  // [6]: step index, block-arrival counter, first step of the running history, of the call;
+                            // RePaint: walk index of the call's first op, of the next op
   RngState* rng = nullptr;  // generator state of the running loop (device-resident: step graphs do not depend on it)
   float *ref_a = nullptr, *ref_b = nullptr;  // reference-layout staging [maxB, D, L]
   uint8_t *ref_mask = nullptr, *ymask = nullptr;
@@ -186,8 +194,13 @@ struct cmdi_engine {
   bool hist_live = false;
   int hist_sampler = 0, hist_order = 0, hist_B = 0, hist_t_start = 0, hist_steps = 0;
   int hist_variant = 0, hist_corrector = 0;  // UniPC
+  int hist_jump_n_sample = 0;                // RePaint (hist_order holds its jump length)
+  std::vector<WalkOp> walk;                  // RePaint: the running walk and the index of its next op
+  size_t walk_next = 0;
+  std::vector<double> h_betas;     // betas of the schedule (float64)
   std::vector<double> h_acp;       // alphas_cumprod of the schedule (float64)
-  std::vector<float> h_dpm_coef;   // [T][4] DPM-Solver++ (or SDE-DPM-Solver++) coefficients of the running history
+  // [T][4] DPM-Solver++ (or SDE-DPM-Solver++) coefficients of the running history, or RePaint's undo coefficients
+  std::vector<float> h_dpm_coef;
   float* dpm_coef = nullptr;       // their device copy
   std::vector<float> h_unipc_coef; // [T][12] UniPC coefficients of the running history
   float* unipc_coef = nullptr;     // their device copy (allocated by the first UniPC call on a schedule)
@@ -848,7 +861,7 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
   A(dev_alloc(e, &e->cond_emb, (size_t)e->maxB * 512));
   A(dev_alloc(e, &e->cond_proj, (size_t)e->maxB * kDModel));
   A(dev_alloc(e, &e->text_scale, e->maxB));
-  A(dev_alloc(e, &e->step_ctr, 4));
+  A(dev_alloc(e, &e->step_ctr, 6));
   A(dev_alloc(e, &e->rng, 1));
   // chained forward path: folded weights, partial row statistics, dependency counters
   e->f_qkv.resize(e->layers);
@@ -1084,6 +1097,7 @@ extern "C" int cmdi_set_schedule(cmdi_engine* e, const double* betas_in, int T, 
     e->h_sqrt_acp[i] = std::sqrt(acp[i]);
     e->h_sqrt_1m_acp[i] = std::sqrt(1.0 - acp[i]);
   }
+  e->h_betas = betas;
   e->h_acp = acp;
   if (e->tables) cudaFree(e->tables);
   if (e->d_tmap) cudaFree(e->d_tmap);
@@ -1392,23 +1406,45 @@ void unipc_coefs(const std::vector<double>& acp, int t_start, int order, int var
   }
 }
 
-// The first argument the samplers added to the reference's (DPM-Solver++ as ODE and SDE, UniPC, DDIM inversion) have no
-// use for but the caller set, or null.
+// RePaint's resampling schedule (Lugmayr et al. 2022, "time travel") from position t0, with jump length j and
+// jump_n_sample r: descend one denoise op at a time; the first time the walk arrives at a jump point t (t % j == 0 and
+// t + j <= t0), go up j positions by undo ops and come back down by denoise ops, r - 1 times, then continue the descent.
+// With K = t0 / j jump points (none when j > t0) that is t0 + 1 + (r - 1) j K denoise ops and (r - 1) j K undo ops; with
+// r = 1 it is p_sample_loop's descent.  The walk ends at position -1, after the denoise op at 0.
+std::vector<WalkOp> repaint_walk(int t0, int j, int r) {
+  std::vector<WalkOp> w;
+  for (int p = t0; p >= 0; --p) {
+    if (p % j == 0 && p + j <= t0) {
+      for (int n = 1; n < r; ++n) {
+        for (int u = p + 1; u <= p + j; ++u) w.push_back({u, true});
+        for (int u = p + j; u > p; --u) w.push_back({u, false});
+      }
+    }
+    w.push_back({p, false});
+  }
+  return w;
+}
+
+// The first argument the samplers added to the reference's (DPM-Solver++ as ODE and SDE, UniPC, DDIM inversion,
+// RePaint) have no use for but the caller set, or null.
 const char* field_to_unset(const cmdi_sample_args* a) {
   const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER, rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
   const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC, sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
-  if (!dpm && !rev && !unipc && !sde) return nullptr;
+  const bool repaint = a->sampler == CMDI_SAMPLER_REPAINT;
+  if (!dpm && !rev && !unipc && !sde && !repaint) return nullptr;
   if (a->eta != 0.f)
     return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
            : unipc ? "eta (UniPC is deterministic after x_T: eta must be 0)"
            : sde ? "eta (the SDE solver's noise is fixed by the schedule: eta must be 0)"
+           : repaint ? "eta (RePaint denoises with p_sample: eta must be 0)"
                  : "eta (the reverse ODE is deterministic: eta must be 0)";
-  if (a->noise_tape && !sde) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
+  if (a->noise_tape && !sde && !repaint) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
   if (rev && a->init_image) return "init_image";
   if (a->dump_xstart) return "dump_xstart";
   if (a->plms_order) return "plms_order";
   if (a->plms_old_eps_out) return "plms_old_eps_out";
-  if ((dpm || unipc || sde) && a->resume && a->init_image) return "init_image (a resume call continues the running state)";
+  if ((dpm || unipc || sde || repaint) && a->resume && a->init_image)
+    return "init_image (a resume call continues the running state)";
   return nullptr;
 }
 
@@ -1451,6 +1487,7 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.guided = guided; key.group = group;
   key.order = plms ? a->plms_order : a->sampler == CMDI_SAMPLER_UNIPC ? a->unipc_order : a->dpm_order;
   key.variant = a->unipc_variant; key.corrector = a->unipc_corrector;
+  key.jump_length = a->repaint_jump_length; key.jump_n_sample = a->repaint_jump_n_sample;
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
@@ -1512,7 +1549,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CKI(check_ready(e, B, true));
   if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
       a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER && a->sampler != CMDI_SAMPLER_UNIPC &&
-      a->sampler != CMDI_SAMPLER_DPM_SOLVER_SDE) {
+      a->sampler != CMDI_SAMPLER_DPM_SOLVER_SDE && a->sampler != CMDI_SAMPLER_REPAINT) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
@@ -1521,7 +1558,9 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
   // SDE-DPM-Solver++: DPM-Solver++'s x0 history, with DDPM's per-step draws
   const bool sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
-  const bool multistep = plms || dpm || unipc || sde;  // samplers with a device-resident history
+  // RePaint: p_sample steps and undo ops along a walk that revisits steps; its running walk is its history
+  const bool repaint = a->sampler == CMDI_SAMPLER_REPAINT;
+  const bool multistep = plms || dpm || unipc || sde || repaint;  // samplers with a device-resident history
   // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
   // nothing and has no q_sample, dump or PLMS history
   const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
@@ -1535,10 +1574,20 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
                    a->unipc_order ? "unipc_order" : a->unipc_variant ? "unipc_variant" : "unipc_corrector", a->sampler);
     return 1;
   }
+  if (!repaint && (a->repaint_jump_length || a->repaint_jump_n_sample)) {
+    set_last_error("%s is a CMDI_SAMPLER_REPAINT field: it must be 0 for sampler %d",
+                   a->repaint_jump_length ? "repaint_jump_length" : "repaint_jump_n_sample", a->sampler);
+    return 1;
+  }
   if (const char* bad = field_to_unset(a)) {
     set_last_error("%s: %s must be unset",
                    dpm ? "CMDI_SAMPLER_DPM_SOLVER" : unipc ? "CMDI_SAMPLER_UNIPC" : sde ? "CMDI_SAMPLER_DPM_SOLVER_SDE"
-                                                                                     : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+                   : repaint ? "CMDI_SAMPLER_REPAINT" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+    return 1;
+  }
+  if (repaint && (a->repaint_jump_length < 1 || a->repaint_jump_n_sample < 1)) {
+    set_last_error("%s %d must be >= 1", a->repaint_jump_length < 1 ? "repaint_jump_length" : "repaint_jump_n_sample",
+                   a->repaint_jump_length < 1 ? a->repaint_jump_length : a->repaint_jump_n_sample);
     return 1;
   }
   if (dpm && (a->dpm_order < 1 || a->dpm_order > 3)) {
@@ -1602,24 +1651,51 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   const size_t n = (size_t)B * e->D * e->L;
   const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
   const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
-  const int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
-  // PLMS / DPM-Solver++ / UniPC / SDE-DPM-Solver++: a call without `resume` starts a new history at t0; a `resume` call
-  // continues the running one
+  int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
+  // PLMS / DPM-Solver++ / UniPC / SDE-DPM-Solver++ / RePaint: a call without `resume` starts a new history at t0; a
+  // `resume` call continues the running one
   int hist_t0 = t0;
   if (multistep) {
-    const int order = plms ? a->plms_order : unipc ? a->unipc_order : a->dpm_order;
+    const int order = plms ? a->plms_order : unipc ? a->unipc_order : repaint ? a->repaint_jump_length : a->dpm_order;
     if (a->resume) {
+      // a RePaint walk resumes at the position its next op starts from: p for a denoise op at p, p - 1 for an undo op
+      // into p
+      const bool at = !repaint ? t0 == e->hist_t_start - e->hist_steps
+                               : e->walk_next < e->walk.size() &&
+                                     t0 == e->walk[e->walk_next].p - (e->walk[e->walk_next].undo ? 1 : 0);
       if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
           e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
-          t0 != e->hist_t_start - e->hist_steps) {
+          e->hist_jump_n_sample != a->repaint_jump_n_sample || !at) {
         set_last_error("%s resume at step %d does not continue the running history",
-                       plms ? "PLMS" : unipc ? "UniPC" : sde ? "SDE-DPM-Solver++" : "DPM-Solver++", t0);
+                       plms ? "PLMS" : unipc ? "UniPC" : sde ? "SDE-DPM-Solver++" : repaint ? "RePaint" : "DPM-Solver++", t0);
         return 1;
       }
       hist_t0 = e->hist_t_start;
     } else {
       const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
-      if (!e->hist) CKI(dev_alloc(e, &e->hist, 3 * slot));
+      if (repaint) {
+        // the walk's ops are numbered in device memory and its engine-generator streams start at 2^30 (the
+        // kernel's kWalkStream): 2^28 ops are far more than any schedule needs
+        const long long j = a->repaint_jump_length, r = a->repaint_jump_n_sample;
+        const long long ops = t0 + 1 + 2 * (r - 1) * j * (j <= t0 ? t0 / j : 0);
+        if (ops > (1LL << 28)) {
+          set_last_error("repaint_jump_length %d and repaint_jump_n_sample %d give a walk of %lld ops (at most 2^28)",
+                         a->repaint_jump_length, a->repaint_jump_n_sample, ops);
+          return 1;
+        }
+        e->walk = repaint_walk(t0, a->repaint_jump_length, a->repaint_jump_n_sample);
+        e->walk_next = 0;
+        // undo into p: x <- a_p x + b_p z, a_p = fp32(sqrt(1 - beta_p)), b_p = fp32(sqrt(beta_p)); one history runs at a
+        // time, so the table takes DPM-Solver++'s buffer
+        e->h_dpm_coef.assign((size_t)4 * e->T, 0.f);
+        for (int p = 0; p < e->T; ++p) {
+          e->h_dpm_coef[(size_t)4 * p] = (float)std::sqrt(1.0 - e->h_betas[p]);
+          e->h_dpm_coef[(size_t)4 * p + 1] = (float)std::sqrt(e->h_betas[p]);
+        }
+        CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
+      } else if (!e->hist) {
+        CKI(dev_alloc(e, &e->hist, 3 * slot));
+      }
       if ((plms || (unipc && a->unipc_corrector)) && !e->hist_keep) CKI(dev_alloc(e, &e->hist_keep, slot));
       if (dpm || sde) {  // one history runs at a time: the SDE table takes the same buffer
         if (dpm) dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
@@ -1634,7 +1710,13 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       e->hist_live = true;
       e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
       e->hist_variant = a->unipc_variant; e->hist_corrector = a->unipc_corrector;
+      e->hist_jump_n_sample = a->repaint_jump_n_sample;
     }
+  }
+  if (repaint) {  // num_steps counts denoise ops
+    int left = 0;
+    for (size_t i = e->walk_next; i < e->walk.size(); ++i) left += e->walk[i].undo ? 0 : 1;
+    nsteps = (a->num_steps > 0 && a->num_steps < left) ? a->num_steps : left;
   }
   CKI(ensure_temb(e, s));
   CKI(prepare_chain(e, a->cfg ? 2 * B : B));
@@ -1700,6 +1782,11 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   // per-step draws of SDE-DPM-Solver++ are numbered (they differ on a resume)
   CK(launch_set_int(e->step_ctr + 2, hist_t0, s, t0));
   e->launches += 2;
+  if (repaint) {
+    // [4]: the walk index of the call's first op, from which its draws are numbered, [5]: that of the next op
+    CK(launch_set_int(e->step_ctr + 4, (int)e->walk_next, s, (int)e->walk_next));
+    e->launches += 1;
+  }
 
   const float* tape = a->noise_tape;
   if (tape && host) {
@@ -1713,13 +1800,19 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     if (guided) CKI(run_backward(e, B, a->cfg != 0, st));
     return 0;
   };
+  // RePaint's two ops; the walk position and the draw number live in step_ctr
+  RepaintParams rq{};
+  rq.jump_length = a->repaint_jump_length; rq.jump_n_sample = a->repaint_jump_n_sample; rq.undo_coef = e->dpm_coef;
   auto enqueue_step = [&](cudaStream_t st, bool guided) -> int {
     CKI(enqueue_eval(st, guided));
     StepParams sp = step_params(e, a, guided);
     sp.advance = 1; sp.sampler = a->sampler; sp.eta = a->eta;
     // first step index: step_ctr[2] (DDPM / DDIM) or step_ctr[3] (SDE-DPM-Solver++); graphs do not depend on it
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
-    if (dpm || sde) {
+    if (repaint) {
+      rq.phase = 0;
+      CK(launch_repaint_step(sp, rq, st));
+    } else if (dpm || sde) {
       DpmParams q{};
       q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
       CK(dpm ? launch_dpm_solver_step(sp, q, st) : launch_dpm_solver_sde_step(sp, q, st));
@@ -1759,7 +1852,32 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   int dump_i = 0;
   // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
   auto guided_at = [&](int k) { return a->recon_guidance && (rev ? t0 + k : t0 - k) >= a->stop_recguidance_at; };
-  for (int k = 0; k < nsteps;) {
+  // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
+  // launch each; a denoise op is one evaluation and the step kernel, guided by its position, through the step graphs.
+  // A graph holds one denoise op.
+  for (int k = 0; repaint && k < nsteps; ++e->walk_next) {
+    const WalkOp op = e->walk[e->walk_next];
+    if (op.undo) {
+      StepParams sp = step_params(e, a, false);
+      sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
+      rq.phase = 1;
+      CK(launch_repaint_step(sp, rq, s));
+      e->launches += 1;
+      continue;
+    }
+    const bool guided = a->recon_guidance && op.p >= a->stop_recguidance_at;
+    const GraphKey key = step_graph_key(a, guided, 1, 0, false);
+    if (step_uses_graph(a->use_graph, e->no_graph, nsteps, tape, e->graphs.count(key) != 0)) {
+      cudaGraphExec_t exec = nullptr;
+      CKI(capture_step_graph(e, key, [&](cudaStream_t cs) { return enqueue_step(cs, guided); }, &exec));
+      CK(cudaGraphLaunch(exec, s));
+    } else {
+      CKI(enqueue_step(s, guided));
+    }
+    e->launches += launches_per_eval(e, guided);
+    ++k;
+  }
+  for (int k = 0; !repaint && k < nsteps;) {
     const bool guided = guided_at(k);
     // PLMS: the kind of this step and the guidance of a first step's second evaluation, at t - 1
     const int kind = !plms || e->hist_steps + k > 0 ? kPlmsSteady : (t0 - k > 0 ? kPlmsFirst : kPlmsFirstAtZero);

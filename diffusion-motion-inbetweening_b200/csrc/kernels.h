@@ -290,6 +290,17 @@ cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStr
 // inputs as StepParams (its sampler, eta, noise, rng, tape and advance fields are not read; x_next / x_next_hi are
 // required).  Advances the step index t -> t + 1, so one captured graph serves every step of an inversion.
 cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream);
+// RePaint resampling (Lugmayr et al. 2022) with launch_diffusion_step's grid and noise sources (noise_ref / rng;
+// StepParams' sampler, eta, advance and tape_t0 are not read; x_next / x_next_hi are required).  One launch is one op of
+// the walk at the position s = step_ptr[0]; step_ptr[2] is the walk's first position, step_ptr[4] the walk index of the
+// call's first op and step_ptr[5] that of this op, which the kernel advances.
+struct RepaintParams {
+  int phase;               // 0: denoise at s (p_sample, DDPM's arithmetic), s -> s - 1; 1: undo into s + 1, s -> s + 1
+  int jump_length;         // >= 1
+  int jump_n_sample;       // >= 1
+  const float* undo_coef;  // [T][4]: (fp32(sqrt(1 - beta_p)), fp32(sqrt(beta_p)), 0, 0) per position p
+};
+cudaError_t launch_repaint_step(const StepParams& p, const RepaintParams& q, cudaStream_t stream);
 
 // HumanML3D vectors -> joint positions (recover_from_ric), strides in elements; mean/stdv null = already de-normalised
 cudaError_t launch_recover_from_ric(const float* data, long long sb, long long sf, long long sc, const float* mean,

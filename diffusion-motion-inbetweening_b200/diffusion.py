@@ -8,11 +8,13 @@ Mirrors (same names, argument meaning and error behaviour; paths relative to the
                                                     + unipc_sample_loop[_progressive] (UniPC, not in the reference)
                                                     + dpm_solver_sde_sample_loop[_progressive] (SDE-DPM-Solver++,
                                                       not in the reference)
+                                                    + repaint_sample_loop[_progressive] (RePaint resampling, not in
+                                                      the reference)
     space_timesteps / SpacedDiffusion               diffusion/respace.py:9-62, :65-116
     create_gaussian_diffusion                       utils/model_util.py:122-165
 
 `p_sample_loop` / `ddim_sample_loop` / `plms_sample_loop` / `ddim_reverse_sample_loop` / `dpm_solver_sample_loop` /
-`unipc_sample_loop` / `dpm_solver_sde_sample_loop` run the WHOLE loop in one native
+`unipc_sample_loop` / `dpm_solver_sde_sample_loop` / `repaint_sample_loop` run the WHOLE loop in one native
 call (`cmdi_sample`): no per-step Python, no per-step H2D table copies, no per-step host sync (the reference syncs on
 `(t >= stop_imputation_at).all()`, utils/editing_util.py:344).  What the reference computes per step in
 `p_mean_variance` / `p_sample` / `ddim_sample_with_grad` / `plms_sample` / `ddim_reverse_sample` is done by the CUDA
@@ -161,7 +163,7 @@ class GaussianDiffusion:
 
     def _run(self, sampler, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps, init_image, randomize_class,
              dump_steps, const_noise, eta, progressive=False, order=2, num_steps=0, want_pred_xstart=False,
-             variant="bh2", corrector=True):
+             variant="bh2", corrector=True, jump_length=10, jump_n_sample=10):
         if model_kwargs is None:
             model_kwargs = {}
         y = self._check_supported(cond_fn, const_noise, randomize_class, model_kwargs)
@@ -253,8 +255,11 @@ class GaussianDiffusion:
             if x_T is None:
                 seed = self.engine_seed if self.engine_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         elif tape is None:
-            # one randn_like per loop iteration (:696, :1407); SDE-DPM-Solver++ draws the same way
+            # one randn_like per loop iteration (:696, :1407); SDE-DPM-Solver++ draws the same way, RePaint once per op
+            # of its walk
             n_draws = self.num_timesteps - skip_timesteps
+            if sampler == capi.SAMPLER_REPAINT:
+                n_draws = len(_repaint_walk(self.num_timesteps - 1 - skip_timesteps, jump_length, jump_n_sample))
             rng_args = _torch_stream_args(device, int(np.prod(shape)), n_draws, lazy=progressive) if self.rng == "torch" else None
             if rng_args is None:
                 if x_T is not None and noise is None:
@@ -286,6 +291,8 @@ class GaussianDiffusion:
         if unipc:
             common.update(unipc_order=int(order), unipc_variant=capi.UNIPC_BH1 if variant == "bh1" else capi.UNIPC_BH2,
                           unipc_corrector=bool(corrector))
+        if sampler == capi.SAMPLER_REPAINT:
+            common.update(repaint_jump_length=int(jump_length), repaint_jump_n_sample=int(jump_n_sample))
         if progressive:
             return self._step_generator(eng, x_T, init_image, skip_timesteps, tape, common)
         if rev:
@@ -303,29 +310,45 @@ class GaussianDiffusion:
         corrected state included), and DDIM inversion draws nothing, so
         their samples equal the fused loop's bit for bit; a caller that stops an inversion early has a partial one.
         PLMS also yields old_eps, the values of the reference's history list at that yield (the reference yields one
-        list it keeps mutating)."""
+        list it keeps mutating).  RePaint makes one call per denoise op, which also runs the undo ops before it, and
+        yields the op's position as "t"."""
         common = dict(common)
         common["use_graph"] = 2 if common.get("use_graph", True) else 0  # one native call per step, same step graph every time
         plms = common["sampler"] == capi.SAMPLER_PLMS
+        repaint = common["sampler"] == capi.SAMPLER_REPAINT
         torch_rng = common.get("rng_mode", capi.RNG_ENGINE) == capi.RNG_TORCH
         off0, inc = common.pop("aten_offset", 0), common.get("aten_increment", 0)
+        T = self.num_timesteps
+        # the native calls: (skip_timesteps of the position the call starts from, index of its first draw, its draws,
+        # the position of its denoise op)
+        calls = [(skip_timesteps + k, k, 1, None) for k in range(T - skip_timesteps)]
+        if repaint:
+            walk = _repaint_walk(T - 1 - skip_timesteps, common["repaint_jump_length"], common["repaint_jump_n_sample"])
+            calls, d0 = [], 0
+            for d, (p, undo) in enumerate(walk):
+                if not undo:
+                    start = walk[d0][0] - 1 if walk[d0][1] else walk[d0][0]
+                    calls.append((T - 1 - start, d0, d + 1 - d0, p))
+                    d0 = d + 1
         state = x_T
-        for k in range(self.num_timesteps - skip_timesteps):
+        for k, (skip, d0, n_draws, t) in enumerate(calls):
             call = {}
             if common["sampler"] != capi.SAMPLER_DDIM_REVERSE:  # an inversion has no q_sample and no history to resume
                 call.update(resume=(k > 0), init_image=init_image if k == 0 else None)
             if torch_rng:
-                call["aten_offset"] = off0 + k * inc  # each one-step call starts at its own draw of the stream
-            res = eng.sample(skip_timesteps=skip_timesteps + k, num_steps=1, x_T=state, want_pred_xstart=True, want_old_eps=plms,
-                             noise_tape=None if tape is None else tape[k:], **call, **common)
+                call["aten_offset"] = off0 + d0 * inc  # each call starts at its own draw of the stream
+            res = eng.sample(skip_timesteps=skip, num_steps=1, x_T=state, want_pred_xstart=True, want_old_eps=plms,
+                             noise_tape=None if tape is None else tape[d0:], **call, **common)
             state = res["sample"]
             if torch_rng:
                 # torch's generator moves one randn_like at a time, as the reference's loop moves it: a caller that
                 # breaks out of the generator early leaves it where the reference would
-                _advance_torch_generator(eng.device, inc)
+                _advance_torch_generator(eng.device, n_draws * inc)
             step = {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
             if plms:
                 step["old_eps"] = res["old_eps"]
+            if repaint:
+                step["t"] = t
             yield step
 
     # ------------------------------------------------------------------------------------------
@@ -432,6 +455,37 @@ class GaussianDiffusion:
         return self._run(capi.SAMPLER_DPM_SOLVER_SDE, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
                          init_image, randomize_class, None, const_noise, 0.0, progressive=True, order=order)
 
+    def repaint_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                            model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                            randomize_class=False, cond_fn_with_grad=False, const_noise=False, jump_length=10,
+                            jump_n_sample=10):
+        """RePaint resampling (Lugmayr et al. 2022, "time travel") around p_sample_loop, for in-betweening by imputation
+        or reconstruction guidance.  The loop walks the spaced steps: it descends one p_sample at a time, and the first
+        time it reaches a step t with t % jump_length == 0 (and jump_length steps above it) it re-noises the state
+        jump_length steps up, one forward step q(x_p | x_{p-1}) at a time, and denoises that stretch again, jump_n_sample - 1
+        times, so the generated frames can settle into agreement with the keyframes.  Each p_sample is p_sample_loop's
+        step (CFG, keyframe input, imputation, guidance decided by its step).  The cost is about jump_n_sample times the
+        denoiser passes.  Noise: one randn(*shape) for x_T, then one randn_like per op of the walk (`rng`, `noise_tape`);
+        jump_n_sample=1 is p_sample_loop.  The whole walk is one native call.  (The reference has no such sampler.)"""
+        _check_repaint_args(jump_length, jump_n_sample)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_REPAINT, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, const_noise, 0.0, jump_length=jump_length,
+                         jump_n_sample=jump_n_sample)["sample"]
+
+    def repaint_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                        cond_fn=None, model_kwargs=None, device=None, progress=False, skip_timesteps=0,
+                                        init_image=None, randomize_class=False, cond_fn_with_grad=False,
+                                        const_noise=False, jump_length=10, jump_n_sample=10):
+        """Yields {"sample", "pred_xstart", "t"} after each p_sample of repaint_sample_loop's walk ("t" its step), one
+        native call per p_sample (with the re-noising ops before it); the samples equal the fused loop's bit for bit,
+        and torch's generator moves one randn_like per op run.  The configuration is validated at the call."""
+        _check_repaint_args(jump_length, jump_n_sample)
+        _check_no_denoised_fn(denoised_fn)
+        return self._run(capi.SAMPLER_REPAINT, model, shape, noise, cond_fn, model_kwargs, device, skip_timesteps,
+                         init_image, randomize_class, None, const_noise, 0.0, progressive=True, jump_length=jump_length,
+                         jump_n_sample=jump_n_sample)
+
     def unipc_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
                           model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
                           randomize_class=False, cond_fn_with_grad=False, order=2, variant="bh2", corrector=True):
@@ -520,6 +574,27 @@ def _check_sde_order(order) -> None:
     """SDE-DPM-Solver++'s multistep orders are 1 and 2 (an int; bools and floats are refused)."""
     if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or int(order) not in (1, 2):
         raise ValueError(f"SDE-DPM-Solver++ order must be an int in {{1, 2}}, got {order!r}")
+
+
+def _check_repaint_args(jump_length, jump_n_sample) -> None:
+    """RePaint's jump_length and jump_n_sample are ints >= 1 (bools and floats are refused)."""
+    for name, v in (("jump_length", jump_length), ("jump_n_sample", jump_n_sample)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or int(v) < 1:
+            raise ValueError(f"RePaint {name} must be an int >= 1, got {v!r}")
+
+
+def _repaint_walk(t0: int, jump_length: int, jump_n_sample: int) -> list:
+    """The engine's RePaint walk from position t0 (csrc/engine.cu, repaint_walk) as [(p, undo)]: a denoise op at p
+    (p -> p - 1) or an undo op into p (p - 1 -> p).  The generators need it to split the walk into one call per denoise
+    op and to count each call's draws."""
+    walk = []
+    for p in range(t0, -1, -1):
+        if p % jump_length == 0 and p + jump_length <= t0:
+            for _ in range(jump_n_sample - 1):
+                walk += [(u, True) for u in range(p + 1, p + jump_length + 1)]
+                walk += [(u, False) for u in range(p + jump_length, p, -1)]
+        walk.append((p, False))
+    return walk
 
 
 def _check_unipc_args(order, variant, corrector) -> None:

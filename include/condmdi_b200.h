@@ -78,8 +78,21 @@ enum {
    min(dpm_order, iterations since the history started + 1, s + 1); the last step returns x0.  skip_timesteps /
    init_image / resume as for DPM_SOLVER; eta must be 0 and dump_xstart, plms_order, plms_old_eps_out and the unipc_*
    fields unset: the call fails naming the field otherwise. */
+/* REPAINT: RePaint resampling (Lugmayr et al. 2022, "time travel") around DDPM, for in-betweening with imputation.  The
+   walk starts at position t0 = T - 1 - skip_timesteps (position p: the state step p takes as input) and is a sequence
+   of +-1 ops: a denoise op at p is p_sample at step p, exactly DDPM's step (CFG, keyframe input, imputation and
+   reconstruction guidance decided by p); an undo op into p is one forward step of the spaced chain,
+   x <- fp32(sqrt(1 - beta_p)) x + fp32(sqrt(beta_p)) z.  The walk descends; the first time it arrives at a jump point t
+   (t % repaint_jump_length == 0, t + repaint_jump_length <= t0) it goes up repaint_jump_length positions by undo ops and
+   comes back down by denoise ops, repaint_jump_n_sample - 1 times.  With repaint_jump_n_sample = 1 it is DDPM.  Noise:
+   one draw per op in walk order (tape slice, CMDI_RNG_TORCH stream, numbered from the call's first op); the engine
+   generator keys the first denoise op at p by DDPM's stream for p and every other op by its index in the walk.
+   num_steps counts denoise ops; the undo ops before each run in the same call.  resume = 1 continues the running walk
+   (same jump fields and batch) with skip_timesteps = T - 1 - the position the walk has reached.  eta must be 0 and
+   dump_xstart, plms_order, plms_old_eps_out, dpm_order and the unipc_* fields unset: the call fails naming the field
+   otherwise. */
 enum { CMDI_SAMPLER_DDPM = 0, CMDI_SAMPLER_DDIM = 1, CMDI_SAMPLER_PLMS = 2, CMDI_SAMPLER_DDIM_REVERSE = 3,
-       CMDI_SAMPLER_DPM_SOLVER = 4, CMDI_SAMPLER_UNIPC = 5, CMDI_SAMPLER_DPM_SOLVER_SDE = 6 };
+       CMDI_SAMPLER_DPM_SOLVER = 4, CMDI_SAMPLER_UNIPC = 5, CMDI_SAMPLER_DPM_SOLVER_SDE = 6, CMDI_SAMPLER_REPAINT = 7 };
 enum { CMDI_UNIPC_BH1 = 1, CMDI_UNIPC_BH2 = 2 };  /* unipc_variant: B(h) = h or e^h - 1 */
 enum { CMDI_ARCH_TRANS_ENC = 0, CMDI_ARCH_UNET = 1 };
 enum { CMDI_RNG_ENGINE = 0, CMDI_RNG_TORCH = 1 };
@@ -187,6 +200,9 @@ typedef struct {
   int32_t unipc_order;          /* 1..3 */
   int32_t unipc_variant;        /* CMDI_UNIPC_BH1 / CMDI_UNIPC_BH2 */
   int32_t unipc_corrector;      /* 0 / 1 */
+  /* CMDI_SAMPLER_REPAINT only (both 0 for every other sampler); RePaint's names */
+  int32_t repaint_jump_length;  /* >= 1: positions an undo run goes up */
+  int32_t repaint_jump_n_sample; /* >= 1: passes over each jumped stretch (1 = no resampling) */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
