@@ -202,22 +202,28 @@ def cfg_forward(sd, x, timesteps, cond_emb, text_scale: torch.Tensor, num_heads:
 # ------------------------------------------------------------------------------------------------
 # MDM_UNET (model/mdm_unet.py): the denoiser of the published CondMDI checkpoints  (SURVEY.md 8f-4, 8f-1)
 # ------------------------------------------------------------------------------------------------
-def _conv_gn(x, sd, conv: str, gn: str, groups: int = 8):
+def _unrounded(t):
+    return t
+
+
+def _conv_gn(x, sd, conv: str, gn: str, groups: int = 8, q=None):
     """Conv1d(k, padding=k//2) -> GroupNorm(8)   (Conv1dBlock / Conv1dAdaGNBlock.block1, mdm_unet.py:33-88)"""
+    q = q or _unrounded
     w = sd[conv + ".weight"]
-    x = F.conv1d(x, w, sd[conv + ".bias"], padding=w.shape[-1] // 2)
+    x = F.conv1d(q(x), q(w), sd[conv + ".bias"], padding=w.shape[-1] // 2)
     return F.group_norm(x, groups, sd[gn + ".weight"], sd[gn + ".bias"], 1e-5)
 
 
-def _residual_temporal_block(x, emb_mish, sd, pre: str):
+def _residual_temporal_block(x, emb_mish, sd, pre: str, q=None):
     """ResidualTemporalBlock with adagn=True (mdm_unet.py:163-218): x (B, C_in, L), emb_mish = Mish(c) (B, 512)"""
-    cond = F.linear(emb_mish, sd[pre + "time_mlp.1.weight"], sd[pre + "time_mlp.1.bias"]).unsqueeze(-1)  # (B, 2*C_out, 1)
+    q = q or _unrounded
+    cond = F.linear(q(emb_mish), q(sd[pre + "time_mlp.1.weight"]), sd[pre + "time_mlp.1.bias"]).unsqueeze(-1)  # (B, 2*C_out, 1)
     scale, shift = cond.chunk(2, dim=1)
-    out = _conv_gn(x, sd, pre + "blocks.0.block1.0", pre + "blocks.0.block1.2")
+    out = _conv_gn(x, sd, pre + "blocks.0.block1.0", pre + "blocks.0.block1.2", q=q)
     out = F.mish(out * (1 + scale) + shift)                                  # ada_shift_scale (:159-160) then Mish
-    out = F.mish(_conv_gn(out, sd, pre + "blocks.1.block.0", pre + "blocks.1.block.2"))
+    out = F.mish(_conv_gn(out, sd, pre + "blocks.1.block.0", pre + "blocks.1.block.2", q=q))
     if pre + "residual_conv.weight" in sd:
-        x = F.conv1d(x, sd[pre + "residual_conv.weight"], sd[pre + "residual_conv.bias"])
+        x = F.conv1d(q(x), q(sd[pre + "residual_conv.weight"]), sd[pre + "residual_conv.bias"])
     return out + x
 
 
@@ -226,9 +232,14 @@ def unet_levels_of(sd) -> int:
 
 
 def unet_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, timesteps: torch.Tensor, cond_emb: Optional[torch.Tensor] = None,
-                 uncond: bool = False, obs_x0: Optional[torch.Tensor] = None, obs_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 uncond: bool = False, obs_x0: Optional[torch.Tensor] = None, obs_mask: Optional[torch.Tensor] = None,
+                 q=None) -> torch.Tensor:
     """MDM_UNET.forward + forward_core + TemporalUnet.forward (mdm_unet.py:765-849, :309-350), arch='unet', adagn,
-    no attention, hml_vec.  keyframe-conditioned when obs_x0 / obs_mask are given (:778-783)."""
+    no attention, hml_vec.  keyframe-conditioned when obs_x0 / obs_mask are given (:778-783).
+
+    q (test aid): a rounding applied to both operands (not the bias) of every convolution and of the time MLPs' linear
+    layers, e.g. to bf16 to model one bf16 MMA per product; the timestep and text embeddings stay unrounded.  None: none."""
+    q = q or _unrounded
     assert (obs_x0 is None) == (obs_mask is None)
     if obs_x0 is not None:
         x = obs_x0 * obs_mask + x * (~obs_mask)
@@ -244,26 +255,26 @@ def unet_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, timesteps: torch.
     h = x.permute(3, 0, 1, 2).reshape(nframes, bs, njoints * nfeats)
     h = F.pad(h, (0, 0, 0, 0, 0, 224 - nframes), value=0)            # right-pad to the training length (:817)
     h = h.permute(1, 2, 0)                                            # 's b d -> b d s'
-    c = F.linear(F.mish(F.linear(emb, sd["unet.time_mlp.0.weight"], sd["unet.time_mlp.0.bias"])),
-                 sd["unet.time_mlp.2.weight"], sd["unet.time_mlp.2.bias"])
+    c = F.linear(q(F.mish(F.linear(q(emb), q(sd["unet.time_mlp.0.weight"]), sd["unet.time_mlp.0.bias"]))),
+                 q(sd["unet.time_mlp.2.weight"]), sd["unet.time_mlp.2.bias"])
     cm = F.mish(c)                                                    # every block's time_mlp starts with Mish (:183)
     levels = unet_levels_of(sd)
     skips = []
     for l in range(levels):
-        h = _residual_temporal_block(h, cm, sd, f"unet.downs.{l}.0.")
-        h = _residual_temporal_block(h, cm, sd, f"unet.downs.{l}.1.")
+        h = _residual_temporal_block(h, cm, sd, f"unet.downs.{l}.0.", q)
+        h = _residual_temporal_block(h, cm, sd, f"unet.downs.{l}.1.", q)
         skips.append(h)
         if l + 1 < levels:
-            h = F.conv1d(h, sd[f"unet.downs.{l}.3.conv.weight"], sd[f"unet.downs.{l}.3.conv.bias"], stride=2, padding=1)
-    h = _residual_temporal_block(h, cm, sd, "unet.mid_block1.")
-    h = _residual_temporal_block(h, cm, sd, "unet.mid_block2.")
+            h = F.conv1d(q(h), q(sd[f"unet.downs.{l}.3.conv.weight"]), sd[f"unet.downs.{l}.3.conv.bias"], stride=2, padding=1)
+    h = _residual_temporal_block(h, cm, sd, "unet.mid_block1.", q)
+    h = _residual_temporal_block(h, cm, sd, "unet.mid_block2.", q)
     for i in range(levels - 1):
         h = torch.cat((h, skips.pop()), dim=1)
-        h = _residual_temporal_block(h, cm, sd, f"unet.ups.{i}.0.")
-        h = _residual_temporal_block(h, cm, sd, f"unet.ups.{i}.1.")
-        h = F.conv_transpose1d(h, sd[f"unet.ups.{i}.3.conv.weight"], sd[f"unet.ups.{i}.3.conv.bias"], stride=2, padding=1)
-    h = F.mish(_conv_gn(h, sd, "unet.final_conv.0.block.0", "unet.final_conv.0.block.2"))
-    h = F.conv1d(h, sd["unet.final_conv.1.weight"], sd["unet.final_conv.1.bias"])
+        h = _residual_temporal_block(h, cm, sd, f"unet.ups.{i}.0.", q)
+        h = _residual_temporal_block(h, cm, sd, f"unet.ups.{i}.1.", q)
+        h = F.conv_transpose1d(q(h), q(sd[f"unet.ups.{i}.3.conv.weight"]), sd[f"unet.ups.{i}.3.conv.bias"], stride=2, padding=1)
+    h = F.mish(_conv_gn(h, sd, "unet.final_conv.0.block.0", "unet.final_conv.0.block.2", q=q))
+    h = F.conv1d(q(h), q(sd["unet.final_conv.1.weight"]), sd["unet.final_conv.1.bias"])
     out = h.permute(2, 0, 1)[:nframes]                                # 'b d s -> s b d', drop the padding
     njoints_out = out.shape[-1]
     return out.reshape(nframes, bs, njoints_out, 1).permute(1, 2, 3, 0).float()

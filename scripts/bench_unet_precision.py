@@ -1,6 +1,7 @@
-"""MDM_UNET sampling at bf16x3 against fp16 ("autocast", CMDI_PRECISION_FP16) on one GPU: whole ddim50 loops of the xl UNet
+"""MDM_UNET sampling at bf16x3 against fp16 ("autocast", CMDI_PRECISION_FP16) and plain bf16 (CMDI_PRECISION_BF16, one bf16 MMA
+per product) on one GPU: whole ddim50 loops of the xl UNet
 (dim 512, dim_mults (2,2,2,2), keyframe input conditioning, text; random weights) at B = 64 with CFG 2.5, timed with CUDA
-events in one process, the two precisions alternating round by round.  One more leg times a single CFG forward pass of the
+events in one process, the precisions alternating round by round.  One more leg times a single CFG forward pass of the
 oracle under torch.autocast("cuda", float16) in eager PyTorch: the reference's own GPU arithmetic.
 
     python scripts/bench_unet_precision.py [--batch 64] [--rounds 5] [--out DIR]
@@ -72,7 +73,7 @@ def main():
     y = {"text": [str(i) for i in range(B)], "text_scale": torch.full((B,), 2.5).cuda()}
     kw = {"model_kwargs": {"y": y, "obs_x0": x_obs, "obs_mask": kf}, "noise": x_T}
     diff = {}
-    for name, prec in (("bf16x3", C.PRECISION_BF16X3), ("fp16", C.PRECISION_FP16)):
+    for name, prec in (("bf16x3", C.PRECISION_BF16X3), ("fp16", C.PRECISION_FP16), ("bf16", C.PRECISION_BF16)):
         diff[name] = C.create_gaussian_diffusion(timestep_respacing="ddim50")
         diff[name].precision = prec
     arms = {name: (lambda d=d: d.ddim_sample_loop(w, (B, D, 1, L), **kw)) for name, d in diff.items()}
@@ -102,7 +103,8 @@ def main():
         med = statistics.median(ts)
         res[name] = {"loop_ms_median": round(med, 2), "loop_ms_min": round(min(ts), 2), "loop_ms_max": round(max(ts), 2),
                      "steps_per_s": round(steps / (med / 1000.0), 1)}
-    res["fp16_over_bf16x3"] = round(res["fp16"]["steps_per_s"] / res["bf16x3"]["steps_per_s"], 3)
+    for name in ("fp16", "bf16"):
+        res[f"{name}_over_bf16x3"] = round(res[name]["steps_per_s"] / res["bf16x3"]["steps_per_s"], 3)
     med = statistics.median(eager_ms)
     res["eager_autocast_cfg_forward"] = {"ms_median": round(med, 2), "ms_min": round(min(eager_ms), 2),
                                          "steps_per_s": round(1000.0 / med, 1)}

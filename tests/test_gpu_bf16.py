@@ -9,6 +9,8 @@ Contract (DESIGN.md section 3): |E - F| <= 2 |A - F| in max and in mean over a d
 runs that round at the same points still part ways where an operand sits next to a bf16 rounding boundary.
 
 The restatement below is pinned without a GPU: with no rounding it is oracle.condmdi_oracle.mdm_forward to fp32 rounding.
+MDM_UNET at PRECISION_BF16 is held to the same contract, with the oracle's unet_forward and its rounding hook as A / F
+(section at the end).
 """
 import ctypes
 import math
@@ -19,6 +21,7 @@ import torch.nn.functional as F
 
 import condmdi_b200 as C
 from oracle import condmdi_oracle as O
+from oracle import make_golden_geometries as G
 
 DEV = "cuda:0"
 BF16 = C.PRECISION_BF16
@@ -274,12 +277,190 @@ def test_bf16_forward_does_not_depend_on_the_calls_before_it():
 
 @gpu
 def test_bf16x3_engine_next_to_a_bf16_one_is_unchanged():
+    """for the transformer and the xl UNet (keyframes, text)"""
     x, cond, _, _ = inputs(2, 263, 196, seed=3)
     t = torch.full((2,), 500)
-    both, _ = module()
-    plain = engine_forward(both, x, t, cond_emb=cond)
-    after = engine_forward(both, x, t, precision=C.PRECISION_BF16X3, cond_emb=cond)
-    alone = engine_forward(module()[0], x, t, precision=C.PRECISION_BF16X3, cond_emb=cond)
-    assert both.engine_for(DEV, max_batch=2, precision=BF16, nframes=196) is not both.engine_for(DEV, max_batch=2, nframes=196)
-    assert torch.equal(after, alone)
-    assert not torch.equal(plain, alone)
+    xo, mask = unet_inputs(2, 263, 196, seed=3)[1:3]
+    for make, kw in ((module, {"cond_emb": cond}), (unet_module, {"cond_emb": cond, "obs_x0": xo, "obs_mask": mask})):
+        both, _ = make()
+        plain = engine_forward(both, x, t, **kw)
+        after = engine_forward(both, x, t, precision=C.PRECISION_BF16X3, **kw)
+        alone = engine_forward(make()[0], x, t, precision=C.PRECISION_BF16X3, **kw)
+        assert both.engine_for(DEV, max_batch=2, precision=BF16, nframes=196) is not both.engine_for(DEV, max_batch=2, nframes=196)
+        assert torch.equal(after, alone)
+        assert not torch.equal(plain, alone)
+
+
+# ------------------------------------------------------------------------------------------------
+# MDM_UNET at PRECISION_BF16
+#
+#   F = oracle.condmdi_oracle.unet_forward in fp64 on the fp32 weights
+#   A = the same with q = bf16r: both operands of every convolution (Downsample and ConvTranspose included) and of the time
+#       MLPs' linear layers rounded to bf16; the timestep and text embeddings stay unrounded (the engine computes them at
+#       bf16x3 / in fp32)
+#
+# The contract is the transformer's, |E - F| <= 2 |A - F| in max and in mean.  GroupNorm, AdaGN, Mish and the residual
+# sums are fp32 in the engine, and an identity residual is added from the hi + lo planes of the block input: a residual
+# rounded to bf16 is exactly the size of |A - F|, which the ratio gate alone may not see, so a forward must also not
+# depend on the calls before it (bit for bit).
+# ------------------------------------------------------------------------------------------------
+UNET_FORWARD = O.unet_forward  # (the loop tests swap the oracle's model function for unet_dev)
+
+
+def unet_dev(q, sd, x, t, cond_emb=None, uncond=False, obs_x0=None, obs_mask=None):
+    """A (q = bf16r) or F (q = exact) on the GPU in fp64"""
+    sdd = {k: v.to(DEV).double() for k, v in sd.items()}
+    dbl = lambda v: None if v is None else v.to(DEV).double()  # noqa: E731
+    with torch.no_grad():
+        return UNET_FORWARD(sdd, dbl(x), t.to(DEV), dbl(cond_emb), uncond, dbl(obs_x0),
+                              None if obs_mask is None else obs_mask.to(DEV), q=q)
+
+
+def test_unet_rounding_hook_identity_is_no_hook():
+    sd = O.random_unet_state_dict(seed=3, mults=(1, 1), text=True)
+    gi = O.golden_inputs()
+    t = torch.tensor([999, 41])
+    for kw in ({"cond_emb": gi["cond"]}, {"cond_emb": gi["cond"], "uncond": True}):
+        args = (sd, gi["x"], t, kw["cond_emb"], kw.get("uncond", False), gi["x_obs"], gi["kf_mask"])
+        assert torch.equal(O.unet_forward(*args, q=exact), O.unet_forward(*args))
+
+
+def test_unet_rounding_hook_costs_bf16_sized_error():
+    sd = {k: v.double() for k, v in O.random_unet_state_dict(seed=3, mults=(1, 1)).items()}
+    gi = O.golden_inputs()
+    t = torch.tensor([41])
+    args = (sd, gi["x"][:1].double(), t, None, False, gi["x_obs"][:1].double(), gi["kf_mask"][:1])
+    a, f = O.unet_forward(*args, q=bf16r), O.unet_forward(*args)
+    err = (a.double() - f.double()).abs().max().item()
+    assert 1e-4 < err < 1e-1, err  # 2^-9 per operand through 14 convolutions; fp32 rounding would be ~1e-6
+
+
+def unet_module(mults=(2, 2, 2, 2), kf=True, text=True, D=263, seed=11, dataset="humanml"):
+    sd = O.random_unet_state_dict(seed=seed, mults=mults, feats=D, keyframe_conditioned=kf, text=text)
+    kw = {"cond_mode": "text", "cond_mask_prob": 0.1} if text else {}
+    m = C.MDM_UNET(njoints=D, dim_mults=mults, keyframe_conditioned=kf, dataset=dataset, **kw)
+    missing, unexpected = m.load_state_dict(sd, strict=False)
+    assert not missing and not unexpected
+    return m.to(DEV), sd
+
+
+def unet_inputs(B, D, L, seed):
+    """x, x_obs, an observation mask (whole frames and single features), text embeddings, per-sample timesteps 999 / 0 / 41,
+    CFG scales"""
+    g = torch.Generator().manual_seed(seed)
+    x, xo = torch.randn(B, D, 1, L, generator=g), torch.randn(B, D, 1, L, generator=g)
+    mask = G.random_obs_mask(g, B, D, L)
+    t = torch.tensor([999, 0, 41])[torch.arange(B) % 3]
+    return x, xo, mask, torch.randn(B, 512, generator=g), t, torch.full((B,), 2.5)
+
+
+# name: D, L, dim_mults, keyframe input conditioning, text, dataset
+UNET_CASES = {
+    "xl": (263, 196, (2, 2, 2, 2), True, True, "humanml"),
+    "11-kf": (263, 196, (1, 1), True, False, "humanml"),
+    "111-nokf": (263, 196, (1, 1, 1), False, False, "humanml"),
+    "251x196-uncond": (251, 196, (1, 1), False, False, "kit"),
+    **{n: (c["D"], c["L"], c["mults"], True, False, c["dataset"]) for n, c in G.CASES.items() if c["kind"] == "unet"},
+}
+
+
+@gpu
+@pytest.mark.parametrize("name,B", [("xl", 2), ("xl", 64)] + [(n, 3) for n in UNET_CASES if n != "xl"])
+def test_bf16_unet_forward_meets_the_contract(name, B):
+    """text and unconditional passes (plain ones for a model without text) at timesteps 999 / 0 / 41, keyframe input
+    conditioning where the model has it; unet.263x224 is the unpadded 224 frames"""
+    D, L, mults, kf, text, dataset = UNET_CASES[name]
+    m, sd = unet_module(mults, kf, text, D, dataset=dataset)
+    x, xo, mask, cond, t, scale = unet_inputs(B, D, L, seed=B * 1000 + D + L)
+    obs = {"obs_x0": xo, "obs_mask": mask} if kf else {}
+    passes = [("text", {"cond_emb": cond}), ("uncond", {"cond_emb": cond, "uncond": True})] if text else [("plain", {})]
+    for what, kw in passes:
+        got = engine_forward(m, x, t, **kw, **obs)
+        gate(got, unet_dev(bf16r, sd, x, t, **kw, **obs), unet_dev(exact, sd, x, t, **kw, **obs), f"unet {name} B={B} {what}")
+    if text:
+        # CFG: the batch-doubled pass computes the two passes above (one shared timestep), combined in fp32
+        t1 = torch.full((B,), 41)
+        u, c = (engine_forward(m, x, t1, cond_emb=cond, uncond=un, **obs) for un in (True, False))
+        got = engine_forward(m, x, t1, cond_emb=cond, cfg=True, text_scale=scale, **obs)
+        assert torch.allclose(got, u + scale.to(DEV).view(-1, 1, 1, 1) * (c - u), rtol=0, atol=1e-5)
+
+
+@gpu
+def test_bf16_unet_forward_does_not_depend_on_the_calls_before_it():
+    """Every identity residual is read from planes the same pass wrote: the first block of each level >= 1 adds the
+    Downsample output back from its hi + lo planes, which the up path's blocks of the same level write again later."""
+    m, _ = unet_module()
+    x1, xo, mask, cond, _, scale = unet_inputs(2, 263, 196, seed=1)
+    x2 = unet_inputs(2, 263, 196, seed=2)[0] * 3
+    t = torch.full((2,), 500)
+    kw = {"cond_emb": cond, "obs_x0": xo, "obs_mask": mask}
+    first = engine_forward(m, x1, t, **kw)
+    engine_forward(m, x2, t, **kw)
+    engine_forward(m, x2, t, cfg=True, text_scale=scale, **kw)
+    again = engine_forward(m, x1, t, **kw)
+    print(f"[unet bf16 forward after other calls] max |diff| = {(again - first).abs().max().item():.3e}")
+    assert torch.equal(again, first)
+
+
+def unet_oracle_loop(sd, run):
+    """run() (an oracle sampling loop) with the oracle's UNet evaluated on the GPU in fp64: A (q = bf16r), then F"""
+    want = []
+    try:
+        for q in (bf16r, exact):
+            def gpu_forward(sd_, x, t, cond_emb=None, uncond=False, obs_x0=None, obs_mask=None, _q=q):
+                return unet_dev(_q, sd, x, t, cond_emb, uncond, obs_x0, obs_mask).float().cpu()
+            O.unet_forward = gpu_forward
+            want.append(run())
+    finally:
+        O.unet_forward = UNET_FORWARD
+    return want
+
+
+def unet_loop_case(B, seed, mults=(2, 2, 2, 2)):
+    """the model with its text table, and the model_kwargs / oracle Conditioning of keyframe input conditioning and
+    imputation over ragged lengths"""
+    m, sd = unet_module(mults)
+    _, x_obs, mask, cond, _, scale = unet_inputs(B, 263, 196, seed)
+    g = torch.Generator().manual_seed(seed + 1)
+    lengths = torch.randint(40, 197, (B,), generator=g)
+    y_mask = (torch.arange(196)[None] < lengths[:, None]).view(B, 1, 1, 196)
+    table = {str(i): cond[i].to(DEV) for i in range(B)}
+    m.encode_text = lambda texts: torch.stack([table[s] for s in texts])
+    y = {"text": [str(i) for i in range(B)], "mask": y_mask.to(DEV), "imputate": 1,
+         "stop_imputation_at": 1, "replacement_distribution": "conditional", "inpainted_motion": x_obs.to(DEV),
+         "inpainting_mask": mask.to(DEV)}
+    kw = {"y": y, "obs_x0": x_obs.to(DEV), "obs_mask": mask.to(DEV)}
+    c = O.Conditioning(cond_emb=cond, text_scale=scale, y_mask=y_mask, imputate=True, stop_imputation_at=1, inpainted_motion=x_obs,
+                       inpainting_mask=mask, obs_x0=x_obs, obs_mask=mask)
+    return m, sd, x_obs, kw, c, g
+
+
+@gpu
+def test_bf16_unet_ddpm_tail_keyframes_imputation_b2():
+    B = 2
+    m, sd, x_obs, kw, c, g = unet_loop_case(B, seed=21)
+    tape = torch.randn(5, B, 263, 1, 196, generator=g)
+    d = C.create_gaussian_diffusion()
+    d.precision = BF16
+    d.noise_tape = tape.to(DEV)
+    got = d.p_sample_loop(m, (B, 263, 1, 196), model_kwargs=kw, skip_timesteps=996, init_image=x_obs.to(DEV))
+    a, f = unet_oracle_loop(sd, lambda: O.sample_loop(sd, O.make_tables(""), (B, 263, 1, 196), c, tape, "ddpm", skip_timesteps=996,
+                                                     init_image=x_obs))
+    gate(got, a, f, "unet xl B=2 ddpm 4-step tail, text + keyframes + imputation")
+
+
+@gpu
+def test_bf16_unet_ddim50_tail_cfg_keyframes_imputation_b64():
+    B = 64
+    m, sd, x_obs, kw, c, g = unet_loop_case(B, seed=22)
+    kw["y"]["text_scale"] = c.text_scale.to(DEV)
+    c.cfg = True
+    tape = torch.randn(5, B, 263, 1, 196, generator=g)
+    d = C.create_gaussian_diffusion(timestep_respacing="ddim50")
+    d.precision = BF16
+    d.noise_tape = tape.to(DEV)
+    got = d.ddim_sample_loop(C.ClassifierFreeSampleModel(m), (B, 263, 1, 196), model_kwargs=kw, skip_timesteps=46,
+                             init_image=x_obs.to(DEV))
+    a, f = unet_oracle_loop(sd, lambda: O.sample_loop(sd, O.make_tables("ddim50"), (B, 263, 1, 196), c, tape, "ddim",
+                                                     skip_timesteps=46, init_image=x_obs))
+    gate(got, a, f, "unet xl B=64 ddim50 4-step tail, cfg 2.5 + keyframes + imputation")

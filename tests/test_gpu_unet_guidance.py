@@ -125,11 +125,13 @@ def test_input_vjp(name, B, mults, kf_cond, text, mode):
 
 
 def test_bf16x3_unet_still_refuses_guidance():
+    """and so does the plain-bf16 UNet, with the same error"""
     m, _ = module((1, 1), True, False, seed=3)
     x, xo, kf, _, _ = inputs(2, seed=1)
-    eng = m.engine_for(DEV, max_batch=2, nframes=L)
-    with pytest.raises(RuntimeError, match="transformer"):
-        eng.test_input_vjp(x, 500, xo, kf, obs_x0=xo, obs_mask=kf)
+    for precision in (C.PRECISION_BF16X3, C.PRECISION_BF16):
+        eng = m.engine_for(DEV, max_batch=2, precision=precision, nframes=L)
+        with pytest.raises(RuntimeError, match="transformer"):
+            eng.test_input_vjp(x, 500, xo, kf, obs_x0=xo, obs_mask=kf)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
