@@ -8,12 +8,14 @@
 Contract (DESIGN.md section 3): |E - F| <= 2 |A - F| in max and in mean over a denoiser output.  |E - A| is printed: two
 runs that round at the same points still part ways where an operand sits next to a bf16 rounding boundary.
 
-The restatement below is pinned without a GPU: with no rounding it is oracle.condmdi_oracle.mdm_forward to fp32 rounding.
+The restatement below is pinned without a GPU: with no rounding it is oracle.condmdi_oracle.mdm_forward to fp32 rounding,
+and its input-VJP (test_gpu_transformer_guidance.py's reference) is autograd through it to fp64 rounding.
 MDM_UNET at PRECISION_BF16 is held to the same contract, with the oracle's unet_forward and its rounding hook as A / F
 (section at the end).
 """
 import ctypes
 import math
+import sys
 
 import pytest
 import torch
@@ -38,9 +40,39 @@ def exact(t):
 
 # ------------------------------------------------------------------------------------------------
 # the model: oracle.condmdi_oracle.mdm_forward / _encoder_layer in fp64 with a rounding hook q on the products' operands
+#
+# Differentiable in x in the same arithmetic: every product's backward forms each input gradient it is asked for as a
+# product of rounded operands, q(g) q(b)^T and q(a)^T q(g), which is what the engine's backward rounds with one MMA per
+# product (the seed and every dY against the W^T planes; the attention backward's dP = dO V^T, dV = P^T dO, dQ = dS K,
+# dK = dS^T Q).  Everything between the products (softmax, LayerNorm, GELU and their derivatives) is exact.
 # ------------------------------------------------------------------------------------------------
+class QProduct(torch.autograd.Function):
+    """q(a) @ q(b); the weights take no gradient, so only what ctx.needs_input_grad asks for is formed"""
+
+    @staticmethod
+    def forward(ctx, a, b, q):
+        ctx.save_for_backward(a, b)
+        ctx.q = q
+        return q(a) @ q(b)
+
+    @staticmethod
+    def backward(ctx, g):
+        a, b = ctx.saved_tensors
+        q = ctx.q
+        ga = gb = None
+        if ctx.needs_input_grad[0]:
+            ga = (q(g) @ q(b).transpose(-1, -2)).sum_to_size(a.shape)
+        if ctx.needs_input_grad[1]:
+            gb = (q(a).transpose(-1, -2) @ q(g)).sum_to_size(b.shape)
+        return ga, gb, None
+
+
+def qmm(q, a, b):
+    return QProduct.apply(a, b, q)
+
+
 def qlinear(q, x, w, b):
-    return F.linear(q(x), q(w), b)
+    return qmm(q, x, w.t()) + b
 
 
 def encoder_layer(q, x, sd, pre, num_heads=4):
@@ -48,9 +80,11 @@ def encoder_layer(q, x, sd, pre, num_heads=4):
     dh = d // num_heads
     heads = lambda t: t.reshape(S, B, num_heads, dh).permute(1, 2, 0, 3)  # noqa: E731
     qq, k, v = (heads(t) for t in qlinear(q, x, sd[pre + "self_attn.in_proj_weight"], sd[pre + "self_attn.in_proj_bias"]).chunk(3, dim=-1))
-    s = q(qq) @ q(k).transpose(-1, -2) / math.sqrt(dh)
-    p = torch.exp(s - s.amax(dim=-1, keepdim=True))  # the product sees exp(s - max); the row sum divides its result
-    a = (q(p) @ q(v) / p.sum(dim=-1, keepdim=True)).permute(2, 0, 1, 3).reshape(S, B, d)
+    s = qmm(q, qq, k.transpose(-1, -2)) / math.sqrt(dh)
+    # the product sees exp(s - max); the row sum divides its result.  The max is a constant of the softmax: its
+    # derivative cancels exactly, and the engine's backward does not form it
+    p = torch.exp(s - s.amax(dim=-1, keepdim=True).detach())
+    a = (qmm(q, p, v) / p.sum(dim=-1, keepdim=True)).permute(2, 0, 1, 3).reshape(S, B, d)
     a = qlinear(q, a, sd[pre + "self_attn.out_proj.weight"], sd[pre + "self_attn.out_proj.bias"])
     x = F.layer_norm(x + a, (d,), sd[pre + "norm1.weight"], sd[pre + "norm1.bias"], 1e-5)
     h = F.gelu(qlinear(q, x, sd[pre + "linear1.weight"], sd[pre + "linear1.bias"]))
@@ -99,6 +133,90 @@ def test_model_rounding_hook_costs_bf16_sized_error():
     assert 1e-4 < err < 1e-1, err  # 2^-9 per operand through two layers; fp32 rounding would be ~1e-6
 
 
+def pass_vjps(forward, x, t, xo, M, cond_emb=None, uncond=False, scale=None):
+    """The input-VJP of a guided evaluation as Engine.test_input_vjp returns it: the gradients of
+    sum((xo - x0_hat)^2 * M) w.r.t. x through each pass, cond pass first, each seeded with what the CFG combine
+    x0_hat = u + s (c - u) hands it (s G and G - s G).  forward(z, t, cond_emb, uncond) is the model; fp64 on x's device."""
+    dev = x.device
+    dbl = lambda v: None if v is None else v.to(dev).double()  # noqa: E731
+    z = x.detach().double().requires_grad_(True)
+    xo, M, cond_emb, t = dbl(xo), dbl(M), dbl(cond_emb), t.to(dev)
+    if scale is None:
+        outs = [forward(z, t, cond_emb, uncond)]
+        hat = outs[0]
+    else:
+        outs = [forward(z, t, cond_emb, False), forward(z, t, cond_emb, True)]
+        hat = outs[1] + dbl(scale).view(-1, 1, 1, 1) * (outs[0] - outs[1])
+    loss = ((xo - hat).square() * M).sum()
+    seeds = torch.autograd.grad(loss, outs, retain_graph=True)
+    return torch.stack([torch.autograd.grad(o, z, s_, retain_graph=True)[0] for o, s_ in zip(outs, seeds)])
+
+
+def vjp_inputs(B, D, L, seed):
+    """x, x_obs, a Bernoulli observation mask, text embeddings, per-sample CFG scales"""
+    g = torch.Generator().manual_seed(seed)
+    x, xo = torch.randn(B, D, 1, L, generator=g), torch.randn(B, D, 1, L, generator=g)
+    return x, xo, G.random_obs_mask(g, B, D, L), torch.randn(B, 512, generator=g), 0.5 + 3 * torch.rand(B, generator=g)
+
+
+# the bf16x3 input-VJP gate (tests/test_gpu_transformer_guidance.py): |E - F| <= BF16X3_VJP_GATE |A - F|.  Measured on
+# H100: 0.001-0.003 in max, 0.002 in mean over every case; one dgrad product at one MMA gives 0.03 / 0.07 (below)
+BF16X3_VJP_GATE = 0.02
+VJP_CPU_L = 20  # frames of the CPU model tests
+
+
+def test_model_vjp_without_rounding_is_the_oracle_vjp():
+    """the product's backward with q = identity is autograd through the oracle, per pass, with and without CFG"""
+    sd = {k: v.double() for k, v in O.random_state_dict(seed=3, text=True).items()}
+    x, xo, M, cond, scale = vjp_inputs(2, 263, VJP_CPU_L, seed=1)
+    t = torch.tensor([999, 41])
+    model = lambda z, t_, c, u: mdm_model(exact, sd, z, t_, c, u)  # noqa: E731
+    oracle = lambda z, t_, c, u: O.mdm_forward(sd, z, t_, c, u)  # noqa: E731
+    for kw in ({}, {"cond_emb": cond}, {"cond_emb": cond, "uncond": True}, {"cond_emb": cond, "scale": scale}):
+        got, want = pass_vjps(model, x, t, xo, M, **kw), pass_vjps(oracle, x, t, xo, M, **kw)
+        assert got.shape == want.shape == (2 if "scale" in kw else 1, 2, 263, 1, VJP_CPU_L)
+        err = ((got - want).abs().max() / want.abs().max()).item()
+        assert want.abs().max() > 0 and err < 1e-12, (kw.keys(), err)  # fp64 rounding of an 8-layer backward
+
+
+def test_model_vjp_rounding_hook_costs_bf16_sized_error():
+    sd = {k: v.double() for k, v in O.random_state_dict(seed=3, layers=2, text=True).items()}
+    x, xo, M, cond, scale = vjp_inputs(2, 263, VJP_CPU_L, seed=2)
+    t = torch.tensor([500, 30])
+    a, f = (pass_vjps(lambda z, t_, c, u, q=q: mdm_model(q, sd, z, t_, c, u), x, t, xo, M, cond, scale=scale) for q in (bf16r, exact))
+    err = ((a - f).abs().max() / f.abs().max()).item()
+    assert 1e-4 < err < 1e-1, err  # 2^-9 per operand of the forward and backward products; fp32 rounding would be ~1e-7
+
+
+def test_bf16x3_vjp_gate_catches_one_dgrad_product_at_one_mma(monkeypatch):
+    """S = F with one dgrad product of the backward, layer 3's out-proj (dAttn = dV1 Wo), formed from bf16-rounded
+    operands and everything else exact: what one product costs that ran with one MMA, or read a stale lo plane at bf16x3.
+    |S - F| must exceed the bf16x3 gate's share of |A - F|, so the gate cannot pass it."""
+    sd = {k: v.double() for k, v in O.random_state_dict(seed=7, text=True).items()}
+    x, xo, M, cond, scale = vjp_inputs(2, 263, VJP_CPU_L, seed=3)
+    t = torch.tensor([500, 500])
+    kw = {"cond_emb": cond, "scale": scale}
+    a, f = (pass_vjps(lambda z, t_, c, u, q=q: mdm_model(q, sd, z, t_, c, u), x, t, xo, M, **kw) for q in (bf16r, exact))
+    wo3 = sd["seqTransEncoder.layers.3.self_attn.out_proj.weight"]
+    plain = qlinear
+
+    def one_rounded_dgrad(q, v, w, b):
+        if w is not wo3:
+            return plain(q, v, w, b)
+        r = plain(bf16r, v, w, b)
+        return r - (r - plain(exact, v, w, b)).detach()  # the exact product forward, the rounded one's backward
+
+    monkeypatch.setattr(sys.modules[__name__], "qlinear", one_rounded_dgrad)
+    s = pass_vjps(lambda z, t_, c, u: mdm_model(exact, sd, z, t_, c, u), x, t, xo, M, **kw)
+    for k in range(2):
+        s_f, a_f = (s[k] - f[k]).abs(), (a[k] - f[k]).abs()
+        r_max, r_mean = (s_f.max() / a_f.max()).item(), (s_f.mean() / a_f.mean()).item()
+        print(f"[one rounded dgrad product, pass {k}] |S-F|/|A-F| max={r_max:.3f} mean={r_mean:.3f}")
+        # the gate fails when either ratio exceeds it (measured max 0.029 / mean 0.074 for the cond pass, 0.028 / 0.070
+        # for the uncond pass: one product's error reaches every element of the gradient, so the mean shows it most)
+        assert r_max > BF16X3_VJP_GATE or r_mean > BF16X3_VJP_GATE, (k, r_max, r_mean)
+
+
 # ------------------------------------------------------------------------------------------------
 # one chained layer launch (cmdi_test_chain_layer) against fp64 of the same four sublayers
 # ------------------------------------------------------------------------------------------------
@@ -108,7 +226,7 @@ def folded_ln_linear(q, v, w, gamma, beta, b):
     mean = v.mean(dim=-1, keepdim=True)
     rstd = torch.rsqrt(v.var(dim=-1, unbiased=False, keepdim=True) + 1e-5)
     wf = w * gamma
-    return rstd * (q(v) @ q(wf).t() - mean * wf.sum(dim=1)) + (w @ beta + b)
+    return rstd * (qmm(q, v, wf.t()) - mean * wf.sum(dim=1)) + (w @ beta + b)
 
 
 def chain_layer_reference(q, t):
@@ -260,17 +378,22 @@ def test_bf16_unchained_path_meets_the_contract(monkeypatch, B):
 
 @gpu
 def test_bf16_forward_does_not_depend_on_the_calls_before_it():
-    """activation planes keep nothing from an earlier pass, a guided (stashing, unchained, backward) one included"""
+    """activation planes keep nothing from an earlier pass, a guided (stashing, unchained, backward) one included, at
+    B = 2 and as a B = 64 CFG pass whose backward writes every row of the planes"""
     m, _ = module()
+    eng = m.engine_for(DEV, max_batch=64, precision=BF16, nframes=196)  # (engine_forward's B = 2 calls run on it too)
     x1, cond, t, _ = inputs(2, 263, 196, seed=1)
     x2 = inputs(2, 263, 196, seed=2)[0] * 3
     t = torch.full((2,), 500)
     first = engine_forward(m, x1, t, cond_emb=cond)
     engine_forward(m, x2, t, cond_emb=cond)
     assert torch.equal(engine_forward(m, x1, t, cond_emb=cond), first)
-    eng = m.engine_for(DEV, max_batch=2, precision=BF16, nframes=196)
     mask = O.get_keyframes_mask(x2, torch.tensor([196, 150]), "benchmark_sparse", 5)
     grad = eng.test_input_vjp(x2, 500, x2, mask, cond_emb=cond)
+    assert torch.isfinite(grad).all()
+    assert torch.equal(engine_forward(m, x1, t, cond_emb=cond), first)
+    x64, xo64, mask64, cond64, scale64 = vjp_inputs(64, 263, 196, seed=3)
+    grad = eng.test_input_vjp(x64 * 3, 30, xo64, mask64, cond_emb=cond64, cfg=True, text_scale=scale64)
     assert torch.isfinite(grad).all()
     assert torch.equal(engine_forward(m, x1, t, cond_emb=cond), first)
 
