@@ -64,7 +64,9 @@ class SampleArgs(Structure):
                 ("host_buffers", c_int32), ("use_graph", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p),
                 ("plms_order", c_int32), ("plms_old_eps_out", c_void_p), ("dpm_order", c_int32),
                 ("unipc_order", c_int32), ("unipc_variant", c_int32), ("unipc_corrector", c_int32),
-                ("repaint_jump_length", c_int32), ("repaint_jump_n_sample", c_int32)]
+                ("repaint_jump_length", c_int32), ("repaint_jump_n_sample", c_int32),
+                ("window_count", c_int32), ("window_frames0", POINTER(c_int32)), ("global_frames", c_int32),
+                ("window_out", c_void_p)]
 
 
 class LibraryMissing(RuntimeError):

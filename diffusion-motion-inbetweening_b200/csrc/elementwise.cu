@@ -229,19 +229,21 @@ __device__ __forceinline__ float step_x0(float mo, float mu, float ob, unsigned 
   return out;
 }
 
-// x_t and x0 (step_x0) of the 4 consecutive features at idx, the frame-major offset of feature c of a frame of sample
-// b, for the evaluation at step index t_eval.  Operands are read with 16-byte loads, each under the predicate that
-// makes it meaningful: an unguided, un-imputed step never touches x_obs / obs_mask / guide_grad, and only a CFG step
-// reads the uncond half.  Padding features (c + j >= D) get x0 = 0.
-__device__ __forceinline__ void load_step_x0(const StepParams& p, size_t idx, int b, int c, int t_eval, float xt[4], float x0[4]) {
-  const bool do_impute = p.impute && (t_eval >= p.stop_imputation_at);
-  const float guide_c = p.guided ? p.guide_coef[t_eval] : 0.f;
+// x0 (step_x0) of the 4 consecutive features at idx, the frame-major offset of feature c of a frame of row b, and
+// x_t there when xt is given.  Operands are read with 16-byte loads, each under the predicate that makes it meaningful:
+// an unguided, un-imputed step never touches x_obs / obs_mask / guide_grad, and only a CFG step reads the uncond half.
+// Padding features (c + j >= D) get x0 = 0.
+__device__ __forceinline__ void step_x0_at(const StepParams& p, size_t idx, int b, int c, bool do_impute, float guide_c,
+                                           float x0[4], float* xt = nullptr) {
   const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
   const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
   const bool need_obs = p.guided || do_impute;
   const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
   const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-  const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+  if (xt) {
+    const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
+    xt[0] = xt4.x; xt[1] = xt4.y; xt[2] = xt4.z; xt[3] = xt4.w;
+  }
   const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
   const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
   float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
@@ -253,10 +255,48 @@ __device__ __forceinline__ void load_step_x0(const StepParams& p, size_t idx, in
   const float ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
   const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
   const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
-  xt[0] = xt4.x; xt[1] = xt4.y; xt[2] = xt4.z; xt[3] = xt4.w;
 #pragma unroll
   for (int j = 0; j < 4; ++j)
     x0[j] = c + j < p.D ? step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c) : 0.f;
+}
+
+// Overlapping windows: x0 of a global frame g that several windows cover becomes
+//   (sum_k w_k(g) x0_k(g)) / sum_k w_k(g),   w_k(g) = 1 + min(g - f0(k), f0(k) + F - 1 - g),
+// summed over the covering windows in ascending k with round-to-nearest fp32 products, sums and quotient.  Every
+// covering window forms the same sum in the same order from the same inputs (each neighbour's x0 is recomputed from its
+// own model output, guidance gradient and keyframes), so all of them store the same bits.  A frame covered by this
+// window alone keeps its x0.  The weights are small integers, exact in fp32.
+__device__ __forceinline__ void blend_window_x0(const StepParams& p, size_t idx, int b, int c, bool do_impute, float guide_c,
+                                                float x0[4]) {
+  const int K = p.win_K, F = p.L;
+  const int k = b % K, row0 = b - k;
+  const int g = p.win_f0[k] + (int)((idx / p.D_pad) % F);
+  int lo = k, hi = k;
+  while (lo > 0 && p.win_f0[lo - 1] + F > g) --lo;
+  while (hi + 1 < K && p.win_f0[hi + 1] <= g) ++hi;
+  if (lo == hi) return;
+  float acc[4], wsum = 0.f;
+  for (int kk = lo; kk <= hi; ++kk) {
+    const int f0 = p.win_f0[kk];
+    const float w = (float)(1 + min(g - f0, f0 + F - 1 - g));
+    float v[4] = {x0[0], x0[1], x0[2], x0[3]};
+    if (kk != k) step_x0_at(p, ((size_t)(row0 + kk) * F + (g - f0)) * p.D_pad + c, row0 + kk, c, do_impute, guide_c, v);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[j] = kk == lo ? __fmul_rn(w, v[j]) : __fadd_rn(acc[j], __fmul_rn(w, v[j]));
+    wsum += w;
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) x0[j] = __fdiv_rn(acc[j], wsum);
+}
+
+// x_t and x0 of the 4 consecutive features at idx (step_x0_at, then the window blend) for the evaluation at step index
+// t_eval.  kWin: the step kernel instance for windowed calls (win_K > 1); the other instance has no blend code.
+template <bool kWin = false>
+__device__ __forceinline__ void load_step_x0(const StepParams& p, size_t idx, int b, int c, int t_eval, float xt[4], float x0[4]) {
+  const bool do_impute = p.impute && (t_eval >= p.stop_imputation_at);
+  const float guide_c = p.guided ? p.guide_coef[t_eval] : 0.f;
+  step_x0_at(p, idx, b, c, do_impute, guide_c, x0, xt);
+  if (kWin) blend_window_x0(p, idx, b, c, do_impute, guide_c, x0);
 }
 
 // Stores the state after a step for the 4 features at idx: x_next as fp32 and as bf16 planes (hi, and lo where the
@@ -302,6 +342,7 @@ __device__ __forceinline__ void advance_step(int* step_ptr, int next) {
 //   phase 2  first step, after the evaluation at t - 1 (= step_ptr[0]): the improved Euler sample from the kept x_t;
 //            leaves the step index at t - 1
 // ---------------------------------------------------------------------------------------------
+template <bool kWin>
 __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, const PlmsParams q) {
   const int t_eval = *p.step_ptr;                    // step index of the evaluation in model_out
   const int t = q.phase == 2 ? t_eval + 1 : t_eval;  // step index of the PLMS step
@@ -334,7 +375,7 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const StepParams p, cons
     const float e2[4] = {e2v.x, e2v.y, e2v.z, e2v.w}, e3[4] = {e3v.x, e3v.y, e3v.z, e3v.w}, e4[4] = {e4v.x, e4v.y, e4v.z, e4v.w};
     const float xk[4] = {xkv.x, xkv.y, xkv.z, xkv.w};
     float xtv[4], x04[4], xn4[4], ep4[4];
-    load_step_x0(p, idx, b, c, t_eval, xtv, x04);
+    load_step_x0<kWin>(p, idx, b, c, t_eval, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float x0 = x04[j];
@@ -425,6 +466,7 @@ __global__ void __launch_bounds__(256) ddim_reverse_step_kernel(const StepParams
 // m2 are the x0 of the previous two loop iterations.  The x0 history is a ring of three [B*L, D_pad] buffers: iteration
 // k = step_ptr[2] - s at slot k % 3, so one kernel serves every step.  No noise is drawn.  Advances s -> s - 1.
 // ---------------------------------------------------------------------------------------------
+template <bool kWin>
 __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p, const DpmParams q) {
   const int s = *p.step_ptr;
   const int k = p.step_ptr[2] - s;                      // loop iteration since the history started
@@ -442,7 +484,7 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p
     if (eff >= 3) m2v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 1) % 3) * q.hist_stride + idx);  // k - 2
     const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w}, m2[4] = {m2v.x, m2v.y, m2v.z, m2v.w};
     float xtv[4], x04[4], xn4[4];
-    load_step_x0(p, idx, b, c, s, xtv, x04);
+    load_step_x0<kWin>(p, idx, b, c, s, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float x0 = x04[j];
@@ -470,6 +512,7 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const StepParams p
 // DPM-Solver++ uses: iteration k at slot k % 3, so m3 (iteration k - 3) sits in this step's own slot and is read before
 // m0 overwrites it.  x_s^c replaces x_{s+1}^c in q.xc.  No noise is drawn.  Advances s -> s - 1.
 // ---------------------------------------------------------------------------------------------
+template <bool kWin>
 __global__ void __launch_bounds__(256) unipc_step_kernel(const StepParams p, const UnipcParams q) {
   const int s = *p.step_ptr;
   const int k = p.step_ptr[2] - s;                                  // loop iteration since the history started
@@ -495,7 +538,7 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const StepParams p, con
     const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w}, m2[4] = {m2v.x, m2v.y, m2v.z, m2v.w};
     const float m3[4] = {m3v.x, m3v.y, m3v.z, m3v.w}, xcp[4] = {xcv.x, xcv.y, xcv.z, xcv.w};
     float xtv[4], x04[4], xn4[4], xc4[4];
-    load_step_x0(p, idx, b, c, s, xtv, x04);
+    load_step_x0<kWin>(p, idx, b, c, s, xtv, x04);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float x0 = x04[j];
@@ -527,11 +570,18 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const StepParams p, con
 // [b][c][l] (l contiguous), into s_noise[c - c0][l - l0]; block 32x8.  tape_t0 is the call's first step index, so
 // (tape_t0 - t) numbers this step's draw within the call.  Three sources: the noise tape, the torch.randn_like stream
 // (draw number (tape_t0 - t) after aten_offset) and the engine generator (stream t + 1, keyed by the global sample
-// index).  The caller synchronises the block before reading the tile.
+// index).  With overlapping windows (win_K > 1) row b is window k of global sample s, and its frame l draws the noise
+// of global frame f0(k) + l of sample s in the (B / win_K, D, 1, win_N) layout, from each of the three sources.  The
+// caller synchronises the block before reading the tile.
 // ---------------------------------------------------------------------------------------------
+template <bool kWin = false>
 __device__ __forceinline__ void fill_noise_tile(const StepParams& p, int t, int tape_t0, int b, int l0, int c0,
                                                 float (&s_noise)[32][33]) {
   const int tx = threadIdx.x, ty = threadIdx.y;
+  int gs = b, gf0 = 0, gL = p.L, gB = p.B;  // global sample, first global frame, global frames and samples
+  if (kWin) {
+    gs = b / p.win_K; gf0 = p.win_f0[b % p.win_K]; gL = p.win_N; gB = p.B / p.win_K;
+  }
   RngState rng{};
   if (!p.noise_ref && p.rng) rng = *p.rng;
   if (!p.noise_ref && rng.mode == 1) {
@@ -541,16 +591,18 @@ __device__ __forceinline__ void fill_noise_tile(const StepParams& p, int t, int 
     for (int i = 0; i < 4; ++i) {
       const int c = c0 + ty + i * 8, l = l0 + tx;
       float nz = 0.f;
-      if (c < p.D && l < p.L) nz = aten_normal(rng.seed, off, rng.aten_threads, ((size_t)b * p.D + c) * p.L + l);
+      if (c < p.D && l < p.L) nz = aten_normal(rng.seed, off, rng.aten_threads, ((size_t)gs * p.D + c) * gL + gf0 + l);
       s_noise[ty + i * 8][tx] = nz;
     }
-  } else if (!p.noise_ref && (p.L & 3) == 0) {
-    // engine generator: one Philox call yields the 4 consecutive frames of a quad (l0 and L are multiples of 4)
+  } else if (!p.noise_ref && (p.L & 3) == 0 && ((gf0 | gL) & 3) == 0) {
+    // engine generator: one Philox call yields the 4 consecutive frames of a quad (l0, L and the global frame offset
+    // and length are multiples of 4)
     const int q = ty * 32 + tx;          // 256 quads = 32 features x 8 frame-quads
     const int cl = q >> 3, lq = (q & 7) * 4;
     const int c = c0 + cl, l = l0 + lq;
     float v[4] = {0.f, 0.f, 0.f, 0.f};
-    if (c < p.D && l < p.L) philox_normal4(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, ((size_t)c * p.L + l) >> 2, v);
+    if (c < p.D && l < p.L)
+      philox_normal4(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + gs, ((size_t)c * gL + gf0 + l) >> 2, v);
 #pragma unroll
     for (int j = 0; j < 4; ++j) s_noise[cl][lq + j] = v[j];
   } else {
@@ -559,9 +611,9 @@ __device__ __forceinline__ void fill_noise_tile(const StepParams& p, int t, int 
       const int c = c0 + ty + i * 8, l = l0 + tx;
       float nz = 0.f;
       if (c < p.D && l < p.L) {
-        const size_t e = (size_t)c * p.L + l;
-        nz = p.noise_ref ? p.noise_ref[((size_t)(tape_t0 - t) * p.B + b) * p.D * p.L + e]
-                         : philox_normal(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + b, e);
+        const size_t e = (size_t)c * gL + gf0 + l;
+        nz = p.noise_ref ? p.noise_ref[((size_t)(tape_t0 - t) * gB + gs) * p.D * gL + e]
+                         : philox_normal(rng.seed, (unsigned long long)(t + 1), rng.sample_offset + gs, e);
       }
       s_noise[ty + i * 8][tx] = nz;
     }
@@ -577,6 +629,7 @@ __device__ __forceinline__ void fill_noise_tile(const StepParams& p, int t, int 
 // call's first step (step_ptr[3], or the tape_t0 argument), as p_sample_loop's draws are; the last step (s = 0)
 // returns m0 and reads no noise.  Advances s -> s - 1.
 // ---------------------------------------------------------------------------------------------
+template <bool kWin>
 __global__ void __launch_bounds__(256) dpm_solver_sde_step_kernel(const StepParams p, const DpmParams q) {
   griddep_launch_dependents();
   griddep_wait();
@@ -588,7 +641,7 @@ __global__ void __launch_bounds__(256) dpm_solver_sde_step_kernel(const StepPara
   const int k = p.step_ptr[2] - s;                      // loop iteration since the history started
   const int call_t0 = p.tape_t0 >= 0 ? p.tape_t0 : p.step_ptr[3];
   const int eff = min(min(q.order, k + 1), s + 1);      // effective order: lower while the history fills and at the end
-  if (s > 0) fill_noise_tile(p, s, call_t0, b, l0, c0, s_noise);
+  if (s > 0) fill_noise_tile<kWin>(p, s, call_t0, b, l0, c0, s_noise);
   __syncthreads();
   const float4 cf = *reinterpret_cast<const float4*>(q.coef + (size_t)s * 4);  // (A, B0, B1, Cn)
   {
@@ -602,7 +655,7 @@ __global__ void __launch_bounds__(256) dpm_solver_sde_step_kernel(const StepPara
       if (eff >= 2) m1v = *reinterpret_cast<const float4*>(q.x0_hist + (size_t)((k + 2) % 3) * q.hist_stride + idx);  // k - 1
       const float m1[4] = {m1v.x, m1v.y, m1v.z, m1v.w};
       float xtv[4], x04[4], xn4[4];
-      load_step_x0(p, idx, b, c, s, xtv, x04);
+      load_step_x0<kWin>(p, idx, b, c, s, xtv, x04);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float x0 = x04[j];
@@ -626,6 +679,7 @@ __global__ void __launch_bounds__(256) dpm_solver_sde_step_kernel(const StepPara
 // tile: frame-major operands are read/written with c fastest, the reference-layout noise tape with
 // l fastest, through a padded smem tile.
 // ---------------------------------------------------------------------------------------------
+template <bool kWin>
 __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p) {
   griddep_launch_dependents();
   griddep_wait();
@@ -639,7 +693,7 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
 
   // ---- noise tile (reference layout [b][c][l], l contiguous) ----
   const bool want_noise = p.sampler != 2;  // the reference draws noise at every step, including t == 0
-  if (want_noise) fill_noise_tile(p, t, tape_t0, b, l0, c0, s_noise);
+  if (want_noise) fill_noise_tile<kWin>(p, t, tape_t0, b, l0, c0, s_noise);
   __syncthreads();
 
   // ---- per-step scalars (fp32, gathered exactly like _extract_into_tensor(...).float()) ----
@@ -656,7 +710,7 @@ __global__ void __launch_bounds__(256) diffusion_step_kernel(const StepParams p)
     if (l < p.L && c < p.D_pad) {
       const size_t idx = ((size_t)b * p.L + l) * p.D_pad + c;
       float xtv[4], x04[4], xn4[4];
-      load_step_x0(p, idx, b, c, t, xtv, x04);
+      load_step_x0<kWin>(p, idx, b, c, t, xtv, x04);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float x0 = x04[j];
@@ -811,6 +865,32 @@ __global__ void __launch_bounds__(256) ref_to_frames_kernel(const float* __restr
       out_hi[idx] = h;
       if (out_lo) out_lo[idx] = lo;
     }
+  }
+}
+
+__global__ void __launch_bounds__(256) window_crop_kernel(const float* __restrict__ global, int Bg, int K, int D, int N, int F,
+                                                          const int* __restrict__ f0, float* __restrict__ windows) {
+  const size_t n = (size_t)Bg * K * D * F;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int l = (int)(i % F);
+    const size_t r = i / F;
+    const int c = (int)(r % D);
+    const int row = (int)(r / D);
+    windows[i] = global[((size_t)(row / K) * D + c) * N + f0[row % K] + l];
+  }
+}
+
+__global__ void __launch_bounds__(256) window_gather_kernel(const float* __restrict__ frames, int Bg, int K, int D, int N, int F,
+                                                            int D_pad, const int* __restrict__ f0, float* __restrict__ global) {
+  const size_t n = (size_t)Bg * D * N;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % N);
+    const size_t r = i / N;
+    const int c = (int)(r % D);
+    const int s = (int)(r / D);
+    int k = 0;
+    while (f0[k] + F <= g) ++k;  // the first window covering g (the last window ends at N)
+    global[i] = frames[(((size_t)s * K + k) * F + (g - f0[k])) * D_pad + c];
   }
 }
 
@@ -1045,7 +1125,8 @@ cudaError_t launch_token_rows(const TokenParams& p, cudaStream_t stream) {
 
 cudaError_t launch_diffusion_step(const StepParams& p, cudaStream_t stream) {
   dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
-  return launch_kernel(diffusion_step_kernel, grid, block, 0, stream, p);
+  const auto kernel = p.win_K > 1 ? diffusion_step_kernel<true> : diffusion_step_kernel<false>;
+  return launch_kernel(kernel, grid, block, 0, stream, p);
 }
 
 cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStream_t stream) {
@@ -1053,21 +1134,24 @@ cudaError_t launch_plms_step(const StepParams& p, const PlmsParams& q, cudaStrea
       !q.x_keep)
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
-  return launch_kernel(plms_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+  const auto kernel = p.win_K > 1 ? plms_step_kernel<true> : plms_step_kernel<false>;
+  return launch_kernel(kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_dpm_solver_step(const StepParams& p, const DpmParams& q, cudaStream_t stream) {
   if (q.order < 1 || q.order > 3 || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
-  return launch_kernel(dpm_solver_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+  const auto kernel = p.win_K > 1 ? dpm_solver_step_kernel<true> : dpm_solver_step_kernel<false>;
+  return launch_kernel(kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_dpm_solver_sde_step(const StepParams& p, const DpmParams& q, cudaStream_t stream) {
   if (q.order < 1 || q.order > 2 || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
     return cudaErrorInvalidValue;
   dim3 grid((p.L + 31) / 32, (p.D_pad + 31) / 32, p.B), block(32, 8);
-  return launch_kernel(dpm_solver_sde_step_kernel, grid, block, 0, stream, p, q);
+  const auto kernel = p.win_K > 1 ? dpm_solver_sde_step_kernel<true> : dpm_solver_sde_step_kernel<false>;
+  return launch_kernel(kernel, grid, block, 0, stream, p, q);
 }
 
 cudaError_t launch_repaint_step(const StepParams& p, const RepaintParams& q, cudaStream_t stream) {
@@ -1082,7 +1166,8 @@ cudaError_t launch_unipc_step(const StepParams& p, const UnipcParams& q, cudaStr
   if (q.order < 1 || q.order > 3 || (q.corrector && !q.xc) || (p.D_pad & 3) || !p.x_next || !p.x_next_hi || !q.x0_hist || !q.coef)
     return cudaErrorInvalidValue;
   const size_t n4 = (size_t)p.B * p.L * p.D_pad / 4;
-  return launch_kernel(unipc_step_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
+  const auto kernel = p.win_K > 1 ? unipc_step_kernel<true> : unipc_step_kernel<false>;
+  return launch_kernel(kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, stream, p, q);
 }
 
 cudaError_t launch_ddim_reverse_step(const StepParams& p, cudaStream_t stream) {
@@ -1101,6 +1186,18 @@ cudaError_t launch_ref_to_frames(const float* ref, int B, int D, int L, int D_pa
 cudaError_t launch_frames_to_ref(const float* frames, int B, int D, int L, int D_pad, float* ref, cudaStream_t stream) {
   dim3 grid((L + 31) / 32, (D + 31) / 32, B), block(32, 8);
   frames_to_ref_kernel<<<grid, block, 0, stream>>>(frames, B, D, L, D_pad, ref);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_crop(const float* global, int Bg, int K, int D, int N, int F, const int* f0, float* windows,
+                               cudaStream_t stream) {
+  window_crop_kernel<<<grid_for((size_t)Bg * K * D * F, 256), 256, 0, stream>>>(global, Bg, K, D, N, F, f0, windows);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_gather(const float* frames, int Bg, int K, int D, int N, int F, int D_pad, const int* f0,
+                                 float* global, cudaStream_t stream) {
+  window_gather_kernel<<<grid_for((size_t)Bg * D * N, 256), 256, 0, stream>>>(frames, Bg, K, D, N, F, D_pad, f0, global);
   return cudaGetLastError();
 }
 

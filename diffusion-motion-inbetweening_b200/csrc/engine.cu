@@ -99,6 +99,7 @@ struct GraphKey {
                                    // step's second evaluation
   int variant, corrector;          // UniPC
   int jump_length, jump_n_sample;  // RePaint
+  int win_K, win_N;                // overlapping windows (the first frames live in device memory)
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -195,6 +196,7 @@ struct cmdi_engine {
   int hist_sampler = 0, hist_order = 0, hist_B = 0, hist_t_start = 0, hist_steps = 0;
   int hist_variant = 0, hist_corrector = 0;  // UniPC
   int hist_jump_n_sample = 0;                // RePaint (hist_order holds its jump length)
+  std::vector<int> hist_win;                 // overlapping windows of the running history: N, then the first frames
   std::vector<WalkOp> walk;                  // RePaint: the running walk and the index of its next op
   size_t walk_next = 0;
   std::vector<double> h_betas;     // betas of the schedule (float64)
@@ -206,6 +208,10 @@ struct cmdi_engine {
   float* unipc_coef = nullptr;     // their device copy (allocated by the first UniPC call on a schedule)
   std::map<GraphKey, cudaGraphExec_t> graphs;
   int64_t launches = 0;
+  // overlapping windows, allocated by the first windowed call: the first frames [maxB] and the windows' x_T [maxB, D, L]
+  int* win_f0 = nullptr;
+  std::vector<int> h_win_f0;  // the first frames last copied to win_f0
+  float* win_ref = nullptr;
 };
 
 namespace {
@@ -1464,6 +1470,7 @@ StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool gui
   sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
   sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
   sp.pred_xstart = e->pred_x0;
+  sp.win_K = a->window_count; sp.win_N = a->global_frames; sp.win_f0 = e->win_f0;
   return sp;
 }
 
@@ -1488,6 +1495,7 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.order = plms ? a->plms_order : a->sampler == CMDI_SAMPLER_UNIPC ? a->unipc_order : a->dpm_order;
   key.variant = a->unipc_variant; key.corrector = a->unipc_corrector;
   key.jump_length = a->repaint_jump_length; key.jump_n_sample = a->repaint_jump_n_sample;
+  key.win_K = a->window_count; key.win_N = a->global_frames;
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
@@ -1533,6 +1541,63 @@ int capture_step_graph(cmdi_engine* e, const GraphKey& key, Enqueue enqueue, cud
   }
   e->graphs[key] = ex;
   *out_exec = ex;
+  return 0;
+}
+
+// The window placement of a call as a history records it: empty without windows, else N and the first frames.
+std::vector<int> window_key(const cmdi_sample_args* a) {
+  std::vector<int> k;
+  if (a->window_count > 0) {
+    k.push_back(a->global_frames);
+    k.insert(k.end(), a->window_frames0, a->window_frames0 + a->window_count);
+  }
+  return k;
+}
+
+// The overlapping-window fields of a call: all unset, or a placement the step kernels can blend (cmdi_sample_args).
+int check_windows(const cmdi_engine* e, const cmdi_sample_args* a) {
+  const int K = a->window_count, N = a->global_frames, F = e->L;
+  if (K == 0) {
+    const char* f = a->window_frames0 ? "window_frames0" : a->global_frames ? "global_frames" : a->window_out ? "window_out" : nullptr;
+    if (f) {
+      set_last_error("%s is a window field: it must be unset when window_count is 0", f);
+      return 1;
+    }
+    return 0;
+  }
+  if (K < 0) {
+    set_last_error("window_count %d must be >= 0", K);
+    return 1;
+  }
+  if (a->sampler == CMDI_SAMPLER_DDIM_REVERSE || a->sampler == CMDI_SAMPLER_REPAINT) {
+    set_last_error("window_count: sampler %d (DDIM inversion / RePaint) does not run on overlapping windows", a->sampler);
+    return 1;
+  }
+  if (a->batch % K) {
+    set_last_error("window_count %d does not divide batch %d (row s * K + k is window k of global sample s)", K, a->batch);
+    return 1;
+  }
+  if (!a->window_frames0) {
+    set_last_error("window_frames0 is required when window_count is set");
+    return 1;
+  }
+  if (N < F) {
+    set_last_error("global_frames %d is shorter than a window (%d frames)", N, F);
+    return 1;
+  }
+  const int32_t* f0 = a->window_frames0;
+  for (int k = 0; k < K; ++k) {
+    const bool bad = k == 0 ? f0[0] != 0 : (f0[k] <= f0[k - 1] || f0[k] > f0[k - 1] + F);
+    if (bad || (k == K - 1 && f0[k] != N - F)) {
+      set_last_error("window_frames0[%d] = %d: the first frames must start at 0, ascend strictly with no gap between "
+                     "windows of %d frames, and end at global_frames - %d = %d", k, f0[k], F, F, N - F);
+      return 1;
+    }
+  }
+  if (a->plms_old_eps_out) {
+    set_last_error("plms_old_eps_out must be NULL on overlapping windows");
+    return 1;
+  }
   return 0;
 }
 
@@ -1618,6 +1683,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     set_last_error("plms_order %d outside [2, 4]", a->plms_order);
     return 1;
   }
+  CKI(check_windows(e, a));
   if (plms && (a->noise_tape || a->dump_xstart)) {
     set_last_error("PLMS draws no per-step noise and has no dump_steps: noise_tape and dump_xstart must be NULL");
     return 1;
@@ -1649,6 +1715,23 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   }
   const bool host = a->host_buffers != 0;
   const size_t n = (size_t)B * e->D * e->L;
+  // overlapping windows: x_T, the noise and the outputs are global (Bg, D, 1, N), everything else is per window
+  const bool win = a->window_count > 0;
+  const int Bg = win ? B / a->window_count : B, N = win ? a->global_frames : e->L;
+  const size_t ng = (size_t)Bg * e->D * N;
+  if (win) {
+    if (!e->win_f0) {
+      CKI(dev_alloc(e, &e->win_f0, (size_t)e->maxB));
+      CKI(dev_alloc(e, &e->win_ref, (size_t)e->maxB * e->D * e->L));
+    }
+    // a copy from pageable host memory waits for the stream: it is made only when the placement changes (the
+    // generators' one-step calls and repeated loops reuse the table on the device)
+    const std::vector<int> f0(a->window_frames0, a->window_frames0 + a->window_count);
+    if (f0 != e->h_win_f0) {
+      CK(cudaMemcpyAsync(e->win_f0, f0.data(), f0.size() * 4, cudaMemcpyHostToDevice, s));
+      e->h_win_f0 = f0;
+    }
+  }
   const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
   const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
   int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
@@ -1665,7 +1748,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
                                      t0 == e->walk[e->walk_next].p - (e->walk[e->walk_next].undo ? 1 : 0);
       if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
           e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
-          e->hist_jump_n_sample != a->repaint_jump_n_sample || !at) {
+          e->hist_jump_n_sample != a->repaint_jump_n_sample || e->hist_win != window_key(a) || !at) {
         set_last_error("%s resume at step %d does not continue the running history",
                        plms ? "PLMS" : unipc ? "UniPC" : sde ? "SDE-DPM-Solver++" : repaint ? "RePaint" : "DPM-Solver++", t0);
         return 1;
@@ -1711,6 +1794,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
       e->hist_variant = a->unipc_variant; e->hist_corrector = a->unipc_corrector;
       e->hist_jump_n_sample = a->repaint_jump_n_sample;
+      e->hist_win = window_key(a);
     }
   }
   if (repaint) {  // num_steps counts denoise ops
@@ -1723,7 +1807,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   int rc = 0;
 
   // ---- x_T (gaussian_diffusion.py:1245-1248) ----
-  const float* xT = (const float*)stage_in(a->x_T, e->ref_a, n * 4, host, s, &rc);
+  const float* xT = (const float*)stage_in(a->x_T, e->ref_a, ng * 4, host, s, &rc);
   if (rc) return 1;
   RngState rng{};
   rng.seed = a->seed; rng.sample_offset = a->sample_offset; rng.mode = a->rng_mode;
@@ -1739,12 +1823,17 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   }
   if (!xT) {
     if (a->rng_mode == CMDI_RNG_TORCH) {
-      CK(launch_fill_normal_aten(e->ref_a, n, a->seed, a->aten_offset, a->aten_threads, s));
+      CK(launch_fill_normal_aten(e->ref_a, ng, a->seed, a->aten_offset, a->aten_threads, s));
       rng.aten_offset += a->aten_increment;  // the per-step draws follow the x_T draw in the stream
     } else {
-      CK(launch_fill_normal_ref(e->ref_a, B, (size_t)e->D * e->L, a->seed, 0ull, a->sample_offset, s));
+      CK(launch_fill_normal_ref(e->ref_a, Bg, (size_t)e->D * N, a->seed, 0ull, a->sample_offset, s));
     }
     xT = e->ref_a;
+    e->launches += 1;
+  }
+  if (win) {  // the windows' crops of the global x_T
+    CK(launch_window_crop(xT, Bg, a->window_count, e->D, N, e->L, e->win_f0, e->win_ref, s));
+    xT = e->win_ref;
     e->launches += 1;
   }
   CK(launch_set_rng(e->rng, rng, s));
@@ -1849,6 +1938,13 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   // is one step.
   const int group = !plms && e->steps_per_graph > 1 ? e->steps_per_graph : 1;
 
+  // a frame-major state [B*L, D_pad] -> the reference layout of the call's outputs: per sample, or on overlapping windows
+  // the global (Bg, D, 1, N) gathered from the first window covering each frame
+  auto to_ref = [&](const float* frames, float* dst) -> int {
+    if (win) CK(launch_window_gather(frames, Bg, a->window_count, e->D, N, e->L, e->D_pad, e->win_f0, dst, s));
+    else CK(launch_frames_to_ref(frames, B, e->D, e->L, e->D_pad, dst, s));
+    return 0;
+  };
   int dump_i = 0;
   // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
   auto guided_at = [&](int k) { return a->recon_guidance && (rev ? t0 + k : t0 - k) >= a->stop_recguidance_at; };
@@ -1903,11 +1999,11 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     k += run;
     if (a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] == k - 1) {
       if (host) {
-        CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, e->ref_b, s));
-        CK(cudaMemcpyAsync(a->dump_xstart + (size_t)dump_i * n, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));
+        CKI(to_ref(e->pred_x0, e->ref_b));
+        CK(cudaMemcpyAsync(a->dump_xstart + (size_t)dump_i * ng, e->ref_b, ng * 4, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
       } else {
-        CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, a->dump_xstart + (size_t)dump_i * n, s));
+        CKI(to_ref(e->pred_x0, a->dump_xstart + (size_t)dump_i * ng));
       }
       e->launches += 1;
       ++dump_i;
@@ -1915,18 +2011,26 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   }
   // ---- results back in the reference layout ----
   if (host) {
-    CK(launch_frames_to_ref(e->x_state, B, e->D, e->L, e->D_pad, e->ref_a, s));
-    CK(cudaMemcpyAsync(out, e->ref_a, n * 4, cudaMemcpyDeviceToHost, s));
+    CKI(to_ref(e->x_state, e->ref_a));
+    CK(cudaMemcpyAsync(out, e->ref_a, ng * 4, cudaMemcpyDeviceToHost, s));
     if (a->pred_xstart_out) {
-      CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, e->ref_b, s));
-      CK(cudaMemcpyAsync(a->pred_xstart_out, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));
+      CKI(to_ref(e->pred_x0, e->ref_b));
+      CK(cudaMemcpyAsync(a->pred_xstart_out, e->ref_b, ng * 4, cudaMemcpyDeviceToHost, s));
     }
     CK(cudaStreamSynchronize(s));
   } else {
-    CK(launch_frames_to_ref(e->x_state, B, e->D, e->L, e->D_pad, out, s));
-    if (a->pred_xstart_out) CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, a->pred_xstart_out, s));
+    CKI(to_ref(e->x_state, out));
+    if (a->pred_xstart_out) CKI(to_ref(e->pred_x0, a->pred_xstart_out));
   }
   e->launches += a->pred_xstart_out ? 2 : 1;
+  if (a->window_out) {  // the windows' own states, in the window layout
+    CK(launch_frames_to_ref(e->x_state, B, e->D, e->L, e->D_pad, host ? e->ref_a : a->window_out, s));
+    if (host) {
+      CK(cudaMemcpyAsync(a->window_out, e->ref_a, n * 4, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+    }
+    e->launches += 1;
+  }
   if (multistep) e->hist_steps += nsteps;
   if (plms) {
     if (a->plms_old_eps_out) {

@@ -238,8 +238,20 @@ struct StepParams {
   __nv_bfloat16* x_next_hi;
   __nv_bfloat16* x_next_lo;
   float* pred_xstart;          // [B*L, D_pad] or null
+  // overlapping windows (win_K > 1): row b = s * win_K + k is window k of global sample s, and its frame l is global
+  // frame win_f0[k] + l of win_N.  x0 is blended over the windows covering a frame (tent weights, ascending k), and the
+  // noise of (b, l) is that of (s, win_f0[k] + l) in the global (B / win_K, D, 1, win_N) layout.  win_K <= 1: off.
+  int win_K, win_N;
+  const int* win_f0;           // device [win_K], strictly ascending; win_f0[0] = 0, win_f0[win_K - 1] = win_N - L
 };
 cudaError_t launch_diffusion_step(const StepParams& p, cudaStream_t stream);
+// global ref layout (Bg, D, 1, N) -> the windows' ref layout (Bg * K, D, 1, F): window s * K + k is frames [f0[k], f0[k] + F)
+cudaError_t launch_window_crop(const float* global, int Bg, int K, int D, int N, int F, const int* f0, float* windows,
+                               cudaStream_t stream);
+// frame-major window state [Bg * K * F, D_pad] -> global ref layout (Bg, D, 1, N), each frame from the first window
+// covering it
+cudaError_t launch_window_gather(const float* frames, int Bg, int K, int D, int N, int F, int D_pad, const int* f0,
+                                 float* global, cudaStream_t stream);
 // PLMS step (gaussian_diffusion.py:1589-1687) on the same state and combine inputs as StepParams (its sampler, eta,
 // noise, rng, tape and advance fields are not read; x_next / x_next_hi are required).  The eps history is a device
 // ring indexed by the loop iteration k = step_ptr[2] - t, so one captured graph serves every Adams-Bashforth step.

@@ -82,6 +82,57 @@ class DiffusionConfig:
     extra: dict = field(default_factory=dict)
 
 
+@dataclass(frozen=True)
+class Window:
+    """Sample motions longer than the denoiser's window as overlapping windows (`GaussianDiffusion.window`).
+
+    A motion of N frames is covered by K = 1 + ceil((N - frames) / (frames - overlap)) windows of `frames` frames
+    (K = 1 when N <= frames: the plain loop at N frames); window k starts at global frame
+    f0(k) = min(k * (frames - overlap), N - frames), so the last one is end-aligned.  At every step the x0 of a frame
+    that several windows cover (after CFG, reconstruction guidance and imputation) is replaced by their tent-weighted
+    mean, w_k(g) = 1 + min(g - f0(k), f0(k) + frames - 1 - g), so the windows agree on their shared frames (the
+    "handshake" of PriorMDM's DoubleTake, MultiDiffusion's averaging).  `frames` must be within the engine's limit for
+    the architecture (207 for the transformer, 224 for MDM_UNET); 0 <= overlap <= frames // 2."""
+    frames: int
+    overlap: int = 0
+
+    def __post_init__(self):
+        for name in ("frames", "overlap"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError(f"Window {name} must be an int, got {v!r}")
+        if self.frames < 1:
+            raise ValueError(f"Window frames must be >= 1, got {self.frames}")
+        if not 0 <= self.overlap <= self.frames // 2:
+            raise ValueError(f"Window overlap must be in [0, frames // 2 = {self.frames // 2}], got {self.overlap}")
+
+    def placement(self, n: int) -> List[int]:
+        """First global frame of each window of an n-frame motion."""
+        F, O = int(self.frames), int(self.overlap)
+        if n <= F:
+            return [0]
+        K = 1 + -(-(n - F) // (F - O))
+        return [min(k * (F - O), n - F) for k in range(K)]
+
+
+def _crop_windows(x: torch.Tensor, f0: List[int], F: int) -> torch.Tensor:
+    """(B, ..., N) in the global layout -> (B * K, ..., F): row b * K + k holds frames [f0[k], f0[k] + F) of sample b."""
+    idx = torch.tensor(f0, device=x.device)[:, None] + torch.arange(F, device=x.device)
+    return x[..., idx].movedim(-2, 1).reshape(x.shape[0] * len(f0), *x.shape[1:-1], F).contiguous()
+
+
+def _window_prompts(text, B: int, K: int) -> list:
+    """y['text'] of a windowed call as one prompt per window: B lists of K prompts (window k of sample b gets
+    text[b][k]), or B prompts (every window of sample b gets text[b])."""
+    if len(text) != B:
+        raise ValueError(f"y['text'] must hold one entry per sample ({B}), got {len(text)}")
+    if all(isinstance(t, (list, tuple)) for t in text):
+        if any(len(t) != K for t in text):
+            raise ValueError(f"per-window prompts: every sample needs one prompt per window ({K})")
+        return [p for t in text for p in t]
+    return [t for t in text for _ in range(K)]
+
+
 def _enum_name(v) -> str:
     return getattr(v, "name", str(v))
 
@@ -133,6 +184,9 @@ class GaussianDiffusion:
         # sample index (sharding-independent; used by distributed.sharded_sample)
         self.rng = "torch"
         self.engine_seed = None  # rng="engine": explicit Philox key (sharded_sample broadcasts rank 0's); None = draw one
+        # Window(frames, overlap): shapes (B, D, 1, N) of any length run as overlapping windows blended at every step;
+        # None = one denoiser window per sequence
+        self.window = None
 
     # ------------------------------------------------------------------------------------------
     def q_sample(self, x_start, t, noise=None):
@@ -181,8 +235,18 @@ class GaussianDiffusion:
             device = next(model.parameters()).device
         device = torch.device(device)
         B = int(shape[0])
-        eng = inner.engine_for(device, max_batch=max(B, self.max_batch or 0), precision=self.precision,
-                                nframes=int(shape[-1]))
+        # overlapping windows: f0 = their first frames, crop = a global-layout tensor -> the windows' rows
+        f0 = None
+        if self.window is not None:
+            if rev or sampler == capi.SAMPLER_REPAINT:
+                raise NotImplementedError("DDIM inversion and RePaint do not run on overlapping windows (diffusion.window)")
+            if not isinstance(self.window, Window):
+                raise TypeError(f"diffusion.window must be a Window or None, got {self.window!r}")
+            f0 = self.window.placement(int(shape[-1]))
+            f0 = f0 if len(f0) > 1 else None  # one window: the plain loop at N frames
+        K, F = (len(f0), self.window.frames) if f0 else (1, int(shape[-1]))
+        crop = (lambda t: None if t is None else _crop_windows(t, f0, F)) if f0 else (lambda t: t)
+        eng = inner.engine_for(device, max_batch=max(B * K, self.max_batch or 0), precision=self.precision, nframes=F)
         eng.set_schedule(self.betas, self.timestep_map)
 
         # ---- conditioning ----
@@ -191,10 +255,12 @@ class GaussianDiffusion:
         if "action" in cond_mode:
             raise NotImplementedError("action conditioning is not on the HumanML3D path")
         if "text" in cond_mode:
-            cond_emb = inner.encode_text(y["text"]).to(device=device, dtype=torch.float32)  # once per loop (mdm.py:249 does it per step)
+            # with a window set, y['text'] may hold one prompt per window, also when one window covers the motion
+            text = _window_prompts(y["text"], B, K) if self.window is not None else y["text"]
+            cond_emb = inner.encode_text(text).to(device=device, dtype=torch.float32)  # once per loop (mdm.py:249 does it per step)
         if is_cfg:
             assert cond_mode in ["text", "action"]  # cfg_sampler.py:27
-            text_scale = y["text_scale"].to(device=device, dtype=torch.float32).reshape(-1)
+            text_scale = y["text_scale"].to(device=device, dtype=torch.float32).reshape(-1).repeat_interleave(K)
         # ---- keyframe imputation (gaussian_diffusion.py:427-442, editing_util.py:336-346) ----
         imputate, stop_at, obs, mask, y_mask = False, 0, None, None, None
         guided_cfg = bool(y.get("reconstruction_guidance", False))
@@ -209,7 +275,7 @@ class GaussianDiffusion:
                 obs = y["inpainted_motion"].to(device=device, dtype=torch.float32)
                 mask = y["inpainting_mask"].to(device=device)
                 assert obs.shape == mask.shape == tuple(shape)
-                y_mask = y["mask"].to(device=device).reshape(B, -1)
+                obs, mask, y_mask = crop(obs), crop(mask), crop(y["mask"].to(device=device).reshape(B, -1))
             elif dist == "marginal":
                 pass  # the reference's 'marginal' branch only calls the model (:437-439)
             else:
@@ -222,7 +288,7 @@ class GaussianDiffusion:
                 obs = y["inpainted_motion"].to(device=device, dtype=torch.float32)
                 mask = y["inpainting_mask"].to(device=device)
                 assert obs.shape == mask.shape == tuple(shape)  # :414
-                y_mask = y["mask"].to(device=device).reshape(B, -1)
+                obs, mask, y_mask = crop(obs), crop(mask), crop(y["mask"].to(device=device).reshape(B, -1))
             # w_r[t] * sqrt(alpha_bar_t) / 2, in fp32 exactly as the reference forms it (:418-422); the schedule is
             # indexed by the sampler step t like _extract_into_tensor(grad_ws, t, ...) does
             ws = get_gradient_schedule(y["gradient_schedule"], y["diffusion_steps"])
@@ -274,14 +340,14 @@ class GaussianDiffusion:
         if skip_timesteps and init_image is None and not rev:
             init_image = torch.zeros(tuple(shape), device=device, dtype=torch.float32)
         if init_image is not None:
-            init_image = init_image.to(device=device, dtype=torch.float32)
+            init_image = crop(init_image.to(device=device, dtype=torch.float32))
         # keyframe INPUT conditioning (MDM_UNET.forward's obs_x0 / obs_mask): top-level model_kwargs, as
         # sample/conditional_synthesis.py:159-162 passes them; the transformer ignores them
         kf_obs, kf_mask = None, None
         if eng.arch == capi.ARCH_UNET and model_kwargs.get("obs_x0") is not None:
-            kf_obs = model_kwargs["obs_x0"].to(device=device, dtype=torch.float32)
-            kf_mask = model_kwargs["obs_mask"].to(device=device)
-        common = dict(batch=B, sampler=sampler, eta=eta, cond_emb=cond_emb, uncond=uncond, cfg=is_cfg, text_scale=text_scale,
+            kf_obs = crop(model_kwargs["obs_x0"].to(device=device, dtype=torch.float32))
+            kf_mask = crop(model_kwargs["obs_mask"].to(device=device))
+        common = dict(batch=B * K, sampler=sampler, eta=eta, cond_emb=cond_emb, uncond=uncond, cfg=is_cfg, text_scale=text_scale,
                       obs_x0=kf_obs, obs_mask=kf_mask,
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
@@ -293,6 +359,8 @@ class GaussianDiffusion:
                           unipc_corrector=bool(corrector))
         if sampler == capi.SAMPLER_REPAINT:
             common.update(repaint_jump_length=int(jump_length), repaint_jump_n_sample=int(jump_n_sample))
+        if f0:  # x_T, the noise and the outputs stay global (B, D, 1, N)
+            common.update(window_frames0=f0, global_frames=int(shape[-1]))
         if progressive:
             return self._step_generator(eng, x_T, init_image, skip_timesteps, tape, common)
         if rev:
@@ -311,11 +379,13 @@ class GaussianDiffusion:
         their samples equal the fused loop's bit for bit; a caller that stops an inversion early has a partial one.
         PLMS also yields old_eps, the values of the reference's history list at that yield (the reference yields one
         list it keeps mutating).  RePaint makes one call per denoise op, which also runs the undo ops before it, and
-        yields the op's position as "t"."""
+        yields the op's position as "t".  On overlapping windows every call crops the global state it starts from,
+        which holds the bits every covering window holds, and PLMS yields no old_eps (its history is per window)."""
         common = dict(common)
         common["use_graph"] = 2 if common.get("use_graph", True) else 0  # one native call per step, same step graph every time
         plms = common["sampler"] == capi.SAMPLER_PLMS
         repaint = common["sampler"] == capi.SAMPLER_REPAINT
+        unwindowed = "window_frames0" not in common
         torch_rng = common.get("rng_mode", capi.RNG_ENGINE) == capi.RNG_TORCH
         off0, inc = common.pop("aten_offset", 0), common.get("aten_increment", 0)
         T = self.num_timesteps
@@ -337,7 +407,7 @@ class GaussianDiffusion:
                 call.update(resume=(k > 0), init_image=init_image if k == 0 else None)
             if torch_rng:
                 call["aten_offset"] = off0 + d0 * inc  # each call starts at its own draw of the stream
-            res = eng.sample(skip_timesteps=skip, num_steps=1, x_T=state, want_pred_xstart=True, want_old_eps=plms,
+            res = eng.sample(skip_timesteps=skip, num_steps=1, x_T=state, want_pred_xstart=True, want_old_eps=plms and unwindowed,
                              noise_tape=None if tape is None else tape[d0:], **call, **common)
             state = res["sample"]
             if torch_rng:
@@ -345,7 +415,7 @@ class GaussianDiffusion:
                 # breaks out of the generator early leaves it where the reference would
                 _advance_torch_generator(eng.device, n_draws * inc)
             step = {"sample": res["sample"], "pred_xstart": res["pred_xstart"]}
-            if plms:
+            if plms and unwindowed:
                 step["old_eps"] = res["old_eps"]
             if repaint:
                 step["t"] = t

@@ -35,6 +35,8 @@ def sharded_sample(diffusion, model, shape, model_kwargs: Optional[dict] = None,
     shape is the GLOBAL (B, njoints, 1, nframes); B must divide by the world size.  Works with any backend
     (NCCL on GPUs; gloo is used by the CPU tests of the sharding logic with a stand-in sampler).
     """
+    if getattr(diffusion, "window", None) is not None:
+        raise NotImplementedError("sharded_sample does not shard overlapping windows (diffusion.window)")
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     B = int(shape[0])

@@ -125,7 +125,8 @@ class Engine:
                use_graph: bool = True, out: Optional[torch.Tensor] = None, obs_x0: Optional[torch.Tensor] = None,
                obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False,
                dpm_order: int = 2, unipc_order: int = 2, unipc_variant: int = capi.UNIPC_BH2, unipc_corrector: bool = True,
-               repaint_jump_length: int = 10, repaint_jump_n_sample: int = 10):
+               repaint_jump_length: int = 10, repaint_jump_n_sample: int = 10,
+               window_frames0: Optional[Sequence[int]] = None, global_frames: int = 0, want_window_out: bool = False):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -146,8 +147,14 @@ class Engine:
         (sent for this sampler only), one draw per op of its walk (noise_tape, seed / rng_mode); num_steps counts
         denoise ops, and resume continues the walk from the position it has reached (skip_timesteps = T - 1 - that
         position).
+        window_frames0 / global_frames: overlapping windows (cmdi_sample_args.window_count): `batch` counts windows, row
+        s * K + k is window k of global sample s and covers global frames [window_frames0[k], window_frames0[k] + nframes)
+        of global_frames.  x_T, noise_tape and the outputs are global (batch // K, njoints, 1, global_frames); the other
+        tensors are per window.  want_window_out adds result["windows"], the windows' final states.
         """
         shape = (batch, self.njoints, 1, self.nframes)
+        K = 0 if window_frames0 is None else len(window_frames0)
+        gshape = (batch // K, self.njoints, 1, int(global_frames)) if K else shape
         dev = torch.device("cpu") if host_buffers else self.device
 
         def prep(t, dtype=torch.float32, shp=None):
@@ -161,7 +168,7 @@ class Engine:
                 raise ValueError(f"tensor on {t.device}, expected {dev} (host_buffers={host_buffers})")
             return t
 
-        init_image, x_T = prep(init_image, shp=shape), prep(x_T, shp=shape)
+        init_image, x_T = prep(init_image, shp=shape), prep(x_T, shp=gshape)
         cond_emb, text_scale = prep(cond_emb, shp=(batch, 512)), prep(text_scale, shp=(batch,))
         y_mask = prep(y_mask, torch.uint8, (batch, self.nframes))
         inpainted_motion = prep(inpainted_motion, shp=shape)
@@ -172,8 +179,10 @@ class Engine:
             if noise_tape.device != self.device:
                 raise ValueError("noise_tape must live on the engine's device")
         if out is None:
-            out = torch.empty(shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
-        pred = torch.empty(shape, dtype=torch.float32, device=dev, pin_memory=host_buffers) if want_pred_xstart else None
+            out = torch.empty(gshape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
+        pred = torch.empty(gshape, dtype=torch.float32, device=dev, pin_memory=host_buffers) if want_pred_xstart else None
+        windows = torch.empty(shape, dtype=torch.float32, device=dev, pin_memory=host_buffers) if want_window_out else None
+        f0_arr = (ctypes.c_int32 * max(K, 1))(*[int(f) for f in (window_frames0 or [])])
         dump, dump_arr, n_dump = None, None, 0
         if dump_steps is not None:
             # one entry per loop iteration that matches, like the reference's `if i in dump_steps` (:1208-1213):
@@ -184,7 +193,7 @@ class Engine:
             steps_sorted = sorted({int(s) for s in dump_steps if 0 <= int(s) < n_iter})
             n_dump = len(steps_sorted)
             dump_arr = (ctypes.c_int32 * max(n_dump, 1))(*steps_sorted)
-            dump = torch.empty((max(n_dump, 1),) + shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
+            dump = torch.empty((max(n_dump, 1),) + gshape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
         coef_arr = None
         if recon_guidance:
             coef = np.ascontiguousarray(np.asarray(recon_coef, dtype=np.float32))
@@ -214,7 +223,8 @@ class Engine:
                             _ptr(old_eps), int(dpm_order) if dpm else 0,
                             int(unipc_order) if unipc else 0, int(unipc_variant) if unipc else 0,
                             int(unipc_corrector) if unipc else 0,
-                            int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0)
+                            int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0,
+                            K, f0_arr if K else None, int(global_frames), _ptr(windows))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
@@ -225,6 +235,8 @@ class Engine:
                 result["old_eps"] = [old_eps[i] for i in range(n_old)]
         if pred is not None:
             result["pred_xstart"] = pred
+        if windows is not None:
+            result["windows"] = windows
         if dump is not None:
             result["dump"] = [dump[i] for i in range(n_dump)]
         return result

@@ -130,6 +130,8 @@ def run_eval_jobs(diffusion, model, jobs: Sequence[EvalJob], sampler: str = "p_s
     the world size.  rng="torch": `fixseed(job.seed_number)` (default torch.manual_seed) before each call and torch's
     generator stream inside it, one call per job (merge is forced to 1), as the reference loop does.
     """
+    if getattr(diffusion, "window", None) is not None:
+        raise NotImplementedError("run_eval_jobs does not run overlapping windows (diffusion.window)")
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     if rng == "torch":

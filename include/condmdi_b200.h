@@ -203,6 +203,27 @@ typedef struct {
   /* CMDI_SAMPLER_REPAINT only (both 0 for every other sampler); RePaint's names */
   int32_t repaint_jump_length;  /* >= 1: positions an undo run goes up */
   int32_t repaint_jump_n_sample; /* >= 1: passes over each jumped stretch (1 = no resampling) */
+  /* Overlapping windows: a motion of global_frames = N frames, longer than the engine's nframes = F, sampled as
+     window_count = K windows of F frames whose x0 is blended at every step (all four fields 0 / NULL: off).  Row
+     s * K + k of the batch is window k of global sample s and covers global frames [window_frames0[k],
+     window_frames0[k] + F); batch counts windows (max_batch too), so batch = B_global * K.
+       - window_frames0[0] = 0, window_frames0[K - 1] = N - F, strictly ascending, and consecutive windows leave no gap.
+       - x0 (after CFG, guidance and imputation) of a frame covered by several windows is sum_k w_k x0_k / sum_k w_k over
+         them in ascending k, fp32 with round-to-nearest products, sums and quotient, w_k = 1 + the frame's distance to
+         the nearer end of window k; a frame covered by one window keeps its x0.  Every covering window stores the same
+         bits at a shared frame (state, pred_xstart, multistep histories).
+       - Global layout (B_global, njoints, 1, N): x_T, noise_tape ((num_steps, B_global, njoints, 1, N)), out,
+         pred_xstart_out and dump_xstart; the engine crops x_T into the windows once per call and gathers the outputs
+         from the first window covering each frame.  Every draw is that of the global tensor: the CMDI_RNG_TORCH stream of
+         B_global * njoints * N elements (aten_increment / aten_threads for that numel), the engine generator keyed by
+         (global sample, element c * N + g).
+       - Window layout (batch, ...): cond_emb, text_scale, y_mask, inpainted_motion, inpainting_mask, obs_x0, obs_mask
+         and init_image, cropped by the caller (a window may carry its own prompt).
+     Samplers DDPM, DDIM, PLMS, DPM_SOLVER, UNIPC and DPM_SOLVER_SDE; plms_old_eps_out must be NULL. */
+  int32_t window_count;         /* K >= 1, or 0: no windows */
+  const int32_t* window_frames0; /* HOST array [K]: first global frame of each window */
+  int32_t global_frames;        /* N */
+  float* window_out;            /* test aid: NULL, or (batch, njoints, 1, F) the windows' final states (window layout) */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
