@@ -32,7 +32,7 @@ EXPORTS = [
     "cmdi_sample", "cmdi_launch_count", "cmdi_last_error", "cmdi_version", "cmdi_test_linear", "cmdi_test_attention",
     "cmdi_test_layernorm", "cmdi_test_step", "cmdi_test_normal", "cmdi_profile_pass", "cmdi_test_layernorm_bwd", "cmdi_test_attention_bwd",
     "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp", "cmdi_joints_to_features", "cmdi_convert_motion",
-    "cmdi_test_chain_layer", "cmdi_test_attention_hi", "cmdi_test_attention_bwd_at",
+    "cmdi_test_chain_layer", "cmdi_test_attention_hi", "cmdi_test_attention_bwd_at", "cmdi_test_unet_ops",
 ]
 
 
@@ -67,6 +67,27 @@ class SampleArgs(Structure):
                 ("repaint_jump_length", c_int32), ("repaint_jump_n_sample", c_int32),
                 ("window_count", c_int32), ("window_frames0", POINTER(c_int32)), ("global_frames", c_int32),
                 ("window_out", c_void_p)]
+
+
+class UnetOpInfo(Structure):
+    """cmdi_unet_op_info: one MDM_UNET op as cmdi_test_unet_ops describes it to its hook."""
+    _fields_ = [("name", c_char_p), ("kind", c_int32), ("list_ops", c_int32), ("num_seqs", c_int32), ("f16", c_int32),
+                ("temb_table", c_void_p), ("cond_proj", c_void_p), ("uncond_proj", c_void_p), ("n_cond_seqs", c_int32),
+                ("in_level", c_int32), ("out_level", c_int32), ("in_hi", c_void_p), ("in_lo", c_void_p), ("in_f32", c_void_p),
+                ("in_ld", c_int32), ("out_hi", c_void_p), ("out_lo", c_void_p), ("out_ld", c_int32), ("out_f32", c_void_p),
+                ("out_ld32", c_int32), ("w_hi", c_void_p), ("w_lo", c_void_p), ("w_ld", c_int32), ("N", c_int32), ("K", c_int32),
+                ("num_taps", c_int32), ("k_per_tap", c_int32), ("nsplit", c_int32), ("nsplit_out", c_int32), ("sum32", c_int32),
+                ("act", c_int32), ("rowmap", c_int32), ("frames", c_int32), ("tap_row", c_int32 * 10), ("tap_a_col", c_int32 * 10),
+                ("tap_w_col", c_int32 * 10), ("bias", c_void_p), ("residual", c_void_p), ("ld_res", c_int32),
+                ("level", c_int32), ("C", c_int32), ("groups", c_int32), ("L", c_int32), ("eps", c_float),
+                ("y", c_void_p), ("ld_y", c_int32), ("gamma", c_void_p), ("beta", c_void_p), ("ada", c_void_p), ("ld_ada", c_int32),
+                ("res_f32", c_void_p), ("res_hi", c_void_p), ("res_lo", c_void_p), ("ld_res_gn", c_int32),
+                ("gn_out_hi", c_void_p), ("gn_out_lo", c_void_p), ("ld_gn_out", c_int32), ("gn_out_f32", c_void_p),
+                ("ld_gn_out_f32", c_int32), ("dout", c_void_p), ("dout_h", c_void_p), ("ld_dout", c_int32),
+                ("dout_add", c_void_p), ("ld_add", c_int32), ("dy", c_void_p), ("ld_dy", c_int32)]
+
+
+UNET_OP_HOOK = ctypes.CFUNCTYPE(None, c_int, c_int, c_int, POINTER(UnetOpInfo), c_void_p)
 
 
 class LibraryMissing(RuntimeError):
@@ -121,6 +142,8 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
     lib.cmdi_test_attention_bwd_at.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
     lib.cmdi_test_chain_layer.argtypes = [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_float, c_void_p]
     lib.cmdi_test_input_vjp.argtypes = [c_void_p, POINTER(ForwardArgs), c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.cmdi_test_unet_ops.argtypes = [c_void_p, POINTER(ForwardArgs), c_int, c_void_p, c_void_p, c_void_p, UNET_OP_HOOK, c_void_p,
+                                       c_void_p]
     _lib = lib
     return lib
 

@@ -2132,6 +2132,21 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
   return 0;
 }
 
+// A forward (cmdi_model_forward) or a guided forward and its input-VJP (cmdi_test_input_vjp) of an MDM_UNET engine with
+// `hook` called on the host around every op the passes enqueue, so that a test can read each op's inputs and output from
+// the engine's own buffers.
+extern "C" int cmdi_test_unet_ops(cmdi_engine* e, const cmdi_forward_args* a, int vjp, const float* inpainted_motion,
+                                  const uint8_t* inpainting_mask, float* out, cmdi_unet_op_hook hook, void* user, void* stream_) {
+  if (!e || !e->unet || !hook) {
+    set_last_error("cmdi_test_unet_ops: needs an MDM_UNET engine and a hook");
+    return 1;
+  }
+  e->unet->hook = hook; e->unet->hook_user = user;
+  const int rc = vjp ? cmdi_test_input_vjp(e, a, inpainted_motion, inpainting_mask, out, stream_) : cmdi_model_forward(e, a, out, stream_);
+  e->unet->hook = nullptr; e->unet->hook_user = nullptr;
+  return rc;
+}
+
 extern "C" int cmdi_recover_from_ric(const float* data, long long stride_seq, long long stride_frame, long long stride_feat,
                                      const float* mean, const float* std, int num_seqs, int nframes, int nfeats,
                                      int joints_num, int abs_3d, float* out, long long ostride_seq, long long ostride_frame,

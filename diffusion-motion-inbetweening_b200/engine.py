@@ -292,3 +292,36 @@ class Engine:
             capi.check(self.lib.cmdi_test_input_vjp(self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask),
                                                     grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_input_vjp")
         return grad
+
+    def test_unet_ops(self, hook, x, timestep, cond_emb=None, uncond=False, cfg=False, text_scale=None, obs_x0=None,
+                      obs_mask=None, inpainted_motion=None, inpainting_mask=None) -> torch.Tensor:
+        """MDM_UNET (cmdi_test_unet_ops): the forward Engine.forward runs, or with inpainted_motion / inpainting_mask the
+        guided forward and input-VJP Engine.test_input_vjp runs, calling hook(list, op, phase, info) on the host before
+        (phase 0) and after (phase 1) each op is enqueued on the current stream; info is a capi.UnetOpInfo.  Returns what
+        the wrapped call returns.  An exception the hook raises is re-raised after the call."""
+        dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
+        x = dev(x)
+        B = x.shape[0]
+        vjp = inpainted_motion is not None
+        cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
+        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
+        out = torch.empty(((2 if cfg else 1,) if vjp else ()) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        errors = []
+
+        def call(lst, op, phase, info, _user):
+            if errors:
+                return
+            try:
+                hook(lst, op, phase, info.contents)
+            except BaseException as ex:  # noqa: BLE001 (ctypes would swallow it)
+                errors.append(ex)
+
+        cb = capi.UNET_OP_HOOK(call)
+        a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
+                             _ptr(obs_x0), _ptr(obs_mask))
+        with torch.cuda.device(self.device):
+            capi.check(self.lib.cmdi_test_unet_ops(self._h, ctypes.byref(a), int(vjp), _ptr(inpainted_motion), _ptr(inpainting_mask),
+                                                   out.data_ptr(), cb, None, _stream_ptr(self.device)), "cmdi_test_unet_ops")
+        if errors:
+            raise errors[0]
+        return out

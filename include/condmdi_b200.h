@@ -260,6 +260,67 @@ CMDI_API int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B
  * (B, njoints, 1, nframes), the cond pass first (the sampler adds the two and masks them).  MDM_UNET: CMDI_PRECISION_FP16 only */
 CMDI_API int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
                         const uint8_t* inpainting_mask, float* grad, void* stream);
+
+/* One MDM_UNET op of a pass, as cmdi_test_unet_ops hands it to its callback.  Views are device pointers into the engine's
+ * own buffers, [rows, cols] with a row pitch; "level layout" is the halo layout of level l: nseq * (256 >> l) rows, the
+ * positions of sequence s at rows s * (256 >> l) + 2 + p.  Which planes a consumer reads (hi alone, hi + lo, one fp16
+ * plane, fp32) follows from the precision, nsplit and f16. */
+typedef struct cmdi_unet_op_info {
+  const char* name;         /* the state-dict prefix of the module the op implements; "^T": its input-VJP */
+  int kind;                 /* 0 GEMM, 1 GroupNorm->[AdaGN]->Mish->[+res], 2 input builder, 3 embedding builder,
+                               4 GroupNorm->AdaGN->Mish backward, 5 the input gradient (launch_unet_input_grad) */
+  int list_ops;             /* the number of ops of the list (list 2: its GEMMs and GroupNorms, then the input gradient) */
+  int num_seqs, f16;
+  /* kind 3: emb[s] = temb_table[t] + (s < n_cond_seqs ? cond_proj[s % B] : uncond_proj), or temb_table[t] alone when
+     cond_proj is null */
+  const float *temb_table, *cond_proj, *uncond_proj;
+  int n_cond_seqs;
+  /* GEMM: logical input / output views in the level layout of in_level / out_level (-1: one row per sequence, or for
+     rowmap 3 frame-major rows of the model output), weight planes [N_pad, K] (tap j at column tap_w_col[j]), epilogue */
+  int in_level, out_level;
+  const void *in_hi, *in_lo;
+  const float* in_f32;      /* kind 5: the fp32 input gradient in the level layout of level 0 */
+  int in_ld;
+  const void *out_hi, *out_lo;
+  int out_ld;
+  const float* out_f32;
+  int out_ld32;
+  const void *w_hi, *w_lo;
+  int w_ld, N, K, num_taps, k_per_tap, nsplit, nsplit_out, sum32, act, rowmap, frames;
+  int tap_row[10], tap_a_col[10], tap_w_col[10];
+  const float* bias;
+  const float* residual;
+  int ld_res;
+  /* GroupNorm (kinds 1, 4): level layout of `level` */
+  int level, C, groups, L;
+  float eps;
+  const void* y;            /* kind 1: fp32; kind 4: the fp16 stash plane */
+  int ld_y;
+  const float *gamma, *beta, *ada;
+  int ld_ada;
+  const float* res_f32;     /* kind 1 */
+  const void *res_hi, *res_lo;
+  int ld_res_gn;
+  const void *gn_out_hi, *gn_out_lo;
+  int ld_gn_out;
+  const float* gn_out_f32;
+  int ld_gn_out_f32;
+  const float* dout;        /* kind 4: fp32 (in / out when dout_add is set) ... */
+  const void* dout_h;       /* ... or fp16 */
+  int ld_dout;
+  const float* dout_add;
+  int ld_add;
+  const void* dy;           /* kind 4 output: fp16 */
+  int ld_dy;
+} cmdi_unet_op_info;
+/* list: 0 the forward pass, 1 the guided forward, 2 the input-VJP; op: index in the list, 0 .. list_ops - 1 (list 2: the
+ * last is the input gradient); phase 0: before the op is enqueued, 1: after.  Runs on the host; work it enqueues on the
+ * call's stream lands between the ops. */
+typedef void (*cmdi_unet_op_hook)(int list, int op, int phase, const cmdi_unet_op_info* info, void* user);
+/* test aid, MDM_UNET only: cmdi_model_forward (vjp = 0; out as there) or cmdi_test_input_vjp (vjp = 1; out receives grad,
+ * inpainted_motion / inpainting_mask as there) with `hook` called around every op of the passes it runs.  Device pointers. */
+CMDI_API int cmdi_test_unet_ops(cmdi_engine* e, const cmdi_forward_args* args, int vjp, const float* inpainted_motion,
+                                const uint8_t* inpainting_mask, float* out, cmdi_unet_op_hook hook, void* user, void* stream);
 /* backward pieces of reconstruction guidance (fp32 in / out) */
 CMDI_API int cmdi_test_layernorm_bwd(const float* dy, const float* v, const float* gamma, float* dv, int rows, void* stream);
 CMDI_API int cmdi_test_attention_bwd(const float* qkv, const float* dO, float* dqkv, int num_seqs, int S, int H, void* stream);
