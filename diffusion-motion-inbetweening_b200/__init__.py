@@ -5,7 +5,7 @@ as `condmdi_b200` through the shim package next to it.
 """
 from . import capi  # noqa: F401
 from .diffusion import (DiffusionConfig, GaussianDiffusion, ModelMeanType, ModelVarType, SpacedDiffusion,  # noqa: F401
-                        Window, create_gaussian_diffusion, from_reference_diffusion, get_named_beta_schedule, space_timesteps)
+                        JointSpace, Window, create_gaussian_diffusion, from_reference_diffusion, get_named_beta_schedule, space_timesteps)
 from .editing_util import get_gradient_schedule, get_keyframes_mask, joint_to_full_mask  # noqa: F401
 from .engine import Engine  # noqa: F401
 from .model import MDM, MDM_UNET, ClassifierFreeSampleModel, resolve_model  # noqa: F401

@@ -33,9 +33,15 @@ __device__ __forceinline__ float bf16_pair_to_f32(const __nv_bfloat16* hi, const
 // ---------------------------------------------------------------------------------------------
 // guidance seed on the frame-major layout [B*L (x2 when cfg), D_pad]
 // ---------------------------------------------------------------------------------------------
-template <bool F16>
+template <bool F16, bool JOINT>
 __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedParams p) {
   const size_t n = (size_t)p.B * p.L * p.D_pad;
+  float cr = 0.f, cj = 0.f;
+  if constexpr (JOINT) {
+    const int t = *p.step_ptr;
+    cr = p.seed_coef[2 * t];
+    cj = p.seed_coef[2 * t + 1];
+  }
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % p.D_pad);
     const int b = (int)(i / ((size_t)p.L * p.D_pad));
@@ -49,7 +55,8 @@ __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedPa
         hat = __fadd_rn(u, __fmul_rn(s, __fsub_rn(hat, u)));  // x0_hat = u + s (c - u)   (cfg_sampler.py:35)
       }
       const float m = p.obs_mask[i] ? 1.f : 0.f;
-      const float G = -2.f * (p.x_obs[i] - hat) * m;  // d/dx0_hat of ((x_obs - x0_hat)^2 * M)
+      float G = -2.f * (p.x_obs[i] - hat) * m;  // d/dx0_hat of ((x_obs - x0_hat)^2 * M)
+      if constexpr (JOINT) G = __fadd_rn(__fmul_rn(cr, G), __fmul_rn(cj, p.joint_grad[i]));
       gc = p.cfg ? s * G : G;
       gu = F16 ? __fsub_rn(G, __fmul_rn(G, s)) : (1.f - s) * G;
     }
@@ -69,6 +76,151 @@ __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedPa
       p.seed_hi[i + n] = h;
       if (p.seed_lo) p.seed_lo[i + n] = l;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// joint-position guidance seed (launch_joint_seed): recover_from_ric's forward and its VJP, one thread per frame
+// ---------------------------------------------------------------------------------------------
+// Inclusive prefix sum over the 256 threads of the block in thread order.  wsum: 8 floats of shared memory.
+__device__ __forceinline__ float block_scan_256(float v, float* wsum) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float u = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v = __fadd_rn(v, u);
+  }
+  if (lane == 31) wsum[w] = v;
+  __syncthreads();
+  if (w == 0) {
+    float t = lane < 8 ? wsum[lane] : 0.f;
+#pragma unroll
+    for (int o = 1; o < 8; o <<= 1) {
+      const float u = __shfl_up_sync(0xffffffffu, t, o);
+      if (lane >= o) t = __fadd_rn(t, u);
+    }
+    if (lane < 8) wsum[lane] = t;
+  }
+  __syncthreads();
+  if (w > 0) v = __fadd_rn(v, wsum[w - 1]);
+  __syncthreads();  // wsum may be reused
+  return v;
+}
+
+// qrot(qinv(q), (x, 0, z)) for q = (cos a, 0, sin a, 0) in qrot's operation order (recover_from_ric_kernel's), i.e. the
+// rotation by 2a about y: x' = C x - S z, z' = S x + C z with C = 1 - 2 sin^2 a, S = 2 sin a cos a
+__device__ __forceinline__ void rot_y(float c, float sn, float x, float z, float& xo, float& zo) {
+  const float qy = -sn;
+  const float uv0 = __fmul_rn(qy, z), uv2 = -__fmul_rn(qy, x);
+  const float uuv0 = __fmul_rn(qy, uv2), uuv2 = -__fmul_rn(qy, uv0);
+  xo = __fadd_rn(x, __fmul_rn(2.f, __fadd_rn(__fmul_rn(c, uv0), uuv0)));
+  zo = __fadd_rn(z, __fmul_rn(2.f, __fadd_rn(__fmul_rn(c, uv2), uuv2)));
+}
+
+__global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p) {
+  __shared__ float sa[256], sb[256], sc[256], wsum[8];
+  const int b = blockIdx.x, f = threadIdx.x, L = p.L;
+  const bool live = f < L;
+  const long long base = (long long)b * p.sb + (long long)f * p.sf;
+  const float s = p.x0_u ? p.text_scale[b] : 0.f;
+  // de-normalised feature c of this thread's frame, x0_hat formed as guidance_seed_kernel forms it
+  auto feat = [&](int c) -> float {
+    const long long o = base + (long long)c * p.sc;
+    float hat = p.x0[o];
+    if (p.x0_u) {
+      const float u = p.x0_u[o];
+      hat = __fadd_rn(u, __fmul_rn(s, __fsub_rn(hat, u)));
+    }
+    return __fadd_rn(__fmul_rn(hat, p.stdv[c]), p.mean[c]);
+  };
+  float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;
+  if (live) { d0 = feat(0); d1 = feat(1); d2 = feat(2); d3 = feat(3); }
+  // ---- forward: heading and root (recover_root_rot_pos) ----
+  float ang = d0, rx = d1, rz = d2, vx = 0.f, vz = 0.f, r_x = 0.f, r_z = 0.f;
+  if (!p.abs_3d) {
+    sa[f] = d0; sb[f] = d1; sc[f] = d2;
+    __syncthreads();
+    const bool prev = live && f >= 1;
+    ang = block_scan_256(prev ? sa[f - 1] : 0.f, wsum);  // exclusive prefix sum of the angular velocity
+    vx = prev ? sb[f - 1] : 0.f;
+    vz = prev ? sc[f - 1] : 0.f;
+    float c0, s0;
+    sincosf(ang, &s0, &c0);
+    rot_y(c0, s0, vx, vz, r_x, r_z);
+    rx = block_scan_256(r_x, wsum);                       // root x, z: inclusive prefix sums of the rotated velocity
+    rz = block_scan_256(r_z, wsum);
+  }
+  float sn, cs;
+  sincosf(ang, &sn, &cs);
+  const float C2 = __fsub_rn(1.f, __fmul_rn(2.f, __fmul_rn(sn, sn))), S2 = __fmul_rn(2.f, __fmul_rn(sn, cs));
+  // ---- joints: residuals, the gradients of the local coordinates, and the sums over joints ----
+  float g_ang = 0.f, g_rx = 0.f, g_rz = 0.f, g_ry = 0.f;
+  float* o = p.out + base;
+  if (live) {
+    const size_t jb = ((size_t)b * L + f) * 66;
+    const float* tg = p.target + jb;
+    const uint8_t* mk = p.mask + jb;
+    g_rx = mk[0] ? __fmul_rn(2.f, __fsub_rn(rx, tg[0])) : 0.f;
+    g_ry = mk[1] ? __fmul_rn(2.f, __fsub_rn(d3, tg[1])) : 0.f;
+    g_rz = mk[2] ? __fmul_rn(2.f, __fsub_rn(rz, tg[2])) : 0.f;
+    for (int j = 1; j < 22; ++j) {
+      const int c0 = 4 + 3 * (j - 1);
+      const float lx = feat(c0), ly = feat(c0 + 1), lz = feat(c0 + 2);
+      float xo, zo;
+      rot_y(cs, sn, lx, lz, xo, zo);
+      const float gx = mk[3 * j] ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(xo, rx), tg[3 * j])) : 0.f;
+      const float gy = mk[3 * j + 1] ? __fmul_rn(2.f, __fsub_rn(ly, tg[3 * j + 1])) : 0.f;
+      const float gz = mk[3 * j + 2] ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(zo, rz), tg[3 * j + 2])) : 0.f;
+      o[(long long)c0 * p.sc] = __fmul_rn(__fadd_rn(__fmul_rn(gx, C2), __fmul_rn(gz, S2)), p.stdv[c0]);
+      o[(long long)(c0 + 1) * p.sc] = __fmul_rn(gy, p.stdv[c0 + 1]);
+      o[(long long)(c0 + 2) * p.sc] = __fmul_rn(__fsub_rn(__fmul_rn(gz, C2), __fmul_rn(gx, S2)), p.stdv[c0 + 2]);
+      g_ang = __fadd_rn(g_ang, __fmul_rn(2.f, __fsub_rn(__fmul_rn(gz, xo), __fmul_rn(gx, zo))));
+      g_rx = __fadd_rn(g_rx, gx);
+      g_rz = __fadd_rn(g_rz, gz);
+    }
+  }
+  // ---- root and heading channels ----
+  float g0 = g_ang, g1 = g_rx, g2 = g_rz;
+  if (!p.abs_3d) {
+    // root_f = sum_{k <= f} r_k: dL/dr_k = sum_{f >= k} dL/droot_f, a suffix sum (thread t scans frame L - 1 - t)
+    __syncthreads();
+    sb[f] = g_rx; sc[f] = g_rz;
+    __syncthreads();
+    const int k = L - 1 - f;
+    const float Gx = block_scan_256(k >= 0 ? sb[k] : 0.f, wsum);
+    const float Gz = block_scan_256(k >= 0 ? sc[k] : 0.f, wsum);
+    if (k >= 0) { sb[k] = Gx; sc[k] = Gz; }
+    __syncthreads();
+    float G_x = 0.f, G_z = 0.f;
+    if (live) { G_x = sb[f]; G_z = sc[f]; }
+    __syncthreads();
+    // r_f = rot(ang_f) v_f, v_f = (d1, d2) of frame f - 1
+    sb[f] = __fadd_rn(__fmul_rn(G_x, C2), __fmul_rn(G_z, S2));
+    sc[f] = __fsub_rn(__fmul_rn(G_z, C2), __fmul_rn(G_x, S2));
+    sa[f] = __fadd_rn(g_ang, __fmul_rn(2.f, __fsub_rn(__fmul_rn(G_z, r_x), __fmul_rn(G_x, r_z))));
+    __syncthreads();
+    // ang_f = sum_{k < f} d0_k: dL/dd0_k = sum_{f > k} dL/dang_f, an exclusive suffix sum
+    const float ga = block_scan_256(k >= 0 && k + 1 < L ? sa[k + 1] : 0.f, wsum);
+    if (k >= 0) o = p.out + (long long)b * p.sb + (long long)k * p.sf;  // this thread now writes frame k's heading
+    g0 = ga;
+    g1 = live && f + 1 < L ? sb[f + 1] : 0.f;
+    g2 = live && f + 1 < L ? sc[f + 1] : 0.f;
+    if (k >= 0) o[0] = __fmul_rn(g0, p.stdv[0]);
+    o = p.out + base;
+  } else if (live) {
+    o[0] = __fmul_rn(g0, p.stdv[0]);
+  }
+  if (live) {
+    o[p.sc] = __fmul_rn(g1, p.stdv[1]);
+    o[2 * p.sc] = __fmul_rn(g2, p.stdv[2]);
+    o[3 * p.sc] = __fmul_rn(g_ry, p.stdv[3]);
+  }
+  // ---- exact zeros on channels 67 .. out_cols - 1 (row-contiguous for the frame-major layout) ----
+  const int nz = p.out_cols - kJointChannels;
+  float* ob = p.out + (long long)b * p.sb;
+  for (int i = threadIdx.x; i < L * nz; i += blockDim.x) {
+    const int ff = i / nz, c = kJointChannels + i % nz;
+    ob[(long long)ff * p.sf + (long long)c * p.sc] = 0.f;
   }
 }
 
@@ -163,8 +315,20 @@ cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t strea
   const size_t n = (size_t)p.B * p.L * p.D_pad;
   size_t grid = (n + 255) / 256;
   if (grid > 132 * 16) grid = 132 * 16;
-  if (p.f16) guidance_seed_kernel<true><<<(unsigned)grid, 256, 0, stream>>>(p);
-  else guidance_seed_kernel<false><<<(unsigned)grid, 256, 0, stream>>>(p);
+  if (p.joint_grad) {
+    if (p.f16) guidance_seed_kernel<true, true><<<(unsigned)grid, 256, 0, stream>>>(p);
+    else guidance_seed_kernel<false, true><<<(unsigned)grid, 256, 0, stream>>>(p);
+  } else {
+    if (p.f16) guidance_seed_kernel<true, false><<<(unsigned)grid, 256, 0, stream>>>(p);
+    else guidance_seed_kernel<false, false><<<(unsigned)grid, 256, 0, stream>>>(p);
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream) {
+  if (p.L < 1 || p.L > 256 || p.D < kJointChannels || p.out_cols < kJointChannels) return cudaErrorInvalidValue;
+  if (p.B == 0) return cudaSuccess;
+  joint_seed_kernel<<<p.B, 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

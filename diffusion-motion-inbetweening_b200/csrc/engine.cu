@@ -46,6 +46,7 @@ namespace {
 constexpr int kDModel = 512;
 constexpr int kBnWide = 256;    // QKV, FFN1
 constexpr int kBnNarrow = 128;  // N = 512 / 264 outputs: more tiles per wave
+constexpr int kMaxT = 5000;     // entries of the per-step coefficient tables (step indices and original timesteps)
 constexpr const char* kUnetGuidancePrecision =
     "reconstruction guidance (the denoiser's input-VJP) is implemented for the transformer denoiser and, at "
     "CMDI_PRECISION_FP16 (condmdi_b200.PRECISION_FP16), for MDM_UNET";
@@ -100,6 +101,8 @@ struct GraphKey {
   int variant, corrector;          // UniPC
   int jump_length, jump_n_sample;  // RePaint
   int win_K, win_N;                // overlapping windows (the first frames live in device memory)
+  int joint, joint_abs3d;          // joint-position guidance and its root representation (the joint seed's launch
+                                   // arguments); its targets and coefficients live in device memory
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -169,6 +172,17 @@ struct cmdi_engine {
   Planes seed_p;               // dL/d(model output rows), frame-major [2*frame_rows_pad, D_pad]
   float* guide_grad = nullptr; // dL/dz per pass, frame-major [2*frame_rows_pad, D_pad]
   float* guide_coef = nullptr; // [T] w_r[t] * sqrt(alpha_bar_t) / 2
+  // joint-position guidance (cmdi_sample_args.joint_guidance): the seed carries both coefficients and the step kernels
+  // read unit_coef instead of guide_coef
+  bool joint_on = false;       // the running call's guided evaluations add the joint seed
+  int joint_abs3d = 0;
+  float* joint_grad = nullptr;   // G_j frame-major [frame_rows_pad, D_pad]
+  float* joint_target = nullptr; // (maxB, L, 22, 3)
+  uint8_t* joint_mask = nullptr; // (maxB, L, 22, 3)
+  float* joint_stats = nullptr;  // mean [D], std [D]
+  float* seed_coef = nullptr;    // [kMaxT][2] (c_r, c_j) per step index
+  float* unit_coef = nullptr;    // [kMaxT] ones
+  std::vector<float> h_seed_coef;
   // forward path with LayerNorm folded into the consuming linear layers and the linear layers of a layer chained into one
   // persistent launch (gemm_chain.cu).  CMDI_CHAIN=0 selects the round-1 path (one launch per layer + LayerNorm kernels),
   // which guided steps (they stash LayerNorm inputs for the backward pass) always use.
@@ -319,6 +333,8 @@ int run_linear(cmdi_engine* e, const Planes& a, const Planes& w, const LinearPar
   CK(launch_linear_pair(a.map_hi, a.map_lo, w.pair_hi, w.pair_lo, p, block_n, e->num_sms, s, &st, f16));
   return 0;
 }
+
+void set_joint_seed(const cmdi_engine* e, GuidanceSeedParams* gp);
 
 }  // namespace
 #include "engine_unet.inc"
@@ -632,6 +648,51 @@ int ensure_stash(cmdi_engine* e, cudaStream_t s) {
   return 0;
 }
 
+// The joint term of the guidance seed while a joint-guided call runs (GuidanceSeedParams::joint_grad).
+void set_joint_seed(const cmdi_engine* e, GuidanceSeedParams* gp) {
+  if (!e->joint_on) return;
+  gp->joint_grad = e->joint_grad; gp->seed_coef = e->seed_coef; gp->step_ptr = e->step_ctr;
+}
+
+// G_j of the running evaluation's x0_hat (model_out, CFG-combined) into joint_grad.
+int run_joint_seed(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
+  JointSeedParams jp{};
+  jp.B = B; jp.L = e->L; jp.D = e->D; jp.x0 = e->model_out;
+  jp.x0_u = cfg ? e->model_out + (size_t)B * e->L * e->D_pad : nullptr; jp.text_scale = e->text_scale;
+  jp.sb = (long long)e->L * e->D_pad; jp.sf = e->D_pad; jp.sc = 1;
+  jp.target = e->joint_target; jp.mask = e->joint_mask; jp.mean = e->joint_stats; jp.stdv = e->joint_stats + e->D;
+  jp.abs_3d = e->joint_abs3d; jp.out = e->joint_grad; jp.out_cols = e->D_pad;
+  CK(launch_joint_seed(jp, s));
+  return 0;
+}
+
+// Buffers of joint-position guidance, allocated at its first use.
+int ensure_joint(cmdi_engine* e) {
+  if (e->joint_grad) return 0;
+  CKI(dev_alloc(e, &e->joint_grad, (size_t)e->frame_rows_pad * e->D_pad));
+  CKI(dev_alloc(e, &e->joint_target, (size_t)e->maxB * e->L * 66));
+  CKI(dev_alloc(e, &e->joint_mask, (size_t)e->maxB * e->L * 66));
+  CKI(dev_alloc(e, &e->joint_stats, (size_t)2 * e->D));
+  CKI(dev_alloc(e, &e->seed_coef, (size_t)2 * kMaxT));
+  CKI(dev_alloc(e, &e->unit_coef, (size_t)kMaxT));
+  const std::vector<float> ones(kMaxT, 1.f);
+  CK(cudaMemcpy(e->unit_coef, ones.data(), ones.size() * 4, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// Joint targets, mask and statistics of a call into the engine's buffers (the step graphs read them there).
+int stage_joint(cmdi_engine* e, int B, const float* target, const uint8_t* mask, const float* mean, const float* stdv,
+                int abs_3d, cudaStream_t s) {
+  CKI(ensure_joint(e));
+  const size_t n = (size_t)B * e->L * 66;
+  CK(cudaMemcpyAsync(e->joint_target, target, n * 4, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(e->joint_mask, mask, n, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(e->joint_stats, mean, (size_t)e->D * 4, cudaMemcpyDefault, s));
+  CK(cudaMemcpyAsync(e->joint_stats + e->D, stdv, (size_t)e->D * 4, cudaMemcpyDefault, s));
+  e->joint_abs3d = abs_3d != 0;
+  return 0;
+}
+
 // Backward pass of the (CFG-wrapped) denoiser w.r.t. its input, seeded with dL/dx0_hat of the reconstruction loss
 // (gaussian_diffusion.py:415-416).  Result: guide_grad[nseq * L, D_pad] (cond rows, then uncond rows under CFG).
 // Scratch: xseq / x1 (fp32 + planes) carry the running gradients; qkv_p / attn_p / ffh_p the per-layer ones.
@@ -643,6 +704,7 @@ int run_backward(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
   GuidanceSeedParams gp{};
   gp.B = B; gp.L = e->L; gp.D = e->D; gp.D_pad = e->D_pad; gp.cfg = cfg; gp.model_out = e->model_out;
   gp.text_scale = e->text_scale; gp.x_obs = e->x_obs; gp.obs_mask = e->obs_mask; gp.seed_hi = e->seed_p.hi; gp.seed_lo = e->seed_p.lo;
+  set_joint_seed(e, &gp);
   CK(launch_guidance_seed(gp, s));
   // output head backward: d(xseq) rows s >= 1; the token rows receive no gradient from the head
   CK(cudaMemsetAsync(e->xseq, 0, (size_t)M * kDModel * 4, s));
@@ -1456,7 +1518,7 @@ const char* field_to_unset(const cmdi_sample_args* a) {
 
 // Kernel launches of one evaluation of a sampling step: the denoiser pass, a guided one's backward pass, the step kernel.
 int launches_per_eval(const cmdi_engine* e, bool guided) {
-  return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) : 0);
+  return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) + (e->joint_on ? 1 : 0) : 0);
 }
 
 // What every sampler's step kernel reads and writes: the schedule, the device step counter, the combine inputs (model
@@ -1467,7 +1529,7 @@ StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool gui
   sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
   sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
   sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
-  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = e->guide_coef;
+  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance ? e->unit_coef : e->guide_coef;
   sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
   sp.pred_xstart = e->pred_x0;
   sp.win_K = a->window_count; sp.win_N = a->global_frames; sp.win_f0 = e->win_f0;
@@ -1496,6 +1558,8 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.variant = a->unipc_variant; key.corrector = a->unipc_corrector;
   key.jump_length = a->repaint_jump_length; key.jump_n_sample = a->repaint_jump_n_sample;
   key.win_K = a->window_count; key.win_N = a->global_frames;
+  key.joint = a->joint_guidance != 0;
+  key.joint_abs3d = key.joint && a->joint_abs3d != 0;
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
@@ -1603,7 +1667,8 @@ int check_windows(const cmdi_engine* e, const cmdi_sample_args* a) {
 
 }  // namespace
 
-extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
+namespace {
+int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
   if (!e || !a || !out) {
     set_last_error("null argument");
     return 1;
@@ -1708,6 +1773,36 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     CKI(ensure_stash(e, s));
     if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
     CK(cudaMemcpyAsync(e->guide_coef, a->recon_coef, (size_t)e->T * 4, cudaMemcpyHostToDevice, s));
+  }
+  e->joint_on = false;
+  const bool joint = a->joint_guidance != 0;
+  if (joint) {
+    if (!a->joint_coef || !a->joint_target || !a->joint_mask || !a->joint_mean || !a->joint_std) {
+      set_last_error("joint_guidance needs joint_coef, joint_target, joint_mask, joint_mean and joint_std");
+      return 1;
+    }
+    if (e->D != 263) {
+      set_last_error("joint-position guidance needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", e->D);
+      return 1;
+    }
+    if (a->window_count > 0) {
+      set_last_error("joint-position guidance does not run on overlapping windows (each window's root starts at its own origin)");
+      return 1;
+    }
+    if (e->unet && !e->f16) {
+      set_last_error(kUnetGuidancePrecision);
+      return 1;
+    }
+    CKI(ensure_stash(e, s));
+    CKI(stage_joint(e, B, a->joint_target, a->joint_mask, a->joint_mean, a->joint_std, a->joint_abs3d, s));
+    // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere
+    e->h_seed_coef.assign((size_t)2 * e->T, 0.f);
+    for (int t = 0; t < e->T; ++t) {
+      if (a->recon_guidance && t >= a->stop_recguidance_at) e->h_seed_coef[2 * t] = a->recon_coef[t];
+      if (t >= a->stop_jointguidance_at) e->h_seed_coef[2 * t + 1] = a->joint_coef[t];
+    }
+    CK(cudaMemcpyAsync(e->seed_coef, e->h_seed_coef.data(), e->h_seed_coef.size() * 4, cudaMemcpyHostToDevice, s));
+    e->joint_on = true;
   }
   if (a->skip_timesteps < 0 || a->skip_timesteps >= e->T) {
     set_last_error("skip_timesteps %d outside [0, %d)", a->skip_timesteps, e->T);
@@ -1853,6 +1948,10 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   CK(launch_ref_to_frames(xT, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
   e->launches += 1;
   // ---- keyframes ----
+  if (joint && !a->imputate && !a->recon_guidance) {  // no feature keyframes: M = 0
+    CK(cudaMemsetAsync(e->x_obs, 0, (size_t)B * e->L * e->D_pad * 4, s));
+    CK(cudaMemsetAsync(e->obs_mask, 0, (size_t)B * e->L * e->D_pad, s));
+  }
   if (a->imputate || a->recon_guidance) {
     const float* obs = (const float*)stage_in(a->inpainted_motion, e->ref_b, n * 4, host, s, &rc);
     const uint8_t* msk = (const uint8_t*)stage_in(a->inpainting_mask, e->ref_mask, n, host, s, &rc);
@@ -1886,6 +1985,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   // one evaluation: the denoiser pass and, for a guided one, its backward pass
   auto enqueue_eval = [&](cudaStream_t st, bool guided) -> int {
     CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
+    if (guided && joint) CKI(run_joint_seed(e, B, a->cfg != 0, st));
     if (guided) CKI(run_backward(e, B, a->cfg != 0, st));
     return 0;
   };
@@ -1946,8 +2046,12 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
     return 0;
   };
   int dump_i = 0;
-  // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch)
-  auto guided_at = [&](int k) { return a->recon_guidance && (rev ? t0 + k : t0 - k) >= a->stop_recguidance_at; };
+  // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch); a step
+  // is guided when reconstruction or joint guidance is active at it
+  auto guided_t = [&](int t) {
+    return (a->recon_guidance && t >= a->stop_recguidance_at) || (joint && t >= a->stop_jointguidance_at);
+  };
+  auto guided_at = [&](int k) { return guided_t(rev ? t0 + k : t0 - k); };
   // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
   // launch each; a denoise op is one evaluation and the step kernel, guided by its position, through the step graphs.
   // A graph holds one denoise op.
@@ -1961,7 +2065,7 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
       e->launches += 1;
       continue;
     }
-    const bool guided = a->recon_guidance && op.p >= a->stop_recguidance_at;
+    const bool guided = guided_t(op.p);
     const GraphKey key = step_graph_key(a, guided, 1, 0, false);
     if (step_uses_graph(a->use_graph, e->no_graph, nsteps, tape, e->graphs.count(key) != 0)) {
       cudaGraphExec_t exec = nullptr;
@@ -2051,6 +2155,15 @@ extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out
   return 0;
 }
 
+}  // namespace
+
+// The sampling loop (sample_call); the joint seed of a joint-guided call is never left on for a later call.
+extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
+  const int rc = sample_call(e, a, out, stream_);
+  if (e) e->joint_on = false;
+  return rc;
+}
+
 extern "C" int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B, const float* model_out_c,
                               const float* model_out_u, const float* text_scale, const float* x_t, const float* noise,
                               int impute, int stop_imputation_at, const float* x_obs, const uint8_t* mask, float* x_next,
@@ -2124,11 +2237,92 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, a->timestep, s));
   CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
+  e->joint_on = false;
   CKI(run_backward(e, B, a->cfg != 0, s));
   const size_t fr = (size_t)B * e->L * e->D_pad;
   for (int pass = 0; pass < (a->cfg ? 2 : 1); ++pass)
     CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
   e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 6;
+  return 0;
+}
+
+// cmdi_test_input_vjp with the joint term: the seed c_r G + c_j G_j, as a joint-guided sampling step at a step index
+// whose coefficients are (c_r, c_j) forms it.
+extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                         const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                         const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                         int joint_abs3d, float c_j, float* grad, void* stream_) {
+  if (!e || !a || !a->x || !grad || a->host_buffers || !joint_target || !joint_mask || !joint_mean || !joint_std ||
+      (!inpainted_motion) != (!inpainting_mask)) {
+    set_last_error("cmdi_test_joint_input_vjp: null argument or host buffers");
+    return 1;
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+  CK(cudaSetDevice(e->device));
+  const int B = a->batch;
+  CKI(check_ready(e, B, false));
+  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
+    set_last_error("cfg needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
+    return 1;
+  }
+  if (a->timestep < 0 || a->timestep >= kMaxT) {
+    set_last_error("timestep %d outside the positional table", a->timestep);
+    return 1;
+  }
+  if (e->unet && !e->f16) {
+    set_last_error(kUnetGuidancePrecision);
+    return 1;
+  }
+  if (e->D != 263) {
+    set_last_error("joint-position guidance needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", e->D);
+    return 1;
+  }
+  CKI(ensure_temb(e, s));
+  CKI(ensure_stash(e, s));
+  CKI(stage_joint(e, B, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, s));
+  const float coef[2] = {c_r, c_j};
+  CK(cudaMemcpy(e->seed_coef + 2 * a->timestep, coef, sizeof(coef), cudaMemcpyHostToDevice));
+  const size_t n = (size_t)B * e->D * e->L, fr = (size_t)B * e->L * e->D_pad;
+  CK(launch_ref_to_frames(a->x, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
+  if (inpainted_motion) {
+    CK(launch_ref_to_frames(inpainted_motion, B, e->D, e->L, e->D_pad, e->x_obs, nullptr, nullptr, s));
+    CK(launch_mask_to_frames(inpainting_mask, nullptr, B, e->D, e->L, e->D_pad, e->obs_mask, s));
+  } else {
+    CK(cudaMemsetAsync(e->x_obs, 0, fr * 4, s));
+    CK(cudaMemsetAsync(e->obs_mask, 0, fr, s));
+  }
+  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
+  CKI(prepare_cond(e, B, a->cond_emb, false, s));
+  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+  CK(launch_set_int(e->step_ctr, a->timestep, s));
+  CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
+  e->joint_on = true;
+  int rc = run_joint_seed(e, B, a->cfg != 0, s);
+  rc = rc || run_backward(e, B, a->cfg != 0, s);
+  e->joint_on = false;
+  if (rc) return 1;
+  for (int pass = 0; pass < (a->cfg ? 2 : 1); ++pass)
+    CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
+  e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 7;
+  return 0;
+}
+
+extern "C" int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,
+                                        const float* mean, const float* std, int abs_3d, float* grad, void* stream_) {
+  if (!x0 || !target || !mask || !mean || !std || !grad || B < 0 || D < kJointChannels || L < 1 || L > 256 ||
+      (ld != 0 && ld < D)) {
+    set_last_error("cmdi_joint_guidance_seed: bad arguments (need non-null pointers, D >= 67, 1 <= L <= 256, ld 0 or >= D)");
+    return 1;
+  }
+  JointSeedParams jp{};
+  jp.B = B; jp.L = L; jp.D = D; jp.x0 = x0;
+  if (ld) {  // frame-major rows of ld columns, the engine's layout
+    jp.sb = (long long)L * ld; jp.sf = ld; jp.sc = 1; jp.out_cols = ld;
+  } else {
+    jp.sb = (long long)D * L; jp.sf = 1; jp.sc = L; jp.out_cols = D;
+  }
+  jp.target = target; jp.mask = mask; jp.mean = mean; jp.stdv = std; jp.abs_3d = abs_3d != 0; jp.out = grad;
+  CK(launch_joint_seed(jp, reinterpret_cast<cudaStream_t>(stream_)));
   return 0;
 }
 

@@ -462,8 +462,35 @@ struct GuidanceSeedParams {
   // sequence q at row q * row_period + row_lo + l; other rows untouched), the seeds rounded to fp16 like autograd's cast
   // at the output's `.float()`; the uncond seed is G - s G, the sum autograd forms
   int f16, row_period, row_lo;
+  // joint-position guidance: with joint_grad set the seed is c_r G + c_j G_j, (c_r, c_j) = seed_coef[2 t], [2 t + 1] at the
+  // device step index t = step_ptr[0] (the step kernels then apply a coefficient of 1); null: the seed is G, unscaled
+  const float* joint_grad;   // [B*L, D_pad] G_j = dL_j/dx0_hat (launch_joint_seed)
+  const float* seed_coef;    // [T][2]
+  const int* step_ptr;
 };
 cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t stream);
+// Joint-position guidance seed: for the 22-joint HumanML3D skeleton, G_j = d/dx0_hat of
+//   sum(mask * (recover_from_ric(x0_hat * std + mean, 22, abs_3d) - target)^2)
+// with x0_hat = u + s[b] (c - u) under CFG (x0_u set) or x0.  One CTA per sequence, one thread per frame (L <= 256); the
+// relative representation's prefix sums over frames (heading, root) and their adjoint suffix sums are block scans.
+// Element (b, f, c) of x0 / x0_u / out at b * sb + f * sf + c * sc; out receives channels 0..66 and exact zeros on
+// channels 67 .. out_cols - 1.
+constexpr int kJointChannels = 67;  // 4 root channels + 21 x 3 rotation-invariant joint coordinates
+struct JointSeedParams {
+  int B, L, D;
+  const float* x0;
+  const float* x0_u;          // CFG: the uncond pass's output, or null
+  const float* text_scale;    // [B] (CFG)
+  long long sb, sf, sc;
+  const float* target;        // (B, L, 22, 3) fp32
+  const uint8_t* mask;        // (B, L, 22, 3) bool bytes
+  const float* mean;          // [D] (channels 0..66 read)
+  const float* stdv;
+  int abs_3d;
+  float* out;
+  int out_cols;
+};
+cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream);
 cudaError_t launch_layernorm512_bwd(const float* dy, const float* v, const float* gamma, float eps, int rows, float* dv,
                                     __nv_bfloat16* dv_hi, __nv_bfloat16* dv_lo, cudaStream_t stream);
 struct AttnBwdParams {

@@ -22,7 +22,8 @@ kernels in csrc/.
 
 Not accelerated (raise NotImplementedError, like the reference does for its own unsupported branches):
 cond_fn / 'gmd' classifier guidance, learned variances, EPSILON/PREVIOUS_X parametrisations,
-const_noise.  `reconstruction_guidance` runs a backward pass through the denoiser on the GPU (csrc/backward.cu).
+const_noise.  `reconstruction_guidance` runs a backward pass through the denoiser on the GPU (csrc/backward.cu), and
+`joint_guidance` (not in the reference) adds a loss on world-space joint positions to the same update (JointSpace).
 """
 from __future__ import annotations
 
@@ -115,6 +116,75 @@ class Window:
         return [min(k * (F - O), n - F) for k in range(K)]
 
 
+@dataclass(frozen=True)
+class JointSpace:
+    """How x0 maps to joint positions for joint-position guidance (`GaussianDiffusion.joint_space`): the (263,)
+    statistics of the dataset's inv_transform (cast to fp32) and its root representation (abs_3d: the absolute root of
+    the conditional checkpoints; False: the relative one).  With y['joint_guidance'] set, every guided step adds
+      L_j = sum(M_j * (recover_from_ric(x0^T * std + mean, 22, abs_3d) - joint_target)^2),  M_j = joint_target_mask & y['mask']
+    to reconstruction guidance's update with the coefficient w_j[t] * joint_guidance_weight * sqrt(alpha_bar_t) / 2
+    (w_j = get_gradient_schedule(y['joint_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_jointguidance_at'].
+    y['joint_target'] and y['joint_target_mask'] are (B, L, 22, 3), recover_from_ric's layout (a float and a bool tensor).
+    HumanML3D's 22-joint skeleton only; random-projection cards (inv_proj) are refused."""
+    mean: torch.Tensor = field(repr=False)
+    std: torch.Tensor = field(repr=False)
+    abs_3d: bool = True
+    inv_proj: Optional[torch.Tensor] = field(default=None, repr=False)
+
+    def __post_init__(self):
+        for name in ("mean", "std"):
+            v = torch.as_tensor(getattr(self, name)).detach().to(device="cpu", dtype=torch.float32).contiguous()
+            if v.dim() != 1:
+                raise ValueError(f"JointSpace {name} must be 1-D (the dataset's per-feature statistics), got {tuple(v.shape)}")
+            object.__setattr__(self, name, v)
+        if self.mean.shape != self.std.shape:
+            raise ValueError(f"JointSpace mean {tuple(self.mean.shape)} and std {tuple(self.std.shape)} differ in shape")
+        if not isinstance(self.abs_3d, (bool, np.bool_)):
+            raise ValueError(f"JointSpace abs_3d must be a bool, got {self.abs_3d!r}")
+        if self.inv_proj is not None:
+            raise NotImplementedError("joint guidance through a random projection (inv_proj) is not implemented")
+
+
+def _joint_guidance_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, window, device) -> dict:
+    """Engine arguments of y['joint_guidance'] (validated here, before any launch)."""
+    if space is None:
+        raise NotImplementedError("joint guidance needs diffusion.joint_space (a JointSpace: the dataset statistics and "
+                                  "abs_3d)")
+    if not isinstance(space, JointSpace):
+        raise TypeError(f"diffusion.joint_space must be a JointSpace or None, got {space!r}")
+    if D != 263 or space.mean.shape != (263,):
+        raise NotImplementedError(f"joint guidance is implemented for HumanML3D's 263 features (22 joints); the motion has "
+                                  f"{D} features and the statistics {tuple(space.mean.shape)}")
+    if window is not None:
+        raise NotImplementedError("joint guidance does not run on overlapping windows (diffusion.window)")
+    for k in ("joint_target", "joint_target_mask", "joint_guidance_weight", "stop_jointguidance_at", "diffusion_steps"):
+        if k not in y:
+            raise ValueError(f"joint guidance needs y[{k!r}]")
+    target, mask = y["joint_target"], y["joint_target_mask"]
+    if not isinstance(target, torch.Tensor) or not target.is_floating_point() or tuple(target.shape) != (B, L, 22, 3):
+        raise ValueError(f"y['joint_target'] must be a float tensor of shape {(B, L, 22, 3)}, got "
+                         f"{getattr(target, 'dtype', type(target))} {tuple(getattr(target, 'shape', ()))}")
+    if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or tuple(mask.shape) != (B, L, 22, 3):
+        raise ValueError(f"y['joint_target_mask'] must be a bool tensor of shape {(B, L, 22, 3)}, got "
+                         f"{getattr(mask, 'dtype', type(mask))} {tuple(getattr(mask, 'shape', ()))}")
+    weight, stop = y["joint_guidance_weight"], y["stop_jointguidance_at"]
+    if isinstance(weight, bool) or not isinstance(weight, (int, float, np.integer, np.floating)):
+        raise ValueError(f"y['joint_guidance_weight'] must be a number, got {weight!r}")
+    if isinstance(stop, bool) or not isinstance(stop, (int, np.integer)):
+        raise ValueError(f"y['stop_jointguidance_at'] must be an int, got {stop!r}")
+    mask = mask.to(device)
+    if y.get("mask") is not None:
+        mask = mask & y["mask"].to(device).reshape(B, L)[:, :, None, None].bool()
+    # w_j[t] * weight * sqrt(alpha_bar_t) / 2 in fp32, as reconstruction guidance forms its coefficient
+    ws = get_gradient_schedule(y.get("joint_gradient_schedule"), y["diffusion_steps"])
+    tt = torch.arange(num_timesteps)
+    w_j = torch.from_numpy(ws)[tt].float() * float(weight)
+    sab = torch.from_numpy(sqrt_alphas_cumprod)[tt].float()
+    return dict(joint_guidance=True, stop_jointguidance_at=int(stop), joint_coef=(w_j * sab / 2).float().numpy(),
+                joint_target=target.to(device=device, dtype=torch.float32), joint_mask=mask,
+                joint_mean=space.mean.to(device), joint_std=space.std.to(device), joint_abs3d=bool(space.abs_3d))
+
+
 def _crop_windows(x: torch.Tensor, f0: List[int], F: int) -> torch.Tensor:
     """(B, ..., N) in the global layout -> (B * K, ..., F): row b * K + k holds frames [f0[k], f0[k] + F) of sample b."""
     idx = torch.tensor(f0, device=x.device)[:, None] + torch.arange(F, device=x.device)
@@ -187,6 +257,8 @@ class GaussianDiffusion:
         # Window(frames, overlap): shapes (B, D, 1, N) of any length run as overlapping windows blended at every step;
         # None = one denoiser window per sequence
         self.window = None
+        # JointSpace: the statistics and root representation joint-position guidance (y['joint_guidance']) needs
+        self.joint_space = None
 
     # ------------------------------------------------------------------------------------------
     def q_sample(self, x_start, t, noise=None):
@@ -246,6 +318,10 @@ class GaussianDiffusion:
             f0 = f0 if len(f0) > 1 else None  # one window: the plain loop at N frames
         K, F = (len(f0), self.window.frames) if f0 else (1, int(shape[-1]))
         crop = (lambda t: None if t is None else _crop_windows(t, f0, F)) if f0 else (lambda t: t)
+        joint = {}
+        if y.get("joint_guidance", False):
+            joint = _joint_guidance_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
+                                         self.sqrt_alphas_cumprod, self.window, device)
         eng = inner.engine_for(device, max_batch=max(B * K, self.max_batch or 0), precision=self.precision, nframes=F)
         eng.set_schedule(self.betas, self.timestep_map)
 
@@ -351,7 +427,7 @@ class GaussianDiffusion:
                       obs_x0=kf_obs, obs_mask=kf_mask,
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
-                      recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **rng_args)
+                      recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **joint, **rng_args)
         if plms or dpm or sampler == capi.SAMPLER_DPM_SOLVER_SDE:
             common["plms_order" if plms else "dpm_order"] = int(order)
         if unipc:

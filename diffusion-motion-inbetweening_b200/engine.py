@@ -126,7 +126,10 @@ class Engine:
                obs_mask: Optional[torch.Tensor] = None, plms_order: int = 2, want_old_eps: bool = False,
                dpm_order: int = 2, unipc_order: int = 2, unipc_variant: int = capi.UNIPC_BH2, unipc_corrector: bool = True,
                repaint_jump_length: int = 10, repaint_jump_n_sample: int = 10,
-               window_frames0: Optional[Sequence[int]] = None, global_frames: int = 0, want_window_out: bool = False):
+               window_frames0: Optional[Sequence[int]] = None, global_frames: int = 0, want_window_out: bool = False,
+               joint_guidance: bool = False, stop_jointguidance_at: int = 0, joint_coef: Optional[Sequence[float]] = None,
+               joint_target: Optional[torch.Tensor] = None, joint_mask: Optional[torch.Tensor] = None,
+               joint_mean: Optional[torch.Tensor] = None, joint_std: Optional[torch.Tensor] = None, joint_abs3d: bool = False):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -151,6 +154,9 @@ class Engine:
         s * K + k is window k of global sample s and covers global frames [window_frames0[k], window_frames0[k] + nframes)
         of global_frames.  x_T, noise_tape and the outputs are global (batch // K, njoints, 1, global_frames); the other
         tensors are per window.  want_window_out adds result["windows"], the windows' final states.
+        joint_*: joint-position guidance (cmdi_sample_args.joint_guidance): joint_target (batch, nframes, 22, 3) fp32,
+        joint_mask of the same shape (y['mask'] folded in), joint_mean / joint_std (njoints,), joint_coef one entry per
+        sampler step.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         K = 0 if window_frames0 is None else len(window_frames0)
@@ -200,6 +206,15 @@ class Engine:
             if coef.shape != (self.num_timesteps,):
                 raise ValueError(f"recon_coef must have one entry per sampler step ({self.num_timesteps})")
             coef_arr = coef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+        jcoef_arr = None
+        if joint_guidance:
+            jcoef = np.ascontiguousarray(np.asarray(joint_coef, dtype=np.float32))
+            if jcoef.shape != (self.num_timesteps,):
+                raise ValueError(f"joint_coef must have one entry per sampler step ({self.num_timesteps})")
+            jcoef_arr = jcoef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+            joint_target = prep(joint_target, shp=(batch, self.nframes, 22, 3))
+            joint_mask = prep(joint_mask, torch.uint8, (batch, self.nframes, 22, 3))
+            joint_mean, joint_std = prep(joint_mean, shp=(self.njoints,)), prep(joint_std, shp=(self.njoints,))
         n_iter = self.num_timesteps - int(skip_timesteps)
         if num_steps:
             n_iter = min(n_iter, int(num_steps))
@@ -224,7 +239,9 @@ class Engine:
                             int(unipc_order) if unipc else 0, int(unipc_variant) if unipc else 0,
                             int(unipc_corrector) if unipc else 0,
                             int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0,
-                            K, f0_arr if K else None, int(global_frames), _ptr(windows))
+                            K, f0_arr if K else None, int(global_frames), _ptr(windows),
+                            int(joint_guidance), int(stop_jointguidance_at), jcoef_arr, _ptr(joint_target),
+                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
@@ -293,6 +310,30 @@ class Engine:
                                                     grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_input_vjp")
         return grad
 
+    def test_joint_input_vjp(self, x, timestep, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, c_j,
+                             inpainted_motion=None, inpainting_mask=None, c_r=0.0, cond_emb=None, uncond=False, cfg=False,
+                             text_scale=None, obs_x0=None, obs_mask=None) -> torch.Tensor:
+        """test_input_vjp of the joint-guided seed (cmdi_test_joint_input_vjp): the gradient of
+        c_r sum((inpainted_motion - x0_hat)^2 * inpainting_mask) + c_j sum(joint_mask * (P(x0_hat) - joint_target)^2)
+        w.r.t. x through each pass, (cfg ? 2 : 1, B, njoints, 1, nframes), cond pass first.  inpainted_motion None: the
+        joint term alone."""
+        dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
+        x = dev(x)
+        B = x.shape[0]
+        cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
+        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
+        joint_target, joint_mask = dev(joint_target), dev(joint_mask, torch.uint8)
+        joint_mean, joint_std = dev(joint_mean), dev(joint_std)
+        grad = torch.empty((2 if cfg else 1,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
+                             _ptr(obs_x0), _ptr(obs_mask))
+        with torch.cuda.device(self.device):
+            capi.check(self.lib.cmdi_test_joint_input_vjp(
+                self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask), float(c_r), _ptr(joint_target),
+                _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), float(c_j), grad.data_ptr(),
+                _stream_ptr(self.device)), "cmdi_test_joint_input_vjp")
+        return grad
+
     def test_unet_ops(self, hook, x, timestep, cond_emb=None, uncond=False, cfg=False, text_scale=None, obs_x0=None,
                       obs_mask=None, inpainted_motion=None, inpainting_mask=None) -> torch.Tensor:
         """MDM_UNET (cmdi_test_unet_ops): the forward Engine.forward runs, or with inpainted_motion / inpainting_mask the
@@ -325,3 +366,28 @@ class Engine:
         if errors:
             raise errors[0]
         return out
+
+
+def joint_guidance_seed(x0: torch.Tensor, target: torch.Tensor, mask: torch.Tensor, mean: torch.Tensor, std: torch.Tensor,
+                        abs_3d: bool, ld: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """cmdi_joint_guidance_seed: d/dx0 of sum(mask * (recover_from_ric(x0 * std + mean, 22, abs_3d) - target)^2) on a CUDA
+    device; target / mask (B, L, 22, 3); mean / std (D,).  ld = 0: x0 in the reference layout (B, D, 1, L); ld >= D: x0
+    frame-major (B, L, ld) with its first D columns the features (the engine's layout).  out: the result tensor (x0's
+    shape), or None for a new one."""
+    lib = capi.load()
+    dev = x0.device
+    if dev.type != "cuda":
+        raise RuntimeError("joint_guidance_seed runs on CUDA devices only (no CPU fallback)")
+    f = lambda t, dt=torch.float32: t.to(dev, dt).contiguous()  # noqa: E731
+    x0, target, mask, mean, std = f(x0), f(target), f(mask, torch.uint8), f(mean), f(std)
+    B, D = x0.shape[0], mean.shape[0]
+    L = x0.shape[1] if ld else x0.shape[-1]
+    want = (B, L, ld) if ld else (B, D, 1, L)
+    if tuple(x0.shape) != want or target.shape != (B, L, 22, 3) or mask.shape != (B, L, 22, 3) or std.shape != (D,):
+        raise ValueError("joint_guidance_seed: x0 must be (B, D, 1, L) (ld = 0) or (B, L, ld), target / mask (B, L, 22, 3) "
+                         "and mean / std (D,)")
+    grad = torch.empty_like(x0) if out is None else out
+    with torch.cuda.device(dev):
+        capi.check(lib.cmdi_joint_guidance_seed(_ptr(x0), B, D, L, int(ld), _ptr(target), _ptr(mask), _ptr(mean), _ptr(std),
+                                                int(abs_3d), grad.data_ptr(), _stream_ptr(dev)), "cmdi_joint_guidance_seed")
+    return grad

@@ -224,6 +224,24 @@ typedef struct {
   const int32_t* window_frames0; /* HOST array [K]: first global frame of each window */
   int32_t global_frames;        /* N */
   float* window_out;            /* test aid: NULL, or (batch, njoints, 1, F) the windows' final states (window layout) */
+  /* Joint-position guidance (all fields 0 / NULL: off): a second loss on world-space joint positions, on the same
+     reconstruction-guidance update.  At a guided step t
+       P(x0_hat) = recover_from_ric(x0_hat * joint_std + joint_mean, 22, joint_abs3d)      (B, L, 22, 3), fp32
+       L_j       = sum(joint_mask * (P - joint_target)^2)
+       x0_tilde  = x0_hat - ~M * (c_r(t) dL_r/dz + c_j(t) dL_j/dz)
+     with c_r(t) = recon_coef[t] while reconstruction guidance is on and t >= stop_recguidance_at (else 0), c_j(t) =
+     joint_coef[t] while t >= stop_jointguidance_at (else 0), and M = inpainting_mask AND y_mask (no keyframes: M = 0).
+     A step is guided when either coefficient applies.  Under CFG x0_hat is the combined output and the seed splits over
+     the passes as reconstruction guidance's does.  HumanML3D's 263 features only (njoints == 263); not on overlapping
+     windows; MDM_UNET at CMDI_PRECISION_FP16 only.  Pointers follow host_buffers like the fields above. */
+  int32_t joint_guidance;
+  int32_t stop_jointguidance_at;
+  const float* joint_coef;      /* HOST array [T]: w_j[t] * joint_guidance_weight * sqrt(alphas_cumprod[t]) / 2, fp32 */
+  const float* joint_target;    /* (B, L, 22, 3) fp32 world-space positions */
+  const uint8_t* joint_mask;    /* (B, L, 22, 3) bool bytes, y_mask already folded in */
+  const float* joint_mean;      /* (njoints) fp32 dataset statistics of the de-normalisation */
+  const float* joint_std;
+  int32_t joint_abs3d;          /* 1: absolute root representation (abs_3d), 0: relative */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
@@ -260,6 +278,20 @@ CMDI_API int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B
  * (B, njoints, 1, nframes), the cond pass first (the sampler adds the two and masks them).  MDM_UNET: CMDI_PRECISION_FP16 only */
 CMDI_API int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
                         const uint8_t* inpainting_mask, float* grad, void* stream);
+
+/* cmdi_test_input_vjp with joint-position guidance: grad receives the gradient of
+ * c_r sum((inpainted_motion - x0_hat)^2 * inpainting_mask) + c_j sum(joint_mask * (P(x0_hat) - joint_target)^2) through
+ * each pass (P as in cmdi_sample_args).  inpainted_motion / inpainting_mask may be NULL (no feature keyframes). */
+CMDI_API int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
+                                       const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                       const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                       int joint_abs3d, float c_j, float* grad, void* stream);
+/* The joint-position guidance seed alone: grad = d/dx0 sum(mask * (recover_from_ric(x0 * std + mean, 22, abs_3d) -
+ * target)^2), target (B, L, 22, 3) fp32, mask (B, L, 22, 3) bytes, mean / std [D].  x0 and grad in the ref layout
+ * (B, D, 1, L) when ld = 0, or frame-major [B * L, ld] (ld >= D, the engine's layout with ld = D_pad).  Channels >= 67 of
+ * grad (up to ld) are zero.  67 <= D, 1 <= L <= 256.  Device pointers. */
+CMDI_API int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,
+                                      const float* mean, const float* std, int abs_3d, float* grad, void* stream);
 
 /* One MDM_UNET op of a pass, as cmdi_test_unet_ops hands it to its callback.  Views are device pointers into the engine's
  * own buffers, [rows, cols] with a row pitch; "level layout" is the halo layout of level l: nseq * (256 >> l) rows, the
