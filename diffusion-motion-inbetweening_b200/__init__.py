@@ -8,7 +8,7 @@ from .diffusion import (DiffusionConfig, GaussianDiffusion, ModelMeanType, Model
                         JointSpace, Window, create_gaussian_diffusion, from_reference_diffusion, get_named_beta_schedule, space_timesteps)
 from .editing_util import get_gradient_schedule, get_keyframes_mask, joint_to_full_mask  # noqa: F401
 from .engine import Engine  # noqa: F401
-from .model import MDM, MDM_UNET, ClassifierFreeSampleModel, resolve_model  # noqa: F401
+from .model import MDM, MDM_UNET, ClassifierFreeSampleModel, KeyframeClassifierFreeSampleModel, resolve_model  # noqa: F401
 from .adapter import accelerate, install  # noqa: F401
 from .distributed import sharded_sample  # noqa: F401
 from .eval_loop import EvalJob, build_jobs, run_eval_jobs  # noqa: F401

@@ -50,7 +50,8 @@ class TensorDesc(Structure):
 
 class ForwardArgs(Structure):
     _fields_ = [("batch", c_int32), ("x", c_void_p), ("timestep", c_int32), ("cond_emb", c_void_p), ("uncond", c_int32),
-                ("cfg", c_int32), ("text_scale", c_void_p), ("host_buffers", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p)]
+                ("cfg", c_int32), ("text_scale", c_void_p), ("host_buffers", c_int32), ("obs_x0", c_void_p), ("obs_mask", c_void_p),
+                ("keyframe_scale", c_void_p)]
 
 
 class SampleArgs(Structure):
@@ -70,7 +71,7 @@ class SampleArgs(Structure):
                 ("window_out", c_void_p),
                 ("joint_guidance", c_int32), ("stop_jointguidance_at", c_int32), ("joint_coef", POINTER(c_float)),
                 ("joint_target", c_void_p), ("joint_mask", c_void_p), ("joint_mean", c_void_p), ("joint_std", c_void_p),
-                ("joint_abs3d", c_int32)]
+                ("joint_abs3d", c_int32), ("keyframe_scale", c_void_p)]
 
 
 class UnetOpInfo(Structure):

@@ -45,26 +45,41 @@ __global__ void __launch_bounds__(256) guidance_seed_kernel(const GuidanceSeedPa
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % p.D_pad);
     const int b = (int)(i / ((size_t)p.L * p.D_pad));
-    float gc = 0.f, gu = 0.f;
+    const bool kf = F16 && p.keyframe_scale;
+    float gc = 0.f, gu = 0.f, gn = 0.f;
     if (c < p.D) {
       float hat = p.model_out[i];
-      float s = 1.f;
+      float s = 1.f, w = 0.f;
       if (p.cfg) {
         const float u = p.model_out[i + n];
         s = p.text_scale[b];
-        hat = __fadd_rn(u, __fmul_rn(s, __fsub_rn(hat, u)));  // x0_hat = u + s (c - u)   (cfg_sampler.py:35)
+        if (kf) {
+          // x0_hat = (n + w_k (u - n)) + s (c - u)   (keyframe CFG)
+          const float nf = p.model_out[i + 2 * n];
+          w = p.keyframe_scale[b];
+          hat = __fadd_rn(__fadd_rn(nf, __fmul_rn(w, __fsub_rn(u, nf))), __fmul_rn(s, __fsub_rn(hat, u)));
+        } else {
+          hat = __fadd_rn(u, __fmul_rn(s, __fsub_rn(hat, u)));  // x0_hat = u + s (c - u)   (cfg_sampler.py:35)
+        }
       }
       const float m = p.obs_mask[i] ? 1.f : 0.f;
       float G = -2.f * (p.x_obs[i] - hat) * m;  // d/dx0_hat of ((x_obs - x0_hat)^2 * M)
       if constexpr (JOINT) G = __fadd_rn(__fmul_rn(cr, G), __fmul_rn(cj, p.joint_grad[i]));
       gc = p.cfg ? s * G : G;
-      gu = F16 ? __fsub_rn(G, __fmul_rn(G, s)) : (1.f - s) * G;
+      // the sums autograd forms: u receives w_k G from (u - n) and -(s G) from (c - u); n receives G and -(w_k G)
+      if (kf) {
+        gu = __fsub_rn(__fmul_rn(G, w), __fmul_rn(G, s));
+        gn = __fsub_rn(G, __fmul_rn(G, w));
+      } else {
+        gu = F16 ? __fsub_rn(G, __fmul_rn(G, s)) : (1.f - s) * G;
+      }
     }
     if constexpr (F16) {
       const int l = (int)((i / p.D_pad) % p.L);
       __half* seed = reinterpret_cast<__half*>(p.seed_hi);
       seed[((size_t)b * p.row_period + p.row_lo + l) * p.D_pad + c] = __float2half_rn(gc);
       if (p.cfg) seed[((size_t)(b + p.B) * p.row_period + p.row_lo + l) * p.D_pad + c] = __float2half_rn(gu);
+      if (kf) seed[((size_t)(b + 2 * p.B) * p.row_period + p.row_lo + l) * p.D_pad + c] = __float2half_rn(gn);
       continue;
     }
     __nv_bfloat16 h, l;
@@ -123,11 +138,15 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
   const bool live = f < L;
   const long long base = (long long)b * p.sb + (long long)f * p.sf;
   const float s = p.x0_u ? p.text_scale[b] : 0.f;
+  const float w = p.x0_n ? p.keyframe_scale[b] : 0.f;
   // de-normalised feature c of this thread's frame, x0_hat formed as guidance_seed_kernel forms it
   auto feat = [&](int c) -> float {
     const long long o = base + (long long)c * p.sc;
     float hat = p.x0[o];
-    if (p.x0_u) {
+    if (p.x0_n) {
+      const float u = p.x0_u[o], nf = p.x0_n[o];
+      hat = __fadd_rn(__fadd_rn(nf, __fmul_rn(w, __fsub_rn(u, nf))), __fmul_rn(s, __fsub_rn(hat, u)));
+    } else if (p.x0_u) {
       const float u = p.x0_u[o];
       hat = __fadd_rn(u, __fmul_rn(s, __fsub_rn(hat, u)));
     }

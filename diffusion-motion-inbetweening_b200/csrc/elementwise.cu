@@ -206,18 +206,21 @@ __global__ void fill_normal_ref_kernel(float* out, int B, size_t per_sample, uns
 
 // ---------------------------------------------------------------------------------------------
 // pred_xstart of one element (START_X, no clipping, :513-515): the model output (+ classifier-free guidance:
-// out_uncond + scale * (out - out_uncond), cfg_sampler.py:35), then reconstruction guidance or the imputation blend
+// out_uncond + scale * (out - out_uncond), cfg_sampler.py:35; or keyframe CFG: (n + w_k (u - n)) + scale * (c - u)),
+// then reconstruction guidance or the imputation blend
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float step_x0(float mo, float mu, float ob, unsigned char mk, float gg, float gu, int cfg, int guided,
-                                         bool do_impute, float text_scale, float guide_c) {
+__device__ __forceinline__ float step_x0(float mo, float mu, float mn, float ob, unsigned char mk, float gg, float gu, float gn, int cfg,
+                                         bool kf, int guided, bool do_impute, float text_scale, float kf_scale, float guide_c) {
   float out = mo;
-  if (cfg) out = __fadd_rn(mu, __fmul_rn(text_scale, __fsub_rn(out, mu)));
+  if (kf) out = __fadd_rn(__fadd_rn(mn, __fmul_rn(kf_scale, __fsub_rn(mu, mn))), __fmul_rn(text_scale, __fsub_rn(out, mu)));
+  else if (cfg) out = __fadd_rn(mu, __fmul_rn(text_scale, __fsub_rn(out, mu)));
   if (guided) {
     // reconstruction guidance (:416-425): cond_grad = grad * ~M ; tilde = hat - (w_r sqrt(abar) / 2) cond_grad ;
     // output = tilde * ~M + (imputing ? x_obs : hat) * M
     const float m = mk ? 1.0f : 0.0f;
     float g = gg;
     if (cfg) g = __fadd_rn(g, gu);
+    if (kf) g = __fadd_rn(g, gn);
     g = __fmul_rn(g, 1.0f - m);
     const float tilde = __fsub_rn(out, __fmul_rn(guide_c, g));
     out = __fadd_rn(__fmul_rn(tilde, 1.0f - m), __fmul_rn(do_impute ? ob : out, m));
@@ -231,33 +234,39 @@ __device__ __forceinline__ float step_x0(float mo, float mu, float ob, unsigned 
 
 // x0 (step_x0) of the 4 consecutive features at idx, the frame-major offset of feature c of a frame of row b, and
 // x_t there when xt is given.  Operands are read with 16-byte loads, each under the predicate that makes it meaningful:
-// an unguided, un-imputed step never touches x_obs / obs_mask / guide_grad, and only a CFG step reads the uncond half.
-// Padding features (c + j >= D) get x0 = 0.
+// an unguided, un-imputed step never touches x_obs / obs_mask / guide_grad, only a CFG step reads the uncond half and
+// only a keyframe-CFG step the keyframe-free third.  Padding features (c + j >= D) get x0 = 0.
 __device__ __forceinline__ void step_x0_at(const StepParams& p, size_t idx, int b, int c, bool do_impute, float guide_c,
                                            float x0[4], float* xt = nullptr) {
   const size_t uoff = (size_t)p.B * p.L * p.D_pad;  // uncond half of the batch-doubled pass
   const float text_scale = p.cfg ? p.text_scale[b] : 0.f;
+  const bool kf = p.keyframe_scale != nullptr;
+  const float kf_scale = kf ? p.keyframe_scale[b] : 0.f;
   const bool need_obs = p.guided || do_impute;
   const float4 mo4 = *reinterpret_cast<const float4*>(p.model_out + idx);
   const float4 mu4 = p.cfg ? *reinterpret_cast<const float4*>(p.model_out + idx + uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 mn4 = kf ? *reinterpret_cast<const float4*>(p.model_out + idx + 2 * uoff) : make_float4(0.f, 0.f, 0.f, 0.f);
   if (xt) {
     const float4 xt4 = *reinterpret_cast<const float4*>(p.x_t + idx);
     xt[0] = xt4.x; xt[1] = xt4.y; xt[2] = xt4.z; xt[3] = xt4.w;
   }
   const float4 ob4 = need_obs ? *reinterpret_cast<const float4*>(p.x_obs + idx) : make_float4(0.f, 0.f, 0.f, 0.f);
   const uchar4 mk4 = need_obs ? *reinterpret_cast<const uchar4*>(p.obs_mask + idx) : make_uchar4(0, 0, 0, 0);
-  float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4;
+  float4 gg4 = make_float4(0.f, 0.f, 0.f, 0.f), gu4 = gg4, gn4 = gg4;
   if (p.guided) {
     gg4 = *reinterpret_cast<const float4*>(p.guide_grad + idx);
     if (p.cfg) gu4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + uoff);
+    if (kf) gn4 = *reinterpret_cast<const float4*>(p.guide_grad + idx + 2 * uoff);
   }
-  const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w};
+  const float mo[4] = {mo4.x, mo4.y, mo4.z, mo4.w}, mu[4] = {mu4.x, mu4.y, mu4.z, mu4.w}, mn[4] = {mn4.x, mn4.y, mn4.z, mn4.w};
   const float ob[4] = {ob4.x, ob4.y, ob4.z, ob4.w};
   const unsigned char mk[4] = {mk4.x, mk4.y, mk4.z, mk4.w};
-  const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w};
+  const float gg[4] = {gg4.x, gg4.y, gg4.z, gg4.w}, gu[4] = {gu4.x, gu4.y, gu4.z, gu4.w}, gn[4] = {gn4.x, gn4.y, gn4.z, gn4.w};
 #pragma unroll
   for (int j = 0; j < 4; ++j)
-    x0[j] = c + j < p.D ? step_x0(mo[j], mu[j], ob[j], mk[j], gg[j], gu[j], p.cfg, p.guided, do_impute, text_scale, guide_c) : 0.f;
+    x0[j] = c + j < p.D ? step_x0(mo[j], mu[j], mn[j], ob[j], mk[j], gg[j], gu[j], gn[j], p.cfg, kf, p.guided, do_impute, text_scale,
+                                  kf_scale, guide_c)
+                        : 0.f;
 }
 
 // Overlapping windows: x0 of a global frame g that several windows cover becomes

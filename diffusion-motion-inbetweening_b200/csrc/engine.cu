@@ -103,7 +103,21 @@ struct GraphKey {
   int win_K, win_N;                // overlapping windows (the first frames live in device memory)
   int joint, joint_abs3d;          // joint-position guidance and its root representation (the joint seed's launch
                                    // arguments); its targets and coefficients live in device memory
+  int passes;                      // denoiser passes per evaluation (Passes::n): keyframe CFG adds one
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
+};
+
+// The passes of one evaluation, stacked along the batch: [0, B) the conditional pass; under CFG [B, 2B) the
+// unconditional one; under keyframe CFG (cmdi_*_args.keyframe_scale) last the keyframe-free pass n (unconditional
+// embedding, x_t unblended, mask channels 0).  Keyframe CFG without CFG is the two-pass combine n + w_k (c - n), CFG's
+// arithmetic with w_k for the scale, so the step, seed and joint kernels see it as CFG; with CFG it is the three-pass
+// combine (n + w_k (u - n)) + s (c - u).
+struct Passes {
+  int n = 1;
+  bool kf = false;                  // the last pass is keyframe-free
+  const float* scale = nullptr;     // the two-pass combine's scale (text_scale, or keyframe_scale without CFG), or null
+  const float* kf_scale = nullptr;  // the three-pass combine's w_k, or null
+  bool combine() const { return n > 1; }
 };
 
 // One op of a RePaint walk: denoise at p (the position moves p -> p - 1) or undo into p (p - 1 -> p).
@@ -157,6 +171,7 @@ struct cmdi_engine {
   CUtensorMap xseq_st{}, x1_st{};  // fp32 TMA-store targets: xseq (backward pass), x1 (v1 of the chained forward path)
   uint8_t* obs_mask = nullptr;
   float *cond_emb = nullptr, *cond_proj = nullptr, *text_scale = nullptr;
+  float* kf_scale = nullptr;  // [maxB] keyframe_scale of the running call (keyframe CFG)
   int* step_ctr = nullptr;  // [6]: step index, block-arrival counter, first step of the running history, of the call;
                             // RePaint: walk index of the call's first op, of the next op
   RngState* rng = nullptr;  // generator state of the running loop (device-resident: step graphs do not depend on it)
@@ -345,11 +360,12 @@ int prepare_chain(cmdi_engine* e, int nseq);
 int run_denoiser_chain(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool has_cond, const int* tmap_dev, cudaStream_t s,
                        std::vector<cudaEvent_t>* evs, int reps);
 
-// One denoiser pass over `nseq` sequences whose frame features are in x_state planes (first B sequences;
-// with dup the frame embedding is written for sequences [0,B) and [B,2B)).
-int run_denoiser(cmdi_engine* e, int B, bool dup, int n_cond_seqs, bool has_cond, const int* tmap_dev, cudaStream_t s,
+// One denoiser evaluation of ps.n passes over B sequences each, whose frame features are in x_state planes (first B
+// sequences; the transformer, one or two passes, writes the frame embedding for sequences [0,B) and [B,2B)).
+int run_denoiser(cmdi_engine* e, int B, const Passes& ps, int n_cond_seqs, bool has_cond, const int* tmap_dev, cudaStream_t s,
                  std::vector<cudaEvent_t>* evs = nullptr, int reps = 1, std::vector<LayerStash>* stash = nullptr) {
-  if (e->unet) return unet_run(e, e->unet, B, dup, n_cond_seqs, has_cond, tmap_dev, s, stash != nullptr);
+  if (e->unet) return unet_run(e, e->unet, B, ps.n, ps.kf, n_cond_seqs, has_cond, tmap_dev, s, stash != nullptr);
+  const bool dup = ps.n > 1;
   if (!stash && chain_eligible(e)) return run_denoiser_chain(e, B, dup, n_cond_seqs, has_cond, tmap_dev, s, evs, reps);
   auto mark = [&]() -> int {
     if (!evs) return 0;
@@ -655,10 +671,12 @@ void set_joint_seed(const cmdi_engine* e, GuidanceSeedParams* gp) {
 }
 
 // G_j of the running evaluation's x0_hat (model_out, CFG-combined) into joint_grad.
-int run_joint_seed(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
+int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
   JointSeedParams jp{};
+  const size_t fr = (size_t)B * e->L * e->D_pad;
   jp.B = B; jp.L = e->L; jp.D = e->D; jp.x0 = e->model_out;
-  jp.x0_u = cfg ? e->model_out + (size_t)B * e->L * e->D_pad : nullptr; jp.text_scale = e->text_scale;
+  jp.x0_u = ps.combine() ? e->model_out + fr : nullptr; jp.text_scale = ps.scale;
+  if (ps.kf_scale) { jp.x0_n = e->model_out + 2 * fr; jp.keyframe_scale = ps.kf_scale; }
   jp.sb = (long long)e->L * e->D_pad; jp.sf = e->D_pad; jp.sc = 1;
   jp.target = e->joint_target; jp.mask = e->joint_mask; jp.mean = e->joint_stats; jp.stdv = e->joint_stats + e->D;
   jp.abs_3d = e->joint_abs3d; jp.out = e->joint_grad; jp.out_cols = e->D_pad;
@@ -697,8 +715,9 @@ int stage_joint(cmdi_engine* e, int B, const float* target, const uint8_t* mask,
 // (gaussian_diffusion.py:415-416).  Result: guide_grad[nseq * L, D_pad] (cond rows, then uncond rows under CFG).
 // Scratch: xseq / x1 (fp32 + planes) carry the running gradients; qkv_p / attn_p / ffh_p the per-layer ones.
 constexpr int kBackwardLaunchesPerLayer = 8;  // the attention backward is two launches (dQ pass, dK/dV pass)
-int run_backward(cmdi_engine* e, int B, bool cfg, cudaStream_t s) {
-  if (e->unet) return unet_backward(e, e->unet, B, cfg, s);
+int run_backward(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
+  if (e->unet) return unet_backward(e, e->unet, B, ps, s);
+  const bool cfg = ps.combine();
   const int nseq = cfg ? 2 * B : B;
   const int M = nseq * e->S, MF = nseq * e->L;
   GuidanceSeedParams gp{};
@@ -779,6 +798,38 @@ int check_ready(cmdi_engine* e, int B, bool need_schedule) {
   }
   if (B < 1 || B > e->maxB) {
     set_last_error("batch %d outside [1, max_batch=%d]", B, e->maxB);
+    return 1;
+  }
+  return 0;
+}
+
+// The passes of an evaluation under CFG `cfg` and keyframe CFG `kf`; the scales are read from the engine's buffers.
+Passes passes_of(const cmdi_engine* e, bool cfg, bool kf) {
+  Passes ps;
+  ps.n = 1 + (cfg ? 1 : 0) + (kf ? 1 : 0);
+  ps.kf = kf;
+  ps.scale = cfg ? e->text_scale : kf ? e->kf_scale : nullptr;
+  ps.kf_scale = cfg && kf ? e->kf_scale : nullptr;
+  return ps;
+}
+
+// Keyframe CFG (a non-null keyframe_scale) needs a keyframe-conditioned MDM_UNET and its keyframes, and its passes must
+// fit the 2 * max_batch sequences the engine's buffers hold.
+int check_keyframe_cfg(const cmdi_engine* e, int B, bool cfg, const float* keyframe_scale, const void* obs_x0,
+                       const void* obs_mask) {
+  if (!keyframe_scale) return 0;
+  if (!e->unet || !e->unet->kf) {
+    set_last_error("keyframe_scale (keyframe CFG) needs a keyframe-conditioned MDM_UNET");
+    return 1;
+  }
+  if (!obs_x0 || !obs_mask) {
+    set_last_error("keyframe_scale (keyframe CFG) needs obs_x0 and obs_mask");
+    return 1;
+  }
+  const int passes = cfg ? 3 : 2;
+  if (passes * B > 2 * e->maxB) {
+    set_last_error("keyframe CFG runs %d passes of batch %d: %d sequences, more than the 2 * max_batch = %d the engine holds",
+                   passes, B, passes * B, 2 * e->maxB);
     return 1;
   }
   return 0;
@@ -929,6 +980,7 @@ extern "C" int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_en
   A(dev_alloc(e, &e->cond_emb, (size_t)e->maxB * 512));
   A(dev_alloc(e, &e->cond_proj, (size_t)e->maxB * kDModel));
   A(dev_alloc(e, &e->text_scale, e->maxB));
+  A(dev_alloc(e, &e->kf_scale, e->maxB));
   A(dev_alloc(e, &e->step_ctr, 6));
   A(dev_alloc(e, &e->rng, 1));
   // chained forward path: folded weights, partial row statistics, dependency counters
@@ -1267,10 +1319,12 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
     set_last_error("timestep %d outside the positional table", a->timestep);
     return 1;
   }
+  CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   const bool host = a->host_buffers != 0;
   const size_t n = (size_t)B * e->D * e->L;
   CKI(ensure_temb(e, s));
-  CKI(prepare_chain(e, a->cfg ? 2 * B : B));
+  CKI(prepare_chain(e, ps.n * B));
   int rc = 0;
   const float* x = (const float*)stage_in(a->x, e->ref_a, n * 4, host, s, &rc);
   if (rc) return 1;
@@ -1278,14 +1332,16 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
   CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, host, s));
   CKI(prepare_cond(e, B, a->cond_emb, host, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
+  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, a->timestep, s));
   const bool has_cond = a->cond_emb != nullptr;
   const int n_cond = a->uncond ? 0 : B;  // y['uncond'] under the CFG wrapper makes BOTH passes unconditional (cfg_sampler.py:28-33)
-  CKI(run_denoiser(e, B, a->cfg != 0, n_cond, has_cond, /*tmap*/ nullptr, s));
+  CKI(run_denoiser(e, B, ps, n_cond, has_cond, /*tmap*/ nullptr, s));
   // combine (cfg) into pred_x0 via the step kernel's pass-through mode, then back to the reference layout
   StepParams sp{};
   sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.advance = 0; sp.B = B; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
-  sp.sampler = 2; sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale; sp.x_t = e->x_state;
+  sp.sampler = 2; sp.model_out = e->model_out; sp.cfg = ps.combine(); sp.text_scale = ps.scale; sp.keyframe_scale = ps.kf_scale;
+  sp.x_t = e->x_state;
   sp.x_next = nullptr; sp.pred_xstart = e->pred_x0;
   CK(launch_diffusion_step(sp, s));
   float* dst = host ? e->ref_b : out;
@@ -1524,9 +1580,10 @@ int launches_per_eval(const cmdi_engine* e, bool guided) {
 // What every sampler's step kernel reads and writes: the schedule, the device step counter, the combine inputs (model
 // output, CFG scale, keyframes, guidance gradient) and the state it advances in place.
 StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool guided) {
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   StepParams sp{};
   sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.B = a->batch; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
-  sp.model_out = e->model_out; sp.cfg = a->cfg != 0; sp.text_scale = e->text_scale;
+  sp.model_out = e->model_out; sp.cfg = ps.combine(); sp.text_scale = ps.scale; sp.keyframe_scale = ps.kf_scale;
   sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
   sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
   sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance ? e->unit_coef : e->guide_coef;
@@ -1560,6 +1617,7 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.win_K = a->window_count; key.win_N = a->global_frames;
   key.joint = a->joint_guidance != 0;
   key.joint_abs3d = key.joint && a->joint_abs3d != 0;
+  key.passes = 1 + (a->cfg ? 1 : 0) + (a->keyframe_scale ? 1 : 0);
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
@@ -1757,6 +1815,8 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     set_last_error("cfg sampling needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
     return 1;
   }
+  CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   if ((a->imputate || a->recon_guidance) && (!a->inpainted_motion || !a->inpainting_mask)) {
     set_last_error("imputate / reconstruction_guidance need inpainted_motion and inpainting_mask (editing_util.py:330, :343)");
     return 1;
@@ -1898,7 +1958,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     nsteps = (a->num_steps > 0 && a->num_steps < left) ? a->num_steps : left;
   }
   CKI(ensure_temb(e, s));
-  CKI(prepare_chain(e, a->cfg ? 2 * B : B));
+  CKI(prepare_chain(e, ps.n * B));
   int rc = 0;
 
   // ---- x_T (gaussian_diffusion.py:1245-1248) ----
@@ -1965,6 +2025,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   // ---- conditioning ----
   CKI(prepare_cond(e, B, a->cond_emb, host, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
+  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, t0, s));
   // [2]: the history's first step (the call's for the single-step samplers), [3]: the call's first step, from which the
   // per-step draws of SDE-DPM-Solver++ are numbered (they differ on a resume)
@@ -1984,9 +2045,9 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   const bool has_cond = a->cond_emb != nullptr;
   // one evaluation: the denoiser pass and, for a guided one, its backward pass
   auto enqueue_eval = [&](cudaStream_t st, bool guided) -> int {
-    CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
-    if (guided && joint) CKI(run_joint_seed(e, B, a->cfg != 0, st));
-    if (guided) CKI(run_backward(e, B, a->cfg != 0, st));
+    CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
+    if (guided && joint) CKI(run_joint_seed(e, B, ps, st));
+    if (guided) CKI(run_backward(e, B, ps, st));
     return 0;
   };
   // RePaint's two ops; the walk position and the draw number live in step_ctr
@@ -2226,6 +2287,8 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
     set_last_error(kUnetGuidancePrecision);
     return 1;
   }
+  CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   CKI(ensure_temb(e, s));
   CKI(ensure_stash(e, s));
   const size_t n = (size_t)B * e->D * e->L;
@@ -2235,12 +2298,13 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
   CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
   CKI(prepare_cond(e, B, a->cond_emb, false, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, a->timestep, s));
-  CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
+  CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
   e->joint_on = false;
-  CKI(run_backward(e, B, a->cfg != 0, s));
+  CKI(run_backward(e, B, ps, s));
   const size_t fr = (size_t)B * e->L * e->D_pad;
-  for (int pass = 0; pass < (a->cfg ? 2 : 1); ++pass)
+  for (int pass = 0; pass < ps.n; ++pass)
     CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
   e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 6;
   return 0;
@@ -2277,6 +2341,8 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
     set_last_error("joint-position guidance needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", e->D);
     return 1;
   }
+  CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   CKI(ensure_temb(e, s));
   CKI(ensure_stash(e, s));
   CKI(stage_joint(e, B, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, s));
@@ -2294,14 +2360,15 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
   CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
   CKI(prepare_cond(e, B, a->cond_emb, false, s));
   if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
+  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, a->timestep, s));
-  CKI(run_denoiser(e, B, a->cfg != 0, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
+  CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
   e->joint_on = true;
-  int rc = run_joint_seed(e, B, a->cfg != 0, s);
-  rc = rc || run_backward(e, B, a->cfg != 0, s);
+  int rc = run_joint_seed(e, B, ps, s);
+  rc = rc || run_backward(e, B, ps, s);
   e->joint_on = false;
   if (rc) return 1;
-  for (int pass = 0; pass < (a->cfg ? 2 : 1); ++pass)
+  for (int pass = 0; pass < ps.n; ++pass)
     CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
   e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 7;
   return 0;
@@ -2383,7 +2450,7 @@ extern "C" int cmdi_profile_pass(cmdi_engine* e, int batch, int cfg, int repeats
   }
   if (repeats < 1) repeats = 1;
   CKI(prepare_chain(e, cfg ? 2 * batch : batch));
-  const int rc = run_denoiser(e, batch, cfg != 0, batch, has_cond, nullptr, s, &evs, repeats);
+  const int rc = run_denoiser(e, batch, passes_of(e, cfg != 0, false), batch, has_cond, nullptr, s, &evs, repeats);
   cudaError_t se = cudaStreamSynchronize(s);
   int n = (int)evs.size() - 1;
   if (rc == 0 && se == cudaSuccess) {

@@ -214,6 +214,9 @@ struct StepParams {
   const float* model_out;   // [B*L (x2 when cfg), D_pad] raw denoiser output(s); uncond half at +B*L rows
   int cfg;                  // 1: out = u + s[b]*(c - u)
   const float* text_scale;  // [B]
+  // keyframe CFG over three passes (cfg must be 1): the keyframe-free pass n at +2*B*L rows of model_out (and of
+  // guide_grad), out = (n + w_k[b] (u - n)) + s[b] (c - u), and a guided step sums the three pass gradients; null: off
+  const float* keyframe_scale;  // [B]
   const float* x_t;         // [B*L, D_pad]
   // imputation (gaussian_diffusion.py:427-435): applied when impute != 0 and t >= stop_imputation_at
   int impute;
@@ -355,7 +358,8 @@ struct UnetInputParams {
   const float* x_t;
   const float* obs;            // observed keyframes (null: not keyframe-conditioned)
   const uint8_t* obs_mask;
-  int copies;                  // 2 under CFG: sequences b and b + B receive the same input
+  int copies;                  // passes: sequence b + k * B of copy k receives the input of sample b
+  int kf_free;                 // 1: the last copy is keyframe CFG's keyframe-free pass: x_t unblended, mask channels 0
   int row_period, row_lo;      // halo layout of the destination
   int ld;                      // destination row pitch (elements, even)
   __nv_bfloat16* out_hi;
@@ -443,9 +447,10 @@ struct DgradWeightParams {
 };
 cudaError_t launch_dgrad_weight_planes(const DgradWeightParams& p, cudaStream_t stream);
 // guide_grad[(seq*L + l), c] = xg[seq*row_period + row_lo + l, c] * !obs_mask[(seq % B)*L + l, c] for c < D (0 for
-// D <= c < D_pad; obs_mask null: no keyframe input blend): the gradient of the network input's x_t channels
-cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int B, int L, int D, int D_pad, int row_period, int row_lo,
-                                   const uint8_t* obs_mask, float* out, cudaStream_t stream);
+// D <= c < D_pad; obs_mask null: no keyframe input blend): the gradient of the network input's x_t channels.  Sequences
+// seq >= kf_seqs (keyframe CFG's keyframe-free pass) have no blend: their gradient passes unmasked.
+cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int kf_seqs, int B, int L, int D, int D_pad, int row_period,
+                                   int row_lo, const uint8_t* obs_mask, float* out, cudaStream_t stream);
 
 // ----------------------------------------------------------------------------------------------
 // backward pieces for reconstruction guidance      (backward.cu)
@@ -467,6 +472,9 @@ struct GuidanceSeedParams {
   const float* joint_grad;   // [B*L, D_pad] G_j = dL_j/dx0_hat (launch_joint_seed)
   const float* seed_coef;    // [T][2]
   const int* step_ptr;
+  // keyframe CFG over three passes (f16 only; cfg must be 1): x0_hat = (n + w_k (u - n)) + s (c - u) with n at +2*B*L
+  // rows of model_out, and seeds (s G, w_k G - s G, G - w_k G) to the rows of sequences b, b + B, b + 2B; null: off
+  const float* keyframe_scale;  // [B]
 };
 cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t stream);
 // Joint-position guidance seed: for the 22-joint HumanML3D skeleton, G_j = d/dx0_hat of
@@ -481,6 +489,8 @@ struct JointSeedParams {
   const float* x0;
   const float* x0_u;          // CFG: the uncond pass's output, or null
   const float* text_scale;    // [B] (CFG)
+  const float* x0_n;          // keyframe CFG over three passes: the keyframe-free pass's output, x0_hat =
+  const float* keyframe_scale; // (n + w_k (u - n)) + s (c - u), [B]; both null: off
   long long sb, sf, sc;
   const float* target;        // (B, L, 22, 3) fp32
   const uint8_t* mask;        // (B, L, 22, 3) bool bytes

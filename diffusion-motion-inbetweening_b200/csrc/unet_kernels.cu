@@ -24,7 +24,8 @@ __device__ __forceinline__ float mish_dev(float x) { return x * tanhf(x > 20.0f 
 
 // ---------------------------------------------------------------------------------------------
 // network input: planes [rows0, ld] (hi, lo), channels [0, D) = keyframe-blended x_t, [D, 2D) = mask (keyframe-
-// conditioned models), zero elsewhere.  One thread per (sequence copy, frame, channel pair).
+// conditioned models), zero elsewhere.  One thread per (sample, frame, channel pair), storing every copy; keyframe CFG's
+// keyframe-free copy (kf_free, the last) receives x_t unblended and zero mask channels, the input of obs_mask = 0.
 // ---------------------------------------------------------------------------------------------
 template <bool F16>
 __global__ void __launch_bounds__(256) unet_input_kernel(const UnetInputParams p) {
@@ -34,25 +35,30 @@ __global__ void __launch_bounds__(256) unet_input_kernel(const UnetInputParams p
     const int cp = (int)(i % pairs);
     const size_t fl = i / pairs;
     const int l = (int)(fl % p.L), b = (int)(fl / p.L);
-    float v[2];
+    float v[2], vf[2];
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int c = cp * 2 + j;
-      float val = 0.f;
+      float val = 0.f, free = 0.f;
       const size_t src = ((size_t)b * p.L + l) * p.D_pad;
       if (c < p.D) {
-        val = p.x_t[src + c];
+        val = free = p.x_t[src + c];
         if (p.obs_mask && p.obs_mask[src + c]) val = p.obs[src + c];
       } else if (p.obs_mask && c < 2 * p.D) {
         val = p.obs_mask[src + c - p.D] ? 1.0f : 0.0f;
       }
       v[j] = val;
+      vf[j] = free;
     }
     uint32_t hw, lw = 0;
     if constexpr (F16) hw = pack_f16x2(v[0], v[1]);  // the blend is fp32; the first conv casts its input to fp16
     else split_bf16x2(v[0], v[1], hw, lw);
     for (int copy = 0; copy < p.copies; ++copy) {
       const size_t row = (size_t)(b + copy * p.B) * p.row_period + p.row_lo + l;
+      if (p.kf_free && copy == p.copies - 1) {
+        if constexpr (F16) hw = pack_f16x2(vf[0], vf[1]);
+        else split_bf16x2(vf[0], vf[1], hw, lw);
+      }
       *reinterpret_cast<uint32_t*>(p.out_hi + row * p.ld + cp * 2) = hw;
       if (!F16 && p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + row * p.ld + cp * 2) = lw;
     }
@@ -405,9 +411,9 @@ __global__ void dgrad_weight_planes_kernel(const DgradWeightParams p) {
   }
 }
 
-__global__ void __launch_bounds__(256) unet_input_grad_kernel(const float* __restrict__ xg, int ld, int num_seqs, int B, int L, int D,
-                                                              int D_pad, int row_period, int row_lo, const uint8_t* __restrict__ obs_mask,
-                                                              float* __restrict__ out) {
+__global__ void __launch_bounds__(256) unet_input_grad_kernel(const float* __restrict__ xg, int ld, int num_seqs, int kf_seqs, int B,
+                                                              int L, int D, int D_pad, int row_period, int row_lo,
+                                                              const uint8_t* __restrict__ obs_mask, float* __restrict__ out) {
   const size_t total = (size_t)num_seqs * L * D_pad;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % D_pad);
@@ -416,7 +422,7 @@ __global__ void __launch_bounds__(256) unet_input_grad_kernel(const float* __res
     float v = 0.f;
     if (c < D) {
       v = xg[((size_t)q * row_period + row_lo + l) * ld + c];
-      if (obs_mask && obs_mask[((size_t)(q % B) * L + l) * D_pad + c]) v = 0.f;  // x = obs_x0 M + x ~M (mdm_unet.py:781)
+      if (obs_mask && q < kf_seqs && obs_mask[((size_t)(q % B) * L + l) * D_pad + c]) v = 0.f;  // x = obs_x0 M + x ~M (mdm_unet.py:781)
     }
     out[i] = v;
   }
@@ -501,10 +507,10 @@ cudaError_t launch_dgrad_weight_planes(const DgradWeightParams& p, cudaStream_t 
   return cudaGetLastError();
 }
 
-cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int B, int L, int D, int D_pad, int row_period, int row_lo,
-                                   const uint8_t* obs_mask, float* out, cudaStream_t stream) {
-  unet_input_grad_kernel<<<grid_1d((size_t)num_seqs * L * D_pad, 256), 256, 0, stream>>>(xg, ld, num_seqs, B, L, D, D_pad, row_period,
-                                                                                        row_lo, obs_mask, out);
+cudaError_t launch_unet_input_grad(const float* xg, int ld, int num_seqs, int kf_seqs, int B, int L, int D, int D_pad, int row_period,
+                                   int row_lo, const uint8_t* obs_mask, float* out, cudaStream_t stream) {
+  unet_input_grad_kernel<<<grid_1d((size_t)num_seqs * L * D_pad, 256), 256, 0, stream>>>(xg, ld, num_seqs, kf_seqs, B, L, D, D_pad,
+                                                                                        row_period, row_lo, obs_mask, out);
   return cudaGetLastError();
 }
 

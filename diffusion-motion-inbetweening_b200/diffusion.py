@@ -39,7 +39,7 @@ import torch
 
 from . import capi
 from .editing_util import get_gradient_schedule
-from .model import resolve_model
+from .model import check_keyframe_cfg_scales, is_keyframe_cfg, keyframe_cfg_max_batch, resolve_model
 
 
 def get_named_beta_schedule(schedule_name, num_diffusion_timesteps, scale_betas=1.):
@@ -303,6 +303,7 @@ class GaussianDiffusion:
             raise NotImplementedError("cond_fn (condition_score_with_grad) is out of scope")
         assert isinstance(shape, (tuple, list))
         inner, is_cfg = resolve_model(model)
+        kf_cfg = is_keyframe_cfg(model)
         if device is None:
             device = next(model.parameters()).device
         device = torch.device(device)
@@ -322,7 +323,8 @@ class GaussianDiffusion:
         if y.get("joint_guidance", False):
             joint = _joint_guidance_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
                                          self.sqrt_alphas_cumprod, self.window, device)
-        eng = inner.engine_for(device, max_batch=max(B * K, self.max_batch or 0), precision=self.precision, nframes=F)
+        rows = keyframe_cfg_max_batch(B * K, is_cfg) if kf_cfg else B * K  # keyframe CFG: its passes fit 2 * max_batch
+        eng = inner.engine_for(device, max_batch=max(rows, self.max_batch or 0), precision=self.precision, nframes=F)
         eng.set_schedule(self.betas, self.timestep_map)
 
         # ---- conditioning ----
@@ -334,9 +336,14 @@ class GaussianDiffusion:
             # with a window set, y['text'] may hold one prompt per window, also when one window covers the motion
             text = _window_prompts(y["text"], B, K) if self.window is not None else y["text"]
             cond_emb = inner.encode_text(text).to(device=device, dtype=torch.float32)  # once per loop (mdm.py:249 does it per step)
+        if kf_cfg:
+            check_keyframe_cfg_scales(y, is_cfg)
         if is_cfg:
             assert cond_mode in ["text", "action"]  # cfg_sampler.py:27
             text_scale = y["text_scale"].to(device=device, dtype=torch.float32).reshape(-1).repeat_interleave(K)
+        keyframe_scale = None
+        if kf_cfg:
+            keyframe_scale = y["keyframe_scale"].to(device=device, dtype=torch.float32).reshape(-1).repeat_interleave(K)
         # ---- keyframe imputation (gaussian_diffusion.py:427-442, editing_util.py:336-346) ----
         imputate, stop_at, obs, mask, y_mask = False, 0, None, None, None
         guided_cfg = bool(y.get("reconstruction_guidance", False))
@@ -424,7 +431,7 @@ class GaussianDiffusion:
             kf_obs = crop(model_kwargs["obs_x0"].to(device=device, dtype=torch.float32))
             kf_mask = crop(model_kwargs["obs_mask"].to(device=device))
         common = dict(batch=B * K, sampler=sampler, eta=eta, cond_emb=cond_emb, uncond=uncond, cfg=is_cfg, text_scale=text_scale,
-                      obs_x0=kf_obs, obs_mask=kf_mask,
+                      obs_x0=kf_obs, obs_mask=kf_mask, keyframe_scale=keyframe_scale,
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
                       recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **joint, **rng_args)

@@ -88,8 +88,9 @@ class Engine:
     # ------------------------------------------------------------------------------------------
     def forward(self, x: torch.Tensor, timestep: int, cond_emb: Optional[torch.Tensor] = None, uncond: bool = False,
                 cfg: bool = False, text_scale: Optional[torch.Tensor] = None, obs_x0: Optional[torch.Tensor] = None,
-                obs_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """MDM.forward / ClassifierFreeSampleModel.forward for a batch sharing one (original) timestep."""
+                obs_mask: Optional[torch.Tensor] = None, keyframe_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """MDM.forward / ClassifierFreeSampleModel.forward for a batch sharing one (original) timestep; keyframe_scale
+        (B,): keyframe classifier-free guidance (cmdi_forward_args.keyframe_scale)."""
         host = not x.is_cuda
         x = x.to(torch.float32).contiguous()
         B = x.shape[0]
@@ -101,12 +102,12 @@ class Engine:
             t = t.to(torch.float32).contiguous()
             return t.cpu() if host else t.to(self.device)
 
-        cond_emb, text_scale, obs_x0 = prep(cond_emb), prep(text_scale), prep(obs_x0)
+        cond_emb, text_scale, obs_x0, keyframe_scale = prep(cond_emb), prep(text_scale), prep(obs_x0), prep(keyframe_scale)
         if obs_mask is not None:
             obs_mask = obs_mask.to(torch.uint8).contiguous()
             obs_mask = obs_mask.cpu() if host else obs_mask.to(self.device)
         a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), int(host),
-                             _ptr(obs_x0), _ptr(obs_mask))
+                             _ptr(obs_x0), _ptr(obs_mask), _ptr(keyframe_scale))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_model_forward(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_model_forward")
@@ -129,7 +130,8 @@ class Engine:
                window_frames0: Optional[Sequence[int]] = None, global_frames: int = 0, want_window_out: bool = False,
                joint_guidance: bool = False, stop_jointguidance_at: int = 0, joint_coef: Optional[Sequence[float]] = None,
                joint_target: Optional[torch.Tensor] = None, joint_mask: Optional[torch.Tensor] = None,
-               joint_mean: Optional[torch.Tensor] = None, joint_std: Optional[torch.Tensor] = None, joint_abs3d: bool = False):
+               joint_mean: Optional[torch.Tensor] = None, joint_std: Optional[torch.Tensor] = None, joint_abs3d: bool = False,
+               keyframe_scale: Optional[torch.Tensor] = None):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -157,6 +159,8 @@ class Engine:
         joint_*: joint-position guidance (cmdi_sample_args.joint_guidance): joint_target (batch, nframes, 22, 3) fp32,
         joint_mask of the same shape (y['mask'] folded in), joint_mean / joint_std (njoints,), joint_coef one entry per
         sampler step.
+        keyframe_scale (batch,): keyframe classifier-free guidance (cmdi_sample_args.keyframe_scale), one entry per
+        window under windows.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         K = 0 if window_frames0 is None else len(window_frames0)
@@ -176,6 +180,7 @@ class Engine:
 
         init_image, x_T = prep(init_image, shp=shape), prep(x_T, shp=gshape)
         cond_emb, text_scale = prep(cond_emb, shp=(batch, 512)), prep(text_scale, shp=(batch,))
+        keyframe_scale = prep(keyframe_scale, shp=(batch,))
         y_mask = prep(y_mask, torch.uint8, (batch, self.nframes))
         inpainted_motion = prep(inpainted_motion, shp=shape)
         inpainting_mask = prep(inpainting_mask, torch.uint8, shape)
@@ -241,7 +246,7 @@ class Engine:
                             int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0,
                             K, f0_arr if K else None, int(global_frames), _ptr(windows),
                             int(joint_guidance), int(stop_jointguidance_at), jcoef_arr, _ptr(joint_target),
-                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d))
+                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), _ptr(keyframe_scale))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
@@ -294,17 +299,19 @@ class Engine:
         return x_next, pred
 
     def test_input_vjp(self, x, timestep, inpainted_motion, inpainting_mask, cond_emb=None, uncond=False, cfg=False,
-                       text_scale=None, obs_x0=None, obs_mask=None) -> torch.Tensor:
-        """One guided evaluation and its input-VJP (cmdi_test_input_vjp): (cfg ? 2 : 1, B, njoints, 1, nframes), the
-        gradient of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) w.r.t. x through each pass, cond pass first."""
+                       text_scale=None, obs_x0=None, obs_mask=None, keyframe_scale=None) -> torch.Tensor:
+        """One guided evaluation and its input-VJP (cmdi_test_input_vjp): (passes, B, njoints, 1, nframes), the
+        gradient of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) w.r.t. x through each pass, cond pass first
+        (passes = 1 + cfg + (keyframe_scale is not None), the keyframe-free pass last)."""
         dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
         x = dev(x)
         B = x.shape[0]
         cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
-        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
-        grad = torch.empty((2 if cfg else 1,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        obs_mask, inpainting_mask, keyframe_scale = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8), dev(keyframe_scale)
+        passes = 1 + int(bool(cfg)) + int(keyframe_scale is not None)
+        grad = torch.empty((passes,) + tuple(x.shape), dtype=torch.float32, device=self.device)
         a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
-                             _ptr(obs_x0), _ptr(obs_mask))
+                             _ptr(obs_x0), _ptr(obs_mask), _ptr(keyframe_scale))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_test_input_vjp(self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask),
                                                     grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_input_vjp")
@@ -312,21 +319,22 @@ class Engine:
 
     def test_joint_input_vjp(self, x, timestep, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, c_j,
                              inpainted_motion=None, inpainting_mask=None, c_r=0.0, cond_emb=None, uncond=False, cfg=False,
-                             text_scale=None, obs_x0=None, obs_mask=None) -> torch.Tensor:
+                             text_scale=None, obs_x0=None, obs_mask=None, keyframe_scale=None) -> torch.Tensor:
         """test_input_vjp of the joint-guided seed (cmdi_test_joint_input_vjp): the gradient of
         c_r sum((inpainted_motion - x0_hat)^2 * inpainting_mask) + c_j sum(joint_mask * (P(x0_hat) - joint_target)^2)
-        w.r.t. x through each pass, (cfg ? 2 : 1, B, njoints, 1, nframes), cond pass first.  inpainted_motion None: the
-        joint term alone."""
+        w.r.t. x through each pass, (passes, B, njoints, 1, nframes) as test_input_vjp returns it.  inpainted_motion
+        None: the joint term alone."""
         dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
         x = dev(x)
         B = x.shape[0]
         cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
         obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
         joint_target, joint_mask = dev(joint_target), dev(joint_mask, torch.uint8)
-        joint_mean, joint_std = dev(joint_mean), dev(joint_std)
-        grad = torch.empty((2 if cfg else 1,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        joint_mean, joint_std, keyframe_scale = dev(joint_mean), dev(joint_std), dev(keyframe_scale)
+        passes = 1 + int(bool(cfg)) + int(keyframe_scale is not None)
+        grad = torch.empty((passes,) + tuple(x.shape), dtype=torch.float32, device=self.device)
         a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
-                             _ptr(obs_x0), _ptr(obs_mask))
+                             _ptr(obs_x0), _ptr(obs_mask), _ptr(keyframe_scale))
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_test_joint_input_vjp(
                 self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask), float(c_r), _ptr(joint_target),

@@ -2,6 +2,8 @@
 
     MDM                          model/mdm.py:10-315   (arch='trans_enc', data_rep='hml_vec', cond_mode no_cond|text)
     ClassifierFreeSampleModel    model/cfg_sampler.py:5-35
+    KeyframeClassifierFreeSampleModel   classifier-free guidance over the keyframes of a keyframe-conditioned MDM_UNET
+                                        (y['keyframe_scale']), which the reference's scripts set and never read
 
 `MDM` owns fp32 parameters under the reference's state-dict keys (so `load_state_dict` of a reference checkpoint
 works, utils/model_util.py:19-23) and evaluates through `cmdi_model_forward`; there is no PyTorch math path.
@@ -276,7 +278,7 @@ class MDM_UNET(nn.Module):
         return _forward_any(self, x, timesteps, y, cfg=False, obs_x0=obs_x0, obs_mask=obs_mask)
 
 
-def _forward_any(inner, x, timesteps, y, cfg: bool, text_scale=None, obs_x0=None, obs_mask=None):
+def _forward_any(inner, x, timesteps, y, cfg: bool, text_scale=None, obs_x0=None, obs_mask=None, keyframe_scale=None):
     y = {} if y is None else y
     if not x.is_cuda:
         raise RuntimeError("condmdi_b200 runs on CUDA tensors only (no CPU fallback)")
@@ -293,16 +295,18 @@ def _forward_any(inner, x, timesteps, y, cfg: bool, text_scale=None, obs_x0=None
             if text_scale is not None:
                 ysub["text_scale"] = y["text_scale"][idx]
             out[idx] = _forward_any(inner, x[idx], ts[idx], ysub, cfg, None if text_scale is None else text_scale[idx],
-                                    None if obs_x0 is None else obs_x0[idx], None if obs_mask is None else obs_mask[idx])
+                                    None if obs_x0 is None else obs_x0[idx], None if obs_mask is None else obs_mask[idx],
+                                    None if keyframe_scale is None else keyframe_scale[idx])
         return out
-    eng = inner.engine_for(x.device, max_batch=x.shape[0], nframes=x.shape[-1])
+    B = x.shape[0]
+    eng = inner.engine_for(x.device, max_batch=B if keyframe_scale is None else keyframe_cfg_max_batch(B, cfg), nframes=x.shape[-1])
     cond_emb = None
     if "text" in getattr(inner, "cond_mode", "no_cond"):
         cond_emb = inner.encode_text(y["text"]).to(device=x.device, dtype=torch.float32)
     if eng.arch != capi.ARCH_UNET:
         obs_x0 = obs_mask = None  # the transformer accepts and ignores them (SURVEY 8b note 2)
     return eng.forward(x, t0, cond_emb=cond_emb, uncond=bool(y.get("uncond", False)), cfg=cfg, text_scale=text_scale,
-                       obs_x0=obs_x0, obs_mask=obs_mask)
+                       obs_x0=obs_x0, obs_mask=obs_mask, keyframe_scale=keyframe_scale)
 
 
 class ClassifierFreeSampleModel(nn.Module):
@@ -330,8 +334,82 @@ class ClassifierFreeSampleModel(nn.Module):
                             obs_mask=obs_mask)
 
 
+def keyframe_cfg_max_batch(batch: int, text_cfg: bool) -> int:
+    """The engine max_batch keyframe CFG needs for `batch` sequences: its passes (3 with text CFG, else 2) must fit the
+    2 * max_batch sequences the engine's buffers hold."""
+    return ((3 if text_cfg else 2) * batch + 1) // 2
+
+
+def _is_keyframe_unet(model) -> bool:
+    """A keyframe-conditioned MDM_UNET (this package's or the reference's), recognised by its state dict as engine_for
+    reads it: the first convolution takes 2 * input_feats channels."""
+    if not isinstance(model, nn.Module):
+        return False
+    sd = model.state_dict()
+    if "unet.time_mlp.0.weight" not in sd:
+        return False
+    return sd["unet.downs.0.0.blocks.0.block1.0.weight"].shape[1] == 2 * sd["unet.final_conv.1.weight"].shape[0]
+
+
+def check_keyframe_cfg_scales(y, text: bool) -> None:
+    """Keyframe CFG reads y['keyframe_scale'], and for a text model y['text_scale'] too (w_t = 1: text conditioning
+    without text guidance)."""
+    for key in ("keyframe_scale",) + (("text_scale",) if text else ()):
+        if y is None or key not in y:
+            raise ValueError(f"KeyframeClassifierFreeSampleModel needs y[{key!r}]"
+                             + (" (a text model's w_t; 1 for no text guidance)" if key == "text_scale" else ""))
+
+
+class KeyframeClassifierFreeSampleModel(nn.Module):
+    """Classifier-free guidance over the keyframes of a keyframe-conditioned MDM_UNET, nested inside text CFG (the
+    two-condition guidance of InstructPix2Pix, Brooks et al. 2023, eq. 3, keyframes the inner condition).  Per sample b:
+
+        c = m(x, text_b, obs)    u = m(x, no text, obs)    n = m(x, no text, obs_mask = 0)
+        text model:     x0 = n + w_k (u - n) + w_t (c - u)    w_t = y['text_scale'][b], w_k = y['keyframe_scale'][b]
+        no_cond model:  x0 = n + w_k (c - n)
+
+    n is the keyframe-dropped input the published checkpoints were trained on (keyframe_mask_prob).  In fp32 each
+    operation rounds to nearest in the order a = n + w_k (u - n), x0 = a + w_t (c - u); at w_k = 1 it is
+    ClassifierFreeSampleModel up to that rounding.  The passes run as one batch-stacked native pass; y['uncond'] makes
+    the text passes unconditional as it does for CFG.  A text model needs y['text_scale'] as ClassifierFreeSampleModel
+    does (1 for keyframe guidance alone).  Every sampler of the package accepts it in place of the model."""
+
+    def __init__(self, model):
+        super().__init__()
+        if not _is_keyframe_unet(model):
+            raise ValueError("KeyframeClassifierFreeSampleModel needs a keyframe-conditioned MDM_UNET "
+                             f"(got {type(model).__name__} without keyframe input)")
+        self.model = model
+        self.rot2xyz = getattr(model, "rot2xyz", None)
+        self.translation = model.translation
+        self.njoints = model.njoints
+        self.nfeats = model.nfeats
+        self.data_rep = model.data_rep
+        self.cond_mode = model.cond_mode
+        self.keyframe_conditioned = model.keyframe_conditioned
+        self.mask_value = -2.0
+
+    def forward(self, x, timesteps, y=None, obs_x0=None, obs_mask=None, **kwargs):
+        text = "text" in self.model.cond_mode
+        check_keyframe_cfg_scales(y, text)
+        inner, _ = resolve_model(self.model)
+        return _forward_any(inner, x, timesteps, y, cfg=text, text_scale=y["text_scale"].reshape(-1) if text else None,
+                            obs_x0=obs_x0, obs_mask=obs_mask, keyframe_scale=y["keyframe_scale"].reshape(-1))
+
+
+def is_keyframe_cfg(model) -> bool:
+    """Whether `model` (or the model a _WrappedModel holds) is a KeyframeClassifierFreeSampleModel."""
+    while type(model).__name__ == "_WrappedModel" and isinstance(getattr(model, "model", None), nn.Module):
+        model = model.model
+    return isinstance(model, KeyframeClassifierFreeSampleModel)
+
+
 def resolve_model(model) -> Tuple[nn.Module, bool]:
-    """(inner MDM-like module, is_cfg).  Accepts this package's classes and the reference's (duck-typed)."""
+    """(inner MDM-like module, is_cfg).  Accepts this package's classes and the reference's (duck-typed).  For a
+    KeyframeClassifierFreeSampleModel is_cfg says whether text CFG runs with keyframe CFG (a text model)."""
+    if isinstance(model, KeyframeClassifierFreeSampleModel):
+        inner, _ = resolve_model(model.model)
+        return inner, "text" in getattr(inner, "cond_mode", "no_cond")
     is_cfg = False
     inner = model
     if hasattr(inner, "model") and isinstance(getattr(inner, "model"), nn.Module) and \

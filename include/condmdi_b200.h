@@ -122,7 +122,19 @@ typedef struct {
 } cmdi_tensor_desc;
 
 /* One denoiser evaluation: out = model(x, timesteps, y).  With cfg != 0 the cond and uncond passes run as one
- * batch-doubled pass and out = out_uncond + text_scale[b] * (out_cond - out_uncond). */
+ * batch-doubled pass and out = out_uncond + text_scale[b] * (out_cond - out_uncond).
+ *
+ * Keyframe classifier-free guidance (keyframe_scale non-NULL; here and in cmdi_sample_args): a keyframe-conditioned
+ * MDM_UNET given obs_x0 / obs_mask also runs a keyframe-free pass n = model(x, no text, obs_mask = 0), the input with
+ * which it was trained to drop its keyframes, stacked after the other passes in one batch:
+ *   cfg = 1   rows [0,B) c = model(x, text, obs), [B,2B) u = model(x, no text, obs), [2B,3B) n;
+ *             out = (n + w_k (u - n)) + s (c - u), w_k = keyframe_scale[b], s = text_scale[b]
+ *   cfg = 0   rows [0,B) c, [B,2B) n;  out = n + w_k (c - n)
+ * each operation rounded to nearest in fp32 in that order (at w_k = 1 the cfg = 1 form is CFG's u + s (c - u) up to
+ * that rounding).  uncond makes the text passes unconditional as it does for CFG.  Imputation, reconstruction and joint
+ * guidance and the window blend act on `out` as they act on CFG's output; a guided step sums the three pass gradients.
+ * The call fails without a keyframe-conditioned UNet, without obs_x0 / obs_mask, or when passes x batch exceeds
+ * 2 * max_batch (the sequences the buffers hold). */
 typedef struct {
   int32_t batch;
   const float* x;             /* ref layout (B, 263, 1, 196) */
@@ -135,6 +147,7 @@ typedef struct {
   const float* obs_x0;        /* ref layout observed keyframes and ... */
   const uint8_t* obs_mask;    /* ... their bool mask: the obs_x0 / obs_mask arguments of MDM_UNET.forward (mdm_unet.py:765);
                                  NULL for the transformer (which ignores them, SURVEY 8b note 2) */
+  const float* keyframe_scale; /* (B,) keyframe CFG's w_k (above), or NULL: off */
 } cmdi_forward_args;
 
 typedef struct {
@@ -242,6 +255,8 @@ typedef struct {
   const float* joint_mean;      /* (njoints) fp32 dataset statistics of the de-normalisation */
   const float* joint_std;
   int32_t joint_abs3d;          /* 1: absolute root representation (abs_3d), 0: relative */
+  const float* keyframe_scale;  /* (B,) keyframe CFG's w_k (cmdi_forward_args), or NULL: off; under windows one entry per
+                                   window like text_scale */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
@@ -274,8 +289,9 @@ CMDI_API int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B
                    const float* x_obs, const uint8_t* mask, float* x_next, float* pred_xstart, void* stream);
 
 /* one guided evaluation (args as cmdi_model_forward, device pointers) and its input-VJP, as a reconstruction-guided step runs
- * them: grad receives d/dx of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) through each pass, (cfg ? 2 : 1) x
- * (B, njoints, 1, nframes), the cond pass first (the sampler adds the two and masks them).  MDM_UNET: CMDI_PRECISION_FP16 only */
+ * them: grad receives d/dx of sum((inpainted_motion - x0_hat)^2 * inpainting_mask) through each pass, passes x
+ * (B, njoints, 1, nframes) in the row order of the passes (1 + cfg + (keyframe_scale != NULL) passes; the sampler adds
+ * them and masks the sum).  MDM_UNET: CMDI_PRECISION_FP16 only */
 CMDI_API int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
                         const uint8_t* inpainting_mask, float* grad, void* stream);
 
