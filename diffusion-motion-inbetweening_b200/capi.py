@@ -33,7 +33,7 @@ EXPORTS = [
     "cmdi_test_layernorm", "cmdi_test_step", "cmdi_test_normal", "cmdi_profile_pass", "cmdi_test_layernorm_bwd", "cmdi_test_attention_bwd",
     "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp", "cmdi_joints_to_features", "cmdi_convert_motion",
     "cmdi_test_chain_layer", "cmdi_test_attention_hi", "cmdi_test_attention_bwd_at", "cmdi_test_unet_ops",
-    "cmdi_test_joint_input_vjp", "cmdi_joint_guidance_seed",
+    "cmdi_test_joint_input_vjp", "cmdi_joint_guidance_seed", "cmdi_test_foot_contact_input_vjp", "cmdi_foot_contact_seed",
 ]
 
 
@@ -71,7 +71,9 @@ class SampleArgs(Structure):
                 ("window_out", c_void_p),
                 ("joint_guidance", c_int32), ("stop_jointguidance_at", c_int32), ("joint_coef", POINTER(c_float)),
                 ("joint_target", c_void_p), ("joint_mask", c_void_p), ("joint_mean", c_void_p), ("joint_std", c_void_p),
-                ("joint_abs3d", c_int32), ("keyframe_scale", c_void_p)]
+                ("joint_abs3d", c_int32), ("keyframe_scale", c_void_p),
+                ("foot_contact", c_int32), ("stop_footcontact_at", c_int32), ("foot_contact_coef", POINTER(c_float)),
+                ("foot_contact_mask", c_void_p)]
 
 
 class UnetOpInfo(Structure):
@@ -153,6 +155,11 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
                                               c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p]
     lib.cmdi_joint_guidance_seed.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                              c_void_p, c_void_p]
+    lib.cmdi_test_foot_contact_input_vjp.argtypes = [c_void_p, POINTER(ForwardArgs), c_void_p, c_void_p, c_float, c_void_p,
+                                                     c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_float, c_void_p,
+                                                     c_void_p]
+    lib.cmdi_foot_contact_seed.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_float, c_float, c_void_p, c_void_p]
     _lib = lib
     return lib
 

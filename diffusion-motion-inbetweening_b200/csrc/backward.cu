@@ -132,8 +132,18 @@ __device__ __forceinline__ void rot_y(float c, float sn, float x, float z, float
   zo = __fadd_rn(z, __fmul_rn(2.f, __fadd_rn(__fmul_rn(c, uv2), uuv2)));
 }
 
+// Foot-contact guidance's foot joints (7, 10, 8, 11) in label order: the index of joint j, or -1.
+__device__ __forceinline__ int foot_index(int j) {
+  return j == 7 ? 0 : j == 10 ? 1 : j == 8 ? 2 : j == 11 ? 3 : -1;
+}
+
+// FC: foot-contact guidance (JointSeedParams::contact).  The instance without it is the joint seed alone.
+template <bool FC>
 __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p) {
   __shared__ float sa[256], sb[256], sc[256], wsum[8];
+  // FC: world positions of the four foot joints per frame ([3 k + axis][f]) and kappa(f, k) m(f) m(f + 1) ([k][f])
+  __shared__ float fpos[FC ? 12 * 256 : 1];
+  __shared__ uint8_t fw[FC ? 4 * 256 : 1];
   const int b = blockIdx.x, f = threadIdx.x, L = p.L;
   const bool live = f < L;
   const long long base = (long long)b * p.sb + (long long)f * p.sf;
@@ -172,24 +182,79 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
   float sn, cs;
   sincosf(ang, &sn, &cs);
   const float C2 = __fsub_rn(1.f, __fmul_rn(2.f, __fmul_rn(sn, sn))), S2 = __fmul_rn(2.f, __fmul_rn(sn, cs));
+  // ---- FC: the foot joints' positions and contact weights, exchanged with the neighbouring frames ----
+  float cj = 1.f, cc = 0.f;
+  if constexpr (FC) {
+    if (p.step_ptr) {
+      const int t = *p.step_ptr;
+      cj = p.coef[2 * t];
+      cc = p.coef[2 * t + 1];
+    } else {
+      cj = p.c_j;
+      cc = p.c_c;
+    }
+    const bool pair = live && f + 1 < L && (!p.valid || (p.valid[(size_t)b * L + f] && p.valid[(size_t)b * L + f + 1]));
+    for (int k = 0; k < 4; ++k) {
+      const int j = k == 0 ? 7 : k == 1 ? 10 : k == 2 ? 8 : 11;
+      const int c0 = 4 + 3 * (j - 1);
+      float xo = 0.f, zo = 0.f, ly = 0.f;
+      bool contact = false;
+      if (live) {
+        const float lx = feat(c0), lz = feat(c0 + 2);
+        ly = feat(c0 + 1);
+        rot_y(cs, sn, lx, lz, xo, zo);
+        contact = feat(kContactChannel + k) > 0.5f;
+      }
+      fpos[(3 * k) * 256 + f] = __fadd_rn(xo, rx);
+      fpos[(3 * k + 1) * 256 + f] = ly;
+      fpos[(3 * k + 2) * 256 + f] = __fadd_rn(zo, rz);
+      fw[k * 256 + f] = pair && contact;
+    }
+    __syncthreads();
+  }
+  // dL_c/dP of coordinate a of foot joint k at this frame: 2 w(f - 1) (P(f) - P(f - 1)) - 2 w(f) (P(f + 1) - P(f))
+  auto contact_grad = [&](int k, int a) -> float {
+    const float* q = fpos + (3 * k + a) * 256;
+    const float in = f >= 1 && fw[k * 256 + f - 1] ? __fmul_rn(2.f, __fsub_rn(q[f], q[f - 1])) : 0.f;
+    const float out = fw[k * 256 + f] ? __fmul_rn(2.f, __fsub_rn(q[f + 1], q[f])) : 0.f;
+    return __fsub_rn(in, out);
+  };
+  // FC: c_j (joint term) + c_c (contact term); otherwise the joint term unscaled
+  auto comb = [&](float gj, float gc) -> float {
+    return FC ? __fadd_rn(__fmul_rn(cj, gj), __fmul_rn(cc, gc)) : gj;
+  };
   // ---- joints: residuals, the gradients of the local coordinates, and the sums over joints ----
   float g_ang = 0.f, g_rx = 0.f, g_rz = 0.f, g_ry = 0.f;
   float* o = p.out + base;
   if (live) {
     const size_t jb = ((size_t)b * L + f) * 66;
-    const float* tg = p.target + jb;
-    const uint8_t* mk = p.mask + jb;
-    g_rx = mk[0] ? __fmul_rn(2.f, __fsub_rn(rx, tg[0])) : 0.f;
-    g_ry = mk[1] ? __fmul_rn(2.f, __fsub_rn(d3, tg[1])) : 0.f;
-    g_rz = mk[2] ? __fmul_rn(2.f, __fsub_rn(rz, tg[2])) : 0.f;
+    // FC without joint targets: the joint term is zero (its mask reads as all-false)
+    const bool jt = !FC || p.mask;
+    const float* tg = jt ? p.target + jb : nullptr;
+    const uint8_t* mk = jt ? p.mask + jb : nullptr;
+    auto on = [&](int i) { return jt && mk[i]; };
+    g_rx = on(0) ? __fmul_rn(2.f, __fsub_rn(rx, tg[0])) : 0.f;
+    g_ry = on(1) ? __fmul_rn(2.f, __fsub_rn(d3, tg[1])) : 0.f;
+    g_rz = on(2) ? __fmul_rn(2.f, __fsub_rn(rz, tg[2])) : 0.f;
+    if constexpr (FC) {
+      g_rx = comb(g_rx, 0.f);
+      g_ry = comb(g_ry, 0.f);
+      g_rz = comb(g_rz, 0.f);
+    }
     for (int j = 1; j < 22; ++j) {
       const int c0 = 4 + 3 * (j - 1);
       const float lx = feat(c0), ly = feat(c0 + 1), lz = feat(c0 + 2);
       float xo, zo;
       rot_y(cs, sn, lx, lz, xo, zo);
-      const float gx = mk[3 * j] ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(xo, rx), tg[3 * j])) : 0.f;
-      const float gy = mk[3 * j + 1] ? __fmul_rn(2.f, __fsub_rn(ly, tg[3 * j + 1])) : 0.f;
-      const float gz = mk[3 * j + 2] ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(zo, rz), tg[3 * j + 2])) : 0.f;
+      float gx = on(3 * j) ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(xo, rx), tg[3 * j])) : 0.f;
+      float gy = on(3 * j + 1) ? __fmul_rn(2.f, __fsub_rn(ly, tg[3 * j + 1])) : 0.f;
+      float gz = on(3 * j + 2) ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(zo, rz), tg[3 * j + 2])) : 0.f;
+      if constexpr (FC) {
+        const int k = foot_index(j);
+        gx = comb(gx, k >= 0 ? contact_grad(k, 0) : 0.f);
+        gy = comb(gy, k >= 0 ? contact_grad(k, 1) : 0.f);
+        gz = comb(gz, k >= 0 ? contact_grad(k, 2) : 0.f);
+      }
       o[(long long)c0 * p.sc] = __fmul_rn(__fadd_rn(__fmul_rn(gx, C2), __fmul_rn(gz, S2)), p.stdv[c0]);
       o[(long long)(c0 + 1) * p.sc] = __fmul_rn(gy, p.stdv[c0 + 1]);
       o[(long long)(c0 + 2) * p.sc] = __fmul_rn(__fsub_rn(__fmul_rn(gz, C2), __fmul_rn(gx, S2)), p.stdv[c0 + 2]);
@@ -346,8 +411,10 @@ cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t strea
 
 cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream) {
   if (p.L < 1 || p.L > 256 || p.D < kJointChannels || p.out_cols < kJointChannels) return cudaErrorInvalidValue;
+  if (p.contact && (p.D < kContactChannel + 4 || (p.step_ptr && !p.coef))) return cudaErrorInvalidValue;
   if (p.B == 0) return cudaSuccess;
-  joint_seed_kernel<<<p.B, 256, 0, stream>>>(p);
+  if (p.contact) joint_seed_kernel<true><<<p.B, 256, 0, stream>>>(p);
+  else joint_seed_kernel<false><<<p.B, 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -104,6 +104,7 @@ struct GraphKey {
   int joint, joint_abs3d;          // joint-position guidance and its root representation (the joint seed's launch
                                    // arguments); its targets and coefficients live in device memory
   int passes;                      // denoiser passes per evaluation (Passes::n): keyframe CFG adds one
+  int contact;                     // foot-contact guidance (the joint seed's FC instance); joint: joint targets
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -195,9 +196,15 @@ struct cmdi_engine {
   float* joint_target = nullptr; // (maxB, L, 22, 3)
   uint8_t* joint_mask = nullptr; // (maxB, L, 22, 3)
   float* joint_stats = nullptr;  // mean [D], std [D]
-  float* seed_coef = nullptr;    // [kMaxT][2] (c_r, c_j) per step index
+  float* seed_coef = nullptr;    // [kMaxT][2] (c_r, c_j) per step index; (c_r, 1) with foot-contact guidance
   float* unit_coef = nullptr;    // [kMaxT] ones
   std::vector<float> h_seed_coef;
+  // foot-contact guidance (cmdi_sample_args.foot_contact): the joint seed's FC instance applies (c_j, c_c) itself
+  bool joint_targets = false;    // the running call's joint seed reads joint_target / joint_mask
+  bool contact_on = false;       // the running call's joint seed adds the foot-contact term
+  uint8_t* contact_valid = nullptr;  // (maxB, L) frame validity
+  float* contact_coef = nullptr;     // [kMaxT][2] (c_j, c_c) per step index
+  std::vector<float> h_contact_coef;
   // forward path with LayerNorm folded into the consuming linear layers and the linear layers of a layer chained into one
   // persistent launch (gemm_chain.cu).  CMDI_CHAIN=0 selects the round-1 path (one launch per layer + LayerNorm kernels),
   // which guided steps (they stash LayerNorm inputs for the backward pass) always use.
@@ -680,6 +687,10 @@ int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
   jp.sb = (long long)e->L * e->D_pad; jp.sf = e->D_pad; jp.sc = 1;
   jp.target = e->joint_target; jp.mask = e->joint_mask; jp.mean = e->joint_stats; jp.stdv = e->joint_stats + e->D;
   jp.abs_3d = e->joint_abs3d; jp.out = e->joint_grad; jp.out_cols = e->D_pad;
+  if (e->contact_on) {
+    if (!e->joint_targets) { jp.target = nullptr; jp.mask = nullptr; }
+    jp.contact = 1; jp.valid = e->contact_valid; jp.coef = e->contact_coef; jp.step_ptr = e->step_ctr;
+  }
   CK(launch_joint_seed(jp, s));
   return 0;
 }
@@ -693,18 +704,21 @@ int ensure_joint(cmdi_engine* e) {
   CKI(dev_alloc(e, &e->joint_stats, (size_t)2 * e->D));
   CKI(dev_alloc(e, &e->seed_coef, (size_t)2 * kMaxT));
   CKI(dev_alloc(e, &e->unit_coef, (size_t)kMaxT));
+  CKI(dev_alloc(e, &e->contact_valid, (size_t)e->maxB * e->L));
+  CKI(dev_alloc(e, &e->contact_coef, (size_t)2 * kMaxT));
   const std::vector<float> ones(kMaxT, 1.f);
   CK(cudaMemcpy(e->unit_coef, ones.data(), ones.size() * 4, cudaMemcpyHostToDevice));
   return 0;
 }
 
-// Joint targets, mask and statistics of a call into the engine's buffers (the step graphs read them there).
+// Joint targets, mask and statistics of a call into the engine's buffers (the step graphs read them there).  target /
+// mask null: only the statistics (foot-contact guidance without joint targets).
 int stage_joint(cmdi_engine* e, int B, const float* target, const uint8_t* mask, const float* mean, const float* stdv,
                 int abs_3d, cudaStream_t s) {
   CKI(ensure_joint(e));
   const size_t n = (size_t)B * e->L * 66;
-  CK(cudaMemcpyAsync(e->joint_target, target, n * 4, cudaMemcpyDefault, s));
-  CK(cudaMemcpyAsync(e->joint_mask, mask, n, cudaMemcpyDefault, s));
+  if (target) CK(cudaMemcpyAsync(e->joint_target, target, n * 4, cudaMemcpyDefault, s));
+  if (mask) CK(cudaMemcpyAsync(e->joint_mask, mask, n, cudaMemcpyDefault, s));
   CK(cudaMemcpyAsync(e->joint_stats, mean, (size_t)e->D * 4, cudaMemcpyDefault, s));
   CK(cudaMemcpyAsync(e->joint_stats + e->D, stdv, (size_t)e->D * 4, cudaMemcpyDefault, s));
   e->joint_abs3d = abs_3d != 0;
@@ -1586,7 +1600,7 @@ StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool gui
   sp.model_out = e->model_out; sp.cfg = ps.combine(); sp.text_scale = ps.scale; sp.keyframe_scale = ps.kf_scale;
   sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
   sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
-  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance ? e->unit_coef : e->guide_coef;
+  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance || a->foot_contact ? e->unit_coef : e->guide_coef;
   sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
   sp.pred_xstart = e->pred_x0;
   sp.win_K = a->window_count; sp.win_N = a->global_frames; sp.win_f0 = e->win_f0;
@@ -1616,7 +1630,8 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.jump_length = a->repaint_jump_length; key.jump_n_sample = a->repaint_jump_n_sample;
   key.win_K = a->window_count; key.win_N = a->global_frames;
   key.joint = a->joint_guidance != 0;
-  key.joint_abs3d = key.joint && a->joint_abs3d != 0;
+  key.contact = a->foot_contact != 0;
+  key.joint_abs3d = (key.joint || key.contact) && a->joint_abs3d != 0;
   key.passes = 1 + (a->cfg ? 1 : 0) + (a->keyframe_scale ? 1 : 0);
   if (!plms) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
@@ -1834,19 +1849,26 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
     CK(cudaMemcpyAsync(e->guide_coef, a->recon_coef, (size_t)e->T * 4, cudaMemcpyHostToDevice, s));
   }
-  e->joint_on = false;
-  const bool joint = a->joint_guidance != 0;
+  e->joint_on = e->contact_on = e->joint_targets = false;
+  const bool contact = a->foot_contact != 0;
+  // the joint seed runs at guided evaluations: joint-position guidance, foot-contact guidance or both
+  const bool joint = a->joint_guidance != 0 || contact;
   if (joint) {
-    if (!a->joint_coef || !a->joint_target || !a->joint_mask || !a->joint_mean || !a->joint_std) {
+    if (a->joint_guidance && (!a->joint_coef || !a->joint_target || !a->joint_mask || !a->joint_mean || !a->joint_std)) {
       set_last_error("joint_guidance needs joint_coef, joint_target, joint_mask, joint_mean and joint_std");
       return 1;
     }
+    if (contact && (!a->foot_contact_coef || !a->joint_mean || !a->joint_std)) {
+      set_last_error("foot_contact needs foot_contact_coef, joint_mean and joint_std");
+      return 1;
+    }
+    const char* what = a->joint_guidance ? "joint-position guidance" : "foot-contact guidance";
     if (e->D != 263) {
-      set_last_error("joint-position guidance needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", e->D);
+      set_last_error("%s needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", what, e->D);
       return 1;
     }
     if (a->window_count > 0) {
-      set_last_error("joint-position guidance does not run on overlapping windows (each window's root starts at its own origin)");
+      set_last_error("%s does not run on overlapping windows (each window's root starts at its own origin)", what);
       return 1;
     }
     if (e->unet && !e->f16) {
@@ -1854,15 +1876,31 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
       return 1;
     }
     CKI(ensure_stash(e, s));
-    CKI(stage_joint(e, B, a->joint_target, a->joint_mask, a->joint_mean, a->joint_std, a->joint_abs3d, s));
-    // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere
+    CKI(stage_joint(e, B, a->joint_guidance ? a->joint_target : nullptr, a->joint_guidance ? a->joint_mask : nullptr,
+                    a->joint_mean, a->joint_std, a->joint_abs3d, s));
+    // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere.  With foot-contact guidance the
+    // joint seed applies (c_j, c_c) itself and the guidance seed's second coefficient is 1.
     e->h_seed_coef.assign((size_t)2 * e->T, 0.f);
+    e->h_contact_coef.assign((size_t)2 * e->T, 0.f);
     for (int t = 0; t < e->T; ++t) {
+      const float cj = a->joint_guidance && t >= a->stop_jointguidance_at ? a->joint_coef[t] : 0.f;
       if (a->recon_guidance && t >= a->stop_recguidance_at) e->h_seed_coef[2 * t] = a->recon_coef[t];
-      if (t >= a->stop_jointguidance_at) e->h_seed_coef[2 * t + 1] = a->joint_coef[t];
+      if (a->joint_guidance && t >= a->stop_jointguidance_at) e->h_seed_coef[2 * t + 1] = a->joint_coef[t];
+      if (contact) {
+        e->h_seed_coef[2 * t + 1] = 1.f;
+        e->h_contact_coef[2 * t] = cj;
+        if (t >= a->stop_footcontact_at) e->h_contact_coef[2 * t + 1] = a->foot_contact_coef[t];
+      }
     }
     CK(cudaMemcpyAsync(e->seed_coef, e->h_seed_coef.data(), e->h_seed_coef.size() * 4, cudaMemcpyHostToDevice, s));
+    if (contact) {
+      CK(cudaMemcpyAsync(e->contact_coef, e->h_contact_coef.data(), e->h_contact_coef.size() * 4, cudaMemcpyHostToDevice, s));
+      if (a->foot_contact_mask) CK(cudaMemcpyAsync(e->contact_valid, a->foot_contact_mask, (size_t)B * e->L, cudaMemcpyDefault, s));
+      else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
+    }
     e->joint_on = true;
+    e->contact_on = contact;
+    e->joint_targets = a->joint_guidance != 0;
   }
   if (a->skip_timesteps < 0 || a->skip_timesteps >= e->T) {
     set_last_error("skip_timesteps %d outside [0, %d)", a->skip_timesteps, e->T);
@@ -2108,9 +2146,10 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   };
   int dump_i = 0;
   // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch); a step
-  // is guided when reconstruction or joint guidance is active at it
+  // is guided when reconstruction, joint or foot-contact guidance is active at it
   auto guided_t = [&](int t) {
-    return (a->recon_guidance && t >= a->stop_recguidance_at) || (joint && t >= a->stop_jointguidance_at);
+    return (a->recon_guidance && t >= a->stop_recguidance_at) || (a->joint_guidance && t >= a->stop_jointguidance_at) ||
+           (contact && t >= a->stop_footcontact_at);
   };
   auto guided_at = [&](int k) { return guided_t(rev ? t0 + k : t0 - k); };
   // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
@@ -2218,10 +2257,10 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
 
 }  // namespace
 
-// The sampling loop (sample_call); the joint seed of a joint-guided call is never left on for a later call.
+// The sampling loop (sample_call); the joint seed of a joint- or foot-contact-guided call is never left on for a later call.
 extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
   const int rc = sample_call(e, a, out, stream_);
-  if (e) e->joint_on = false;
+  if (e) e->joint_on = e->contact_on = e->joint_targets = false;
   return rc;
 }
 
@@ -2301,7 +2340,7 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
   if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
   CK(launch_set_int(e->step_ctr, a->timestep, s));
   CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
-  e->joint_on = false;
+  e->joint_on = e->contact_on = false;
   CKI(run_backward(e, B, ps, s));
   const size_t fr = (size_t)B * e->L * e->D_pad;
   for (int pass = 0; pass < ps.n; ++pass)
@@ -2310,15 +2349,19 @@ extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, c
   return 0;
 }
 
-// cmdi_test_input_vjp with the joint term: the seed c_r G + c_j G_j, as a joint-guided sampling step at a step index
-// whose coefficients are (c_r, c_j) forms it.
-extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
-                                         const uint8_t* inpainting_mask, float c_r, const float* joint_target,
-                                         const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
-                                         int joint_abs3d, float c_j, float* grad, void* stream_) {
-  if (!e || !a || !a->x || !grad || a->host_buffers || !joint_target || !joint_mask || !joint_mean || !joint_std ||
+namespace {
+
+// cmdi_test_joint_input_vjp and cmdi_test_foot_contact_input_vjp: one guided evaluation whose seed is c_r G + c_j G_j
+// (contact 0) or c_r G + (c_j G_j + c_c G_c) (contact 1, joint_target / joint_mask may be null), as a guided sampling
+// step at a step index with those coefficients forms it.
+int joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion, const uint8_t* inpainting_mask,
+                    float c_r, const float* joint_target, const uint8_t* joint_mask, const float* joint_mean,
+                    const float* joint_std, int joint_abs3d, float c_j, int contact, const uint8_t* contact_valid, float c_c,
+                    float* grad, void* stream_, const char* fn) {
+  if (!e || !a || !a->x || !grad || a->host_buffers || !joint_mean || !joint_std ||
+      (!contact && (!joint_target || !joint_mask)) || (!joint_target) != (!joint_mask) ||
       (!inpainted_motion) != (!inpainting_mask)) {
-    set_last_error("cmdi_test_joint_input_vjp: null argument or host buffers");
+    set_last_error("%s: null argument or host buffers", fn);
     return 1;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
@@ -2338,7 +2381,8 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
     return 1;
   }
   if (e->D != 263) {
-    set_last_error("joint-position guidance needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", e->D);
+    set_last_error("%s needs HumanML3D's 263 features (22 joints), the engine has njoints = %d",
+                   contact ? "foot-contact guidance" : "joint-position guidance", e->D);
     return 1;
   }
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
@@ -2346,8 +2390,14 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
   CKI(ensure_temb(e, s));
   CKI(ensure_stash(e, s));
   CKI(stage_joint(e, B, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, s));
-  const float coef[2] = {c_r, c_j};
+  const float coef[2] = {c_r, contact ? 1.f : c_j};
   CK(cudaMemcpy(e->seed_coef + 2 * a->timestep, coef, sizeof(coef), cudaMemcpyHostToDevice));
+  if (contact) {
+    const float cc[2] = {c_j, c_c};
+    CK(cudaMemcpy(e->contact_coef + 2 * a->timestep, cc, sizeof(cc), cudaMemcpyHostToDevice));
+    if (contact_valid) CK(cudaMemcpyAsync(e->contact_valid, contact_valid, (size_t)B * e->L, cudaMemcpyDeviceToDevice, s));
+    else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
+  }
   const size_t n = (size_t)B * e->D * e->L, fr = (size_t)B * e->L * e->D_pad;
   CK(launch_ref_to_frames(a->x, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
   if (inpainted_motion) {
@@ -2364,14 +2414,39 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
   CK(launch_set_int(e->step_ctr, a->timestep, s));
   CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
   e->joint_on = true;
+  e->contact_on = contact != 0;
+  e->joint_targets = joint_target != nullptr;
   int rc = run_joint_seed(e, B, ps, s);
   rc = rc || run_backward(e, B, ps, s);
-  e->joint_on = false;
+  e->joint_on = e->contact_on = e->joint_targets = false;
   if (rc) return 1;
   for (int pass = 0; pass < ps.n; ++pass)
     CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
   e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 7;
   return 0;
+}
+
+}  // namespace
+
+// cmdi_test_input_vjp with the joint term: the seed c_r G + c_j G_j, as a joint-guided sampling step at a step index
+// whose coefficients are (c_r, c_j) forms it.
+extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                         const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                         const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                         int joint_abs3d, float c_j, float* grad, void* stream_) {
+  return joint_input_vjp(e, a, inpainted_motion, inpainting_mask, c_r, joint_target, joint_mask, joint_mean, joint_std,
+                         joint_abs3d, c_j, 0, nullptr, 0.f, grad, stream_, "cmdi_test_joint_input_vjp");
+}
+
+// cmdi_test_joint_input_vjp with the foot-contact term: the seed c_r G + (c_j G_j + c_c G_c), as a foot-contact-guided
+// sampling step at a step index whose coefficients are (c_r, c_j, c_c) forms it.
+extern "C" int cmdi_test_foot_contact_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                                const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                                const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                                int joint_abs3d, float c_j, const uint8_t* valid, float c_c, float* grad,
+                                                void* stream_) {
+  return joint_input_vjp(e, a, inpainted_motion, inpainting_mask, c_r, joint_target, joint_mask, joint_mean, joint_std,
+                         joint_abs3d, c_j, 1, valid, c_c, grad, stream_, "cmdi_test_foot_contact_input_vjp");
 }
 
 extern "C" int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,
@@ -2389,6 +2464,28 @@ extern "C" int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, in
     jp.sb = (long long)D * L; jp.sf = 1; jp.sc = L; jp.out_cols = D;
   }
   jp.target = target; jp.mask = mask; jp.mean = mean; jp.stdv = std; jp.abs_3d = abs_3d != 0; jp.out = grad;
+  CK(launch_joint_seed(jp, reinterpret_cast<cudaStream_t>(stream_)));
+  return 0;
+}
+
+extern "C" int cmdi_foot_contact_seed(const float* x0, int B, int D, int L, int ld, const uint8_t* valid, const float* target,
+                                      const uint8_t* mask, const float* mean, const float* std, int abs_3d, float c_j,
+                                      float c_c, float* grad, void* stream_) {
+  if (!x0 || !mean || !std || !grad || (!target) != (!mask) || B < 0 || D < kContactChannel + 4 || L < 1 || L > 256 ||
+      (ld != 0 && ld < D)) {
+    set_last_error("cmdi_foot_contact_seed: bad arguments (need non-null x0, mean, std and grad, target and mask both or "
+                   "neither, D >= 263, 1 <= L <= 256, ld 0 or >= D)");
+    return 1;
+  }
+  JointSeedParams jp{};
+  jp.B = B; jp.L = L; jp.D = D; jp.x0 = x0;
+  if (ld) {
+    jp.sb = (long long)L * ld; jp.sf = ld; jp.sc = 1; jp.out_cols = ld;
+  } else {
+    jp.sb = (long long)D * L; jp.sf = 1; jp.sc = L; jp.out_cols = D;
+  }
+  jp.target = target; jp.mask = mask; jp.mean = mean; jp.stdv = std; jp.abs_3d = abs_3d != 0; jp.out = grad;
+  jp.contact = 1; jp.valid = valid; jp.c_j = c_j; jp.c_c = c_c;
   CK(launch_joint_seed(jp, reinterpret_cast<cudaStream_t>(stream_)));
   return 0;
 }

@@ -499,7 +499,18 @@ struct JointSeedParams {
   int abs_3d;
   float* out;
   int out_cols;
+  // foot-contact guidance (contact != 0; D >= 263): out = c_j G_j + c_c G_c, where G_c = d/dx0_hat of
+  //   L_c = sum_{f, k} kappa(f, k) m(f) m(f + 1) |P_{J_k}(f + 1) - P_{J_k}(f)|^2,  J = (7, 10, 8, 11)
+  // with kappa(f, k) = [channel 259 + k of the de-normalised x0_hat > 0.5] a constant and m = valid.  (c_j, c_c) =
+  // coef[2 t], [2 t + 1] at t = step_ptr[0], or (c_j, c_c) below when step_ptr is null.  target / mask null: the joint
+  // term is off.  contact == 0: out = G_j, unscaled (the fields below are not read).
+  int contact;
+  const uint8_t* valid;       // (B, L) frame validity bytes (y['mask']), or null: every frame valid
+  const float* coef;          // [T][2] (c_j, c_c) per step index
+  const int* step_ptr;
+  float c_j, c_c;
 };
+constexpr int kContactChannel = 259;  // HumanML3D's foot-contact labels: channels 259 .. 262 for joints 7, 10, 8, 11
 cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream);
 cudaError_t launch_layernorm512_bwd(const float* dy, const float* v, const float* gamma, float eps, int rows, float* dv,
                                     __nv_bfloat16* dv_hi, __nv_bfloat16* dv_lo, cudaStream_t stream);

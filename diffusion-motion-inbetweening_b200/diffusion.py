@@ -23,7 +23,8 @@ kernels in csrc/.
 Not accelerated (raise NotImplementedError, like the reference does for its own unsupported branches):
 cond_fn / 'gmd' classifier guidance, learned variances, EPSILON/PREVIOUS_X parametrisations,
 const_noise.  `reconstruction_guidance` runs a backward pass through the denoiser on the GPU (csrc/backward.cu), and
-`joint_guidance` (not in the reference) adds a loss on world-space joint positions to the same update (JointSpace).
+`joint_guidance` (not in the reference) adds a loss on world-space joint positions to the same update (JointSpace), and
+`foot_contact_guidance` (not in the reference) one against foot sliding on the frames x0 marks as in contact.
 """
 from __future__ import annotations
 
@@ -125,7 +126,13 @@ class JointSpace:
     to reconstruction guidance's update with the coefficient w_j[t] * joint_guidance_weight * sqrt(alpha_bar_t) / 2
     (w_j = get_gradient_schedule(y['joint_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_jointguidance_at'].
     y['joint_target'] and y['joint_target_mask'] are (B, L, 22, 3), recover_from_ric's layout (a float and a bool tensor).
-    HumanML3D's 22-joint skeleton only; random-projection cards (inv_proj) are refused."""
+    HumanML3D's 22-joint skeleton only; random-projection cards (inv_proj) are refused.
+
+    With y['foot_contact_guidance'] set, every guided step also adds, with J = (7, 10, 8, 11) and P as above,
+      L_c = sum_{b, f, k} kappa(b, f, k) m(b, f) m(b, f + 1) |P_{J_k}(f + 1) - P_{J_k}(f)|^2,
+      kappa(b, f, k) = [channel 259 + k of x0^T * std + mean > 0.5] (a constant), m = y['mask']
+    with the coefficient w_c[t] * foot_contact_weight * sqrt(alpha_bar_t) / 2 (w_c = get_gradient_schedule(
+    y['foot_contact_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_footcontact_at']."""
     mean: torch.Tensor = field(repr=False)
     std: torch.Tensor = field(repr=False)
     abs_3d: bool = True
@@ -147,16 +154,7 @@ class JointSpace:
 
 def _joint_guidance_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, window, device) -> dict:
     """Engine arguments of y['joint_guidance'] (validated here, before any launch)."""
-    if space is None:
-        raise NotImplementedError("joint guidance needs diffusion.joint_space (a JointSpace: the dataset statistics and "
-                                  "abs_3d)")
-    if not isinstance(space, JointSpace):
-        raise TypeError(f"diffusion.joint_space must be a JointSpace or None, got {space!r}")
-    if D != 263 or space.mean.shape != (263,):
-        raise NotImplementedError(f"joint guidance is implemented for HumanML3D's 263 features (22 joints); the motion has "
-                                  f"{D} features and the statistics {tuple(space.mean.shape)}")
-    if window is not None:
-        raise NotImplementedError("joint guidance does not run on overlapping windows (diffusion.window)")
+    _check_joint_space(space, D, window, "joint guidance")
     for k in ("joint_target", "joint_target_mask", "joint_guidance_weight", "stop_jointguidance_at", "diffusion_steps"):
         if k not in y:
             raise ValueError(f"joint guidance needs y[{k!r}]")
@@ -183,6 +181,45 @@ def _joint_guidance_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, 
     return dict(joint_guidance=True, stop_jointguidance_at=int(stop), joint_coef=(w_j * sab / 2).float().numpy(),
                 joint_target=target.to(device=device, dtype=torch.float32), joint_mask=mask,
                 joint_mean=space.mean.to(device), joint_std=space.std.to(device), joint_abs3d=bool(space.abs_3d))
+
+
+def _check_joint_space(space, D, window, what) -> None:
+    """The refusals joint-position and foot-contact guidance share, raised before any launch."""
+    if space is None:
+        raise NotImplementedError(f"{what} needs diffusion.joint_space (a JointSpace: the dataset statistics and abs_3d)")
+    if not isinstance(space, JointSpace):
+        raise TypeError(f"diffusion.joint_space must be a JointSpace or None, got {space!r}")
+    if D != 263 or space.mean.shape != (263,):
+        raise NotImplementedError(f"{what} is implemented for HumanML3D's 263 features (22 joints); the motion has "
+                                  f"{D} features and the statistics {tuple(space.mean.shape)}")
+    if window is not None:
+        raise NotImplementedError(f"{what} does not run on overlapping windows (diffusion.window)")
+
+
+def _foot_contact_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, window, device) -> dict:
+    """Engine arguments of y['foot_contact_guidance'] (validated here, before any launch)."""
+    _check_joint_space(space, D, window, "foot-contact guidance")
+    for k in ("foot_contact_weight", "stop_footcontact_at", "diffusion_steps"):
+        if k not in y:
+            raise ValueError(f"foot-contact guidance needs y[{k!r}]")
+    weight, stop = y["foot_contact_weight"], y["stop_footcontact_at"]
+    if isinstance(weight, bool) or not isinstance(weight, (int, float, np.integer, np.floating)):
+        raise ValueError(f"y['foot_contact_weight'] must be a number, got {weight!r}")
+    if isinstance(stop, bool) or not isinstance(stop, (int, np.integer)):
+        raise ValueError(f"y['stop_footcontact_at'] must be an int, got {stop!r}")
+    valid = y.get("mask")
+    if valid is not None:
+        if not isinstance(valid, torch.Tensor) or valid.numel() != B * L:
+            raise ValueError(f"y['mask'] must hold one entry per frame ({B} x {L}), got {tuple(getattr(valid, 'shape', ()))}")
+        valid = valid.to(device).reshape(B, L).bool()
+    # w_c[t] * weight * sqrt(alpha_bar_t) / 2 in fp32, as reconstruction guidance forms its coefficient
+    ws = get_gradient_schedule(y.get("foot_contact_gradient_schedule"), y["diffusion_steps"])
+    tt = torch.arange(num_timesteps)
+    w_c = torch.from_numpy(ws)[tt].float() * float(weight)
+    sab = torch.from_numpy(sqrt_alphas_cumprod)[tt].float()
+    return dict(foot_contact=True, stop_footcontact_at=int(stop), foot_contact_coef=(w_c * sab / 2).float().numpy(),
+                foot_contact_mask=valid, joint_mean=space.mean.to(device), joint_std=space.std.to(device),
+                joint_abs3d=bool(space.abs_3d))
 
 
 def _crop_windows(x: torch.Tensor, f0: List[int], F: int) -> torch.Tensor:
@@ -323,6 +360,9 @@ class GaussianDiffusion:
         if y.get("joint_guidance", False):
             joint = _joint_guidance_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
                                          self.sqrt_alphas_cumprod, self.window, device)
+        if y.get("foot_contact_guidance", False):
+            joint.update(_foot_contact_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
+                                            self.sqrt_alphas_cumprod, self.window, device))
         rows = keyframe_cfg_max_batch(B * K, is_cfg) if kf_cfg else B * K  # keyframe CFG: its passes fit 2 * max_batch
         eng = inner.engine_for(device, max_batch=max(rows, self.max_batch or 0), precision=self.precision, nframes=F)
         eng.set_schedule(self.betas, self.timestep_map)

@@ -131,7 +131,8 @@ class Engine:
                joint_guidance: bool = False, stop_jointguidance_at: int = 0, joint_coef: Optional[Sequence[float]] = None,
                joint_target: Optional[torch.Tensor] = None, joint_mask: Optional[torch.Tensor] = None,
                joint_mean: Optional[torch.Tensor] = None, joint_std: Optional[torch.Tensor] = None, joint_abs3d: bool = False,
-               keyframe_scale: Optional[torch.Tensor] = None):
+               keyframe_scale: Optional[torch.Tensor] = None, foot_contact: bool = False, stop_footcontact_at: int = 0,
+               foot_contact_coef: Optional[Sequence[float]] = None, foot_contact_mask: Optional[torch.Tensor] = None):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -161,6 +162,9 @@ class Engine:
         sampler step.
         keyframe_scale (batch,): keyframe classifier-free guidance (cmdi_sample_args.keyframe_scale), one entry per
         window under windows.
+        foot_contact*: foot-contact guidance (cmdi_sample_args.foot_contact): foot_contact_coef one entry per sampler
+        step, foot_contact_mask (batch, nframes) the valid frames or None; it reads joint_mean / joint_std / joint_abs3d,
+        and joint_target / joint_mask only with joint_guidance.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         K = 0 if window_frames0 is None else len(window_frames0)
@@ -220,6 +224,14 @@ class Engine:
             joint_target = prep(joint_target, shp=(batch, self.nframes, 22, 3))
             joint_mask = prep(joint_mask, torch.uint8, (batch, self.nframes, 22, 3))
             joint_mean, joint_std = prep(joint_mean, shp=(self.njoints,)), prep(joint_std, shp=(self.njoints,))
+        fcoef_arr = None
+        if foot_contact:
+            fcoef = np.ascontiguousarray(np.asarray(foot_contact_coef, dtype=np.float32))
+            if fcoef.shape != (self.num_timesteps,):
+                raise ValueError(f"foot_contact_coef must have one entry per sampler step ({self.num_timesteps})")
+            fcoef_arr = fcoef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+            foot_contact_mask = prep(foot_contact_mask, torch.uint8, (batch, self.nframes))
+            joint_mean, joint_std = prep(joint_mean, shp=(self.njoints,)), prep(joint_std, shp=(self.njoints,))
         n_iter = self.num_timesteps - int(skip_timesteps)
         if num_steps:
             n_iter = min(n_iter, int(num_steps))
@@ -246,7 +258,9 @@ class Engine:
                             int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0,
                             K, f0_arr if K else None, int(global_frames), _ptr(windows),
                             int(joint_guidance), int(stop_jointguidance_at), jcoef_arr, _ptr(joint_target),
-                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), _ptr(keyframe_scale))
+                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), _ptr(keyframe_scale),
+                            int(foot_contact), int(stop_footcontact_at), fcoef_arr,
+                            _ptr(foot_contact_mask) if foot_contact else None)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
@@ -342,6 +356,38 @@ class Engine:
                 _stream_ptr(self.device)), "cmdi_test_joint_input_vjp")
         return grad
 
+    def test_foot_contact_input_vjp(self, x, timestep, joint_mean, joint_std, joint_abs3d, c_c, valid=None, joint_target=None,
+                                    joint_mask=None, c_j=0.0, inpainted_motion=None, inpainting_mask=None, c_r=0.0,
+                                    cond_emb=None, uncond=False, cfg=False, text_scale=None, obs_x0=None, obs_mask=None,
+                                    keyframe_scale=None) -> torch.Tensor:
+        """test_joint_input_vjp with foot-contact guidance (cmdi_test_foot_contact_input_vjp): the gradient of
+        c_r L_r + c_j L_j + c_c L_c w.r.t. x through each pass, (passes, B, njoints, 1, nframes).  valid (B, nframes): the
+        valid frames (None: all).  joint_target None: no joint term; inpainted_motion None: no reconstruction term."""
+        dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
+        x = dev(x)
+        B = x.shape[0]
+        cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
+        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
+        joint_target, joint_mask, valid = dev(joint_target), dev(joint_mask, torch.uint8), dev(valid, torch.uint8)
+        joint_mean, joint_std, keyframe_scale = dev(joint_mean), dev(joint_std), dev(keyframe_scale)
+        if valid is not None:
+            valid = valid.reshape(B, -1).contiguous()
+        passes = 1 + int(bool(cfg)) + int(keyframe_scale is not None)
+        grad = torch.empty((passes,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
+                             _ptr(obs_x0), _ptr(obs_mask), _ptr(keyframe_scale))
+        with torch.cuda.device(self.device):
+            capi.check(self.lib.cmdi_test_foot_contact_input_vjp(
+                self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask), float(c_r), _ptr(joint_target),
+                _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), float(c_j), _ptr(valid), float(c_c),
+                grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_foot_contact_input_vjp")
+        return grad
+
+    @staticmethod
+    def foot_contact_seed(*args, **kwargs) -> torch.Tensor:
+        """foot_contact_seed (cmdi_foot_contact_seed), the seed kernel alone"""
+        return foot_contact_seed(*args, **kwargs)
+
     def test_unet_ops(self, hook, x, timestep, cond_emb=None, uncond=False, cfg=False, text_scale=None, obs_x0=None,
                       obs_mask=None, inpainted_motion=None, inpainting_mask=None) -> torch.Tensor:
         """MDM_UNET (cmdi_test_unet_ops): the forward Engine.forward runs, or with inpainted_motion / inpainting_mask the
@@ -398,4 +444,32 @@ def joint_guidance_seed(x0: torch.Tensor, target: torch.Tensor, mask: torch.Tens
     with torch.cuda.device(dev):
         capi.check(lib.cmdi_joint_guidance_seed(_ptr(x0), B, D, L, int(ld), _ptr(target), _ptr(mask), _ptr(mean), _ptr(std),
                                                 int(abs_3d), grad.data_ptr(), _stream_ptr(dev)), "cmdi_joint_guidance_seed")
+    return grad
+
+
+def foot_contact_seed(x0: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, abs_3d: bool, valid: Optional[torch.Tensor] = None,
+                      c_c: float = 1.0, target: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None,
+                      c_j: float = 0.0, ld: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """cmdi_foot_contact_seed: c_j dL_j/dx0 + c_c dL_c/dx0 on a CUDA device, L_c the foot-contact loss
+    (cmdi_sample_args.foot_contact) with valid (B, L) the valid frames (None: all) and L_j joint_guidance_seed's loss
+    (target / mask None: no joint term).  Layouts as joint_guidance_seed."""
+    lib = capi.load()
+    dev = x0.device
+    if dev.type != "cuda":
+        raise RuntimeError("foot_contact_seed runs on CUDA devices only (no CPU fallback)")
+    f = lambda t, dt=torch.float32: None if t is None else t.to(dev, dt).contiguous()  # noqa: E731
+    x0, mean, std, valid, target, mask = f(x0), f(mean), f(std), f(valid, torch.uint8), f(target), f(mask, torch.uint8)
+    B, D = x0.shape[0], mean.shape[0]
+    L = x0.shape[1] if ld else x0.shape[-1]
+    want = (B, L, ld) if ld else (B, D, 1, L)
+    if (tuple(x0.shape) != want or std.shape != (D,) or (valid is not None and valid.numel() != B * L) or
+            (target is None) != (mask is None) or
+            (target is not None and (target.shape != (B, L, 22, 3) or mask.shape != (B, L, 22, 3)))):
+        raise ValueError("foot_contact_seed: x0 must be (B, D, 1, L) (ld = 0) or (B, L, ld), mean / std (D,), valid B * L "
+                         "frames, and target / mask (B, L, 22, 3) both or neither")
+    grad = torch.empty_like(x0) if out is None else out
+    with torch.cuda.device(dev):
+        capi.check(lib.cmdi_foot_contact_seed(_ptr(x0), B, D, L, int(ld), _ptr(valid), _ptr(target), _ptr(mask), _ptr(mean),
+                                              _ptr(std), int(abs_3d), float(c_j), float(c_c), grad.data_ptr(), _stream_ptr(dev)),
+                   "cmdi_foot_contact_seed")
     return grad

@@ -257,6 +257,19 @@ typedef struct {
   int32_t joint_abs3d;          /* 1: absolute root representation (abs_3d), 0: relative */
   const float* keyframe_scale;  /* (B,) keyframe CFG's w_k (cmdi_forward_args), or NULL: off; under windows one entry per
                                    window like text_scale */
+  /* Foot-contact guidance (all fields 0 / NULL: off): a third loss on the same update, against foot sliding on the
+     frames x0_hat itself marks as in contact.  With P as for joint guidance (joint_mean, joint_std and joint_abs3d are
+     read; joint_target / joint_mask only with joint_guidance on), J = (7, 10, 8, 11) and
+       kappa(b, f, k) = [channel 259 + k of x0_hat * joint_std + joint_mean > 0.5]     a constant: no gradient
+       L_c = sum over b, f < L - 1, k of kappa(b, f, k) m(b, f) m(b, f + 1) |P_Jk(f + 1) - P_Jk(f)|^2
+       x0_tilde = x0_hat - ~M * (c_r(t) dL_r/dz + c_j(t) dL_j/dz + c_c(t) dL_c/dz)
+     with m = foot_contact_mask (NULL: every frame valid) and c_c(t) = foot_contact_coef[t] while t >= stop_footcontact_at
+     (else 0).  A step is guided when any of c_r, c_j, c_c applies.  The limits of joint guidance apply.  Pointers follow
+     host_buffers like the fields above. */
+  int32_t foot_contact;
+  int32_t stop_footcontact_at;
+  const float* foot_contact_coef;  /* HOST array [T]: w_c[t] * foot_contact_weight * sqrt(alphas_cumprod[t]) / 2, fp32 */
+  const uint8_t* foot_contact_mask; /* (B, L) bool bytes: the valid frames (y['mask']), or NULL */
 } cmdi_sample_args;
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
@@ -308,6 +321,20 @@ CMDI_API int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* 
  * grad (up to ld) are zero.  67 <= D, 1 <= L <= 256.  Device pointers. */
 CMDI_API int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,
                                       const float* mean, const float* std, int abs_3d, float* grad, void* stream);
+/* cmdi_test_joint_input_vjp with foot-contact guidance: grad receives the gradient of
+ * c_r L_r + c_j L_j + c_c L_c through each pass (L_c as in cmdi_sample_args, m = valid (B, L) bytes or NULL: every frame
+ * valid).  joint_target / joint_mask may both be NULL (no joint term); inpainted_motion / inpainting_mask may be NULL. */
+CMDI_API int cmdi_test_foot_contact_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
+                                              const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                              const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                              int joint_abs3d, float c_j, const uint8_t* valid, float c_c, float* grad,
+                                              void* stream);
+/* The foot-contact guidance seed alone: grad = c_j dL_j/dx0 + c_c dL_c/dx0 (L_j as cmdi_joint_guidance_seed, with target
+ * / mask both NULL: no joint term; L_c as in cmdi_sample_args with m = valid, (B, L) bytes or NULL).  Layouts as
+ * cmdi_joint_guidance_seed; channels >= 67 of grad are zero.  263 <= D, 1 <= L <= 256.  Device pointers. */
+CMDI_API int cmdi_foot_contact_seed(const float* x0, int B, int D, int L, int ld, const uint8_t* valid, const float* target,
+                                    const uint8_t* mask, const float* mean, const float* std, int abs_3d, float c_j, float c_c,
+                                    float* grad, void* stream);
 
 /* One MDM_UNET op of a pass, as cmdi_test_unet_ops hands it to its callback.  Views are device pointers into the engine's
  * own buffers, [rows, cols] with a row pitch; "level layout" is the halo layout of level l: nseq * (256 >> l) rows, the
