@@ -121,6 +121,14 @@ struct Passes {
   bool combine() const { return n > 1; }
 };
 
+// The joint seed of a call's guided evaluations (joint-position guidance, foot-contact guidance or both): whether it
+// runs, whether it adds the foot-contact term, whether it reads joint_target / joint_mask, and the root representation.
+// Its targets, statistics and coefficients live in the engine's buffers (the step graphs read them there).
+struct Guidance {
+  bool joint = false, contact = false, targets = false;
+  int abs3d = 0;
+};
+
 // One op of a RePaint walk: denoise at p (the position moves p -> p - 1) or undo into p (p - 1 -> p).
 struct WalkOp {
   int p;
@@ -190,8 +198,6 @@ struct cmdi_engine {
   float* guide_coef = nullptr; // [T] w_r[t] * sqrt(alpha_bar_t) / 2
   // joint-position guidance (cmdi_sample_args.joint_guidance): the seed carries both coefficients and the step kernels
   // read unit_coef instead of guide_coef
-  bool joint_on = false;       // the running call's guided evaluations add the joint seed
-  int joint_abs3d = 0;
   float* joint_grad = nullptr;   // G_j frame-major [frame_rows_pad, D_pad]
   float* joint_target = nullptr; // (maxB, L, 22, 3)
   uint8_t* joint_mask = nullptr; // (maxB, L, 22, 3)
@@ -200,8 +206,6 @@ struct cmdi_engine {
   float* unit_coef = nullptr;    // [kMaxT] ones
   std::vector<float> h_seed_coef;
   // foot-contact guidance (cmdi_sample_args.foot_contact): the joint seed's FC instance applies (c_j, c_c) itself
-  bool joint_targets = false;    // the running call's joint seed reads joint_target / joint_mask
-  bool contact_on = false;       // the running call's joint seed adds the foot-contact term
   uint8_t* contact_valid = nullptr;  // (maxB, L) frame validity
   float* contact_coef = nullptr;     // [kMaxT][2] (c_j, c_c) per step index
   std::vector<float> h_contact_coef;
@@ -356,7 +360,7 @@ int run_linear(cmdi_engine* e, const Planes& a, const Planes& w, const LinearPar
   return 0;
 }
 
-void set_joint_seed(const cmdi_engine* e, GuidanceSeedParams* gp);
+void set_joint_seed(const cmdi_engine* e, const Guidance& g, GuidanceSeedParams* gp);
 
 }  // namespace
 #include "engine_unet.inc"
@@ -671,14 +675,14 @@ int ensure_stash(cmdi_engine* e, cudaStream_t s) {
   return 0;
 }
 
-// The joint term of the guidance seed while a joint-guided call runs (GuidanceSeedParams::joint_grad).
-void set_joint_seed(const cmdi_engine* e, GuidanceSeedParams* gp) {
-  if (!e->joint_on) return;
+// The joint term of the guidance seed of a joint-guided evaluation (GuidanceSeedParams::joint_grad).
+void set_joint_seed(const cmdi_engine* e, const Guidance& g, GuidanceSeedParams* gp) {
+  if (!g.joint) return;
   gp->joint_grad = e->joint_grad; gp->seed_coef = e->seed_coef; gp->step_ptr = e->step_ctr;
 }
 
 // G_j of the running evaluation's x0_hat (model_out, CFG-combined) into joint_grad.
-int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
+int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, const Guidance& g, cudaStream_t s) {
   JointSeedParams jp{};
   const size_t fr = (size_t)B * e->L * e->D_pad;
   jp.B = B; jp.L = e->L; jp.D = e->D; jp.x0 = e->model_out;
@@ -686,9 +690,9 @@ int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
   if (ps.kf_scale) { jp.x0_n = e->model_out + 2 * fr; jp.keyframe_scale = ps.kf_scale; }
   jp.sb = (long long)e->L * e->D_pad; jp.sf = e->D_pad; jp.sc = 1;
   jp.target = e->joint_target; jp.mask = e->joint_mask; jp.mean = e->joint_stats; jp.stdv = e->joint_stats + e->D;
-  jp.abs_3d = e->joint_abs3d; jp.out = e->joint_grad; jp.out_cols = e->D_pad;
-  if (e->contact_on) {
-    if (!e->joint_targets) { jp.target = nullptr; jp.mask = nullptr; }
+  jp.abs_3d = g.abs3d; jp.out = e->joint_grad; jp.out_cols = e->D_pad;
+  if (g.contact) {
+    if (!g.targets) { jp.target = nullptr; jp.mask = nullptr; }
     jp.contact = 1; jp.valid = e->contact_valid; jp.coef = e->contact_coef; jp.step_ptr = e->step_ctr;
   }
   CK(launch_joint_seed(jp, s));
@@ -714,14 +718,13 @@ int ensure_joint(cmdi_engine* e) {
 // Joint targets, mask and statistics of a call into the engine's buffers (the step graphs read them there).  target /
 // mask null: only the statistics (foot-contact guidance without joint targets).
 int stage_joint(cmdi_engine* e, int B, const float* target, const uint8_t* mask, const float* mean, const float* stdv,
-                int abs_3d, cudaStream_t s) {
+                cudaStream_t s) {
   CKI(ensure_joint(e));
   const size_t n = (size_t)B * e->L * 66;
   if (target) CK(cudaMemcpyAsync(e->joint_target, target, n * 4, cudaMemcpyDefault, s));
   if (mask) CK(cudaMemcpyAsync(e->joint_mask, mask, n, cudaMemcpyDefault, s));
   CK(cudaMemcpyAsync(e->joint_stats, mean, (size_t)e->D * 4, cudaMemcpyDefault, s));
   CK(cudaMemcpyAsync(e->joint_stats + e->D, stdv, (size_t)e->D * 4, cudaMemcpyDefault, s));
-  e->joint_abs3d = abs_3d != 0;
   return 0;
 }
 
@@ -729,15 +732,15 @@ int stage_joint(cmdi_engine* e, int B, const float* target, const uint8_t* mask,
 // (gaussian_diffusion.py:415-416).  Result: guide_grad[nseq * L, D_pad] (cond rows, then uncond rows under CFG).
 // Scratch: xseq / x1 (fp32 + planes) carry the running gradients; qkv_p / attn_p / ffh_p the per-layer ones.
 constexpr int kBackwardLaunchesPerLayer = 8;  // the attention backward is two launches (dQ pass, dK/dV pass)
-int run_backward(cmdi_engine* e, int B, const Passes& ps, cudaStream_t s) {
-  if (e->unet) return unet_backward(e, e->unet, B, ps, s);
+int run_backward(cmdi_engine* e, int B, const Passes& ps, const Guidance& g, cudaStream_t s) {
+  if (e->unet) return unet_backward(e, e->unet, B, ps, g, s);
   const bool cfg = ps.combine();
   const int nseq = cfg ? 2 * B : B;
   const int M = nseq * e->S, MF = nseq * e->L;
   GuidanceSeedParams gp{};
   gp.B = B; gp.L = e->L; gp.D = e->D; gp.D_pad = e->D_pad; gp.cfg = cfg; gp.model_out = e->model_out;
   gp.text_scale = e->text_scale; gp.x_obs = e->x_obs; gp.obs_mask = e->obs_mask; gp.seed_hi = e->seed_p.hi; gp.seed_lo = e->seed_p.lo;
-  set_joint_seed(e, &gp);
+  set_joint_seed(e, g, &gp);
   CK(launch_guidance_seed(gp, s));
   // output head backward: d(xseq) rows s >= 1; the token rows receive no gradient from the head
   CK(cudaMemsetAsync(e->xseq, 0, (size_t)M * kDModel * 4, s));
@@ -801,7 +804,7 @@ int launches_per_pass(const cmdi_engine* e, bool guided = false) {
   return 1 + 1 + e->layers * 7 + 1;
 }
 
-int check_ready(cmdi_engine* e, int B, bool need_schedule) {
+int check_ready(const cmdi_engine* e, int B, bool need_schedule) {
   if (!e->weights_loaded) {
     set_last_error("weights not loaded (cmdi_load_weights)");
     return 1;
@@ -1275,42 +1278,71 @@ const void* stage_in(const void* user, void* dev_scratch, size_t bytes, bool hos
   return dev_scratch;
 }
 
-int prepare_cond(cmdi_engine* e, int B, const float* cond_emb_user, bool host, cudaStream_t s) {
-  if (!cond_emb_user) return 0;
-  if (!e->cfg.has_text) {
-    set_last_error("cond_emb given but the engine was created with has_text = 0");
+// The first refusals of a denoiser evaluation at a given step (cmdi_forward_args): an engine ready for batch B, the
+// inputs of CFG (`what` names the call in its refusal) and a timestep inside the positional table.
+int check_forward_args(const cmdi_engine* e, const cmdi_forward_args* a, const char* what) {
+  CKI(check_ready(e, a->batch, false));
+  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
+    set_last_error("%s needs cond_emb and text_scale (cfg_sampler.py:26, :35)", what);
     return 1;
   }
-  CK(cudaMemcpyAsync(e->cond_emb, cond_emb_user, (size_t)B * 512 * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
-  // embed_text(enc_text): once per call instead of once per step and pass (mdm.py:249-250 re-runs it every step)
-  if (e->f16) CK(launch_small_linear_f16(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, s));
-  else CK(launch_small_linear(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, 0, s));
-  e->launches += 1;
+  if (a->timestep < 0 || a->timestep >= kMaxT) {
+    set_last_error("timestep %d outside the positional table", a->timestep);
+    return 1;
+  }
   return 0;
 }
 
-// model_kwargs['obs_x0'] / ['obs_mask'] of a keyframe-conditioned MDM_UNET (mdm_unet.py:765-783): staged frame-major once
-// per call; the transformer ignores them (SURVEY 8b note 2)
-int stage_keyframe_input(cmdi_engine* e, int B, const float* obs_x0, const uint8_t* obs_mask, bool host, cudaStream_t s) {
-  if (!e->unet) return 0;
-  if ((obs_x0 == nullptr) != (obs_mask == nullptr)) {
+// The refusals of what stage_cond stages: an MDM_UNET's keyframe input (both or neither of obs_x0 / obs_mask, and both
+// for a keyframe-conditioned one) and a text embedding (only for a text model).  `Args` is cmdi_forward_args or
+// cmdi_sample_args.
+template <class Args>
+int check_cond(const cmdi_engine* e, const Args* a) {
+  if (e->unet && (a->obs_x0 == nullptr) != (a->obs_mask == nullptr)) {
     set_last_error("with spatial conditioning, both obs_x0 and obs_mask must be provided (mdm_unet.py:775)");
     return 1;
   }
-  if (e->unet->kf && !obs_x0) {
+  if (e->unet && e->unet->kf && !a->obs_x0) {
     set_last_error("a keyframe-conditioned UNet needs obs_x0 and obs_mask");
     return 1;
   }
-  e->unet->has_kf = e->unet->kf && obs_x0 != nullptr;
-  if (!e->unet->has_kf) return 0;
-  int rc = 0;
-  const size_t n = (size_t)B * e->D * e->L;
-  const float* obs = (const float*)stage_in(obs_x0, e->ref_b, n * 4, host, s, &rc);
-  const uint8_t* msk = (const uint8_t*)stage_in(obs_mask, e->ref_mask, n, host, s, &rc);
-  if (rc) return 1;
-  CK(launch_ref_to_frames(obs, B, e->D, e->L, e->D_pad, e->unet->kf_obs, nullptr, nullptr, s));
-  CK(launch_mask_to_frames(msk, nullptr, B, e->D, e->L, e->D_pad, e->unet->kf_mask, s));
-  e->launches += 2;
+  if (a->cond_emb && !e->cfg.has_text) {
+    set_last_error("cond_emb given but the engine was created with has_text = 0");
+    return 1;
+  }
+  return 0;
+}
+
+// The per-call conditioning of the denoiser's evaluations, checked by check_cond: the keyframe input, the text
+// embedding, the CFG and keyframe-CFG scales, and the step counter at `step`.
+template <class Args>
+int stage_cond(cmdi_engine* e, const Args* a, const Passes& ps, bool host, int step, cudaStream_t s) {
+  const int B = a->batch;
+  const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+  // model_kwargs['obs_x0'] / ['obs_mask'] of a keyframe-conditioned MDM_UNET (mdm_unet.py:765-783): staged frame-major
+  // once per call; the transformer ignores them (SURVEY 8b note 2)
+  if (e->unet) e->unet->has_kf = e->unet->kf && a->obs_x0 != nullptr;
+  if (e->unet && e->unet->has_kf) {
+    int rc = 0;
+    const size_t n = (size_t)B * e->D * e->L;
+    const float* obs = (const float*)stage_in(a->obs_x0, e->ref_b, n * 4, host, s, &rc);
+    const uint8_t* msk = (const uint8_t*)stage_in(a->obs_mask, e->ref_mask, n, host, s, &rc);
+    if (rc) return 1;
+    CK(launch_ref_to_frames(obs, B, e->D, e->L, e->D_pad, e->unet->kf_obs, nullptr, nullptr, s));
+    CK(launch_mask_to_frames(msk, nullptr, B, e->D, e->L, e->D_pad, e->unet->kf_mask, s));
+    e->launches += 2;
+  }
+  if (a->cond_emb) {
+    CK(cudaMemcpyAsync(e->cond_emb, a->cond_emb, (size_t)B * 512 * 4, kind, s));
+    // embed_text(enc_text): once per call instead of once per step and pass (mdm.py:249-250 re-runs it every step)
+    if (e->f16) CK(launch_small_linear_f16(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, s));
+    else CK(launch_small_linear(e->cond_emb, e->et_w, e->et_b, e->cond_proj, B, kDModel, 512, 0, s));
+    e->launches += 1;
+  }
+  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, kind, s));
+  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, kind, s));
+  CK(launch_set_int(e->step_ctr, step, s));
+  e->launches += 1;
   return 0;
 }
 
@@ -1324,16 +1356,9 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
   CK(cudaSetDevice(e->device));
   const int B = a->batch;
-  CKI(check_ready(e, B, false));
-  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
-    set_last_error("cfg forward needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
-    return 1;
-  }
-  if (a->timestep < 0 || a->timestep >= 5000) {
-    set_last_error("timestep %d outside the positional table", a->timestep);
-    return 1;
-  }
+  CKI(check_forward_args(e, a, "cfg forward"));
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  CKI(check_cond(e, a));
   const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   const bool host = a->host_buffers != 0;
   const size_t n = (size_t)B * e->D * e->L;
@@ -1343,11 +1368,7 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
   const float* x = (const float*)stage_in(a->x, e->ref_a, n * 4, host, s, &rc);
   if (rc) return 1;
   CK(launch_ref_to_frames(x, B, e->D, e->L, e->D_pad, e->unet ? e->x_state : nullptr, e->x_state_p.hi, e->x_state_p.lo, s));  // the UNet's input builder reads fp32
-  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, host, s));
-  CKI(prepare_cond(e, B, a->cond_emb, host, s));
-  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
-  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
-  CK(launch_set_int(e->step_ctr, a->timestep, s));
+  CKI(stage_cond(e, a, ps, host, a->timestep, s));
   const bool has_cond = a->cond_emb != nullptr;
   const int n_cond = a->uncond ? 0 : B;  // y['uncond'] under the CFG wrapper makes BOTH passes unconditional (cfg_sampler.py:28-33)
   CKI(run_denoiser(e, B, ps, n_cond, has_cond, /*tmap*/ nullptr, s));
@@ -1360,7 +1381,7 @@ extern "C" int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* a, fl
   CK(launch_diffusion_step(sp, s));
   float* dst = host ? e->ref_b : out;
   CK(launch_frames_to_ref(e->pred_x0, B, e->D, e->L, e->D_pad, dst, s));
-  e->launches += launches_per_pass(e) + 4;
+  e->launches += launches_per_pass(e) + 3;
   if (host) {
     CK(cudaMemcpyAsync(out, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1563,32 +1584,70 @@ std::vector<WalkOp> repaint_walk(int t0, int j, int r) {
   return w;
 }
 
-// The first argument the samplers added to the reference's (DPM-Solver++ as ODE and SDE, UniPC, DDIM inversion,
-// RePaint) have no use for but the caller set, or null.
-const char* field_to_unset(const cmdi_sample_args* a) {
-  const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER, rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC, sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
-  const bool repaint = a->sampler == CMDI_SAMPLER_REPAINT;
-  if (!dpm && !rev && !unipc && !sde && !repaint) return nullptr;
-  if (a->eta != 0.f)
-    return dpm ? "eta (DPM-Solver++ is deterministic after x_T: eta must be 0)"
-           : unipc ? "eta (UniPC is deterministic after x_T: eta must be 0)"
-           : sde ? "eta (the SDE solver's noise is fixed by the schedule: eta must be 0)"
-           : repaint ? "eta (RePaint denoises with p_sample: eta must be 0)"
-                 : "eta (the reverse ODE is deterministic: eta must be 0)";
-  if (a->noise_tape && !sde && !repaint) return dpm || unipc ? "noise_tape (no noise is drawn after x_T)" : "noise_tape";
-  if (rev && a->init_image) return "init_image";
-  if (a->dump_xstart) return "dump_xstart";
-  if (a->plms_order) return "plms_order";
-  if (a->plms_old_eps_out) return "plms_old_eps_out";
-  if ((dpm || unipc || sde || repaint) && a->resume && a->init_image)
-    return "init_image (a resume call continues the running state)";
-  return nullptr;
+// The running history a sampler keeps on the device and a `resume` call continues: none, the eps ring (PLMS), the x0
+// ring (DPM-Solver++ as ODE and SDE, UniPC) or the walk (RePaint).
+enum class History { kNone, kEps, kX0, kWalk };
+
+// What cmdi_sample needs to know of a sampler, indexed by CMDI_SAMPLER_*.
+struct SamplerInfo {
+  const char* name;                  // in refusals
+  const char* label;                 // the history's name in the resume refusal
+  int32_t cmdi_sample_args::*order;  // the field the sampler's order comes from (RePaint: its jump length), or null
+  const char* order_name;
+  int order_lo, order_hi;            // its bounds; order_hi 0: no upper bound
+  const char* bounds_note;           // the end of the bounds refusal
+  History hist;
+  bool ascends;                      // DDIM inversion: up from t0 = skip_timesteps, from the given x_T, no q_sample
+  bool windows;                      // runs on overlapping windows
+  const char* no_tape_or_dump;       // the refusal of a noise_tape or dump_xstart (after the window checks), or null
+  // the generic fields eta, noise_tape, init_image, dump_xstart, plms_order, plms_old_eps_out and init_image on a resume
+  // call, checked in that order: the reason each must be unset ("<name>: <reason> must be unset"), or null: it may be set
+  const char* unset[7];
+};
+constexpr const char* kResumeInit = "init_image (a resume call continues the running state)";
+constexpr SamplerInfo kSamplers[] = {
+    {"CMDI_SAMPLER_DDPM", nullptr, nullptr, nullptr, 0, 0, "", History::kNone, false, true, nullptr, {}},
+    {"CMDI_SAMPLER_DDIM", nullptr, nullptr, nullptr, 0, 0, "", History::kNone, false, true, nullptr, {}},
+    {"CMDI_SAMPLER_PLMS", "PLMS", &cmdi_sample_args::plms_order, "plms_order", 2, 4, "", History::kEps, false, true,
+     "PLMS draws no per-step noise and has no dump_steps: noise_tape and dump_xstart must be NULL", {}},
+    {"CMDI_SAMPLER_DDIM_REVERSE", nullptr, nullptr, nullptr, 0, 0, "", History::kNone, true, false, nullptr,
+     {"eta (the reverse ODE is deterministic: eta must be 0)", "noise_tape", "init_image", "dump_xstart", "plms_order",
+      "plms_old_eps_out", nullptr}},
+    {"CMDI_SAMPLER_DPM_SOLVER", "DPM-Solver++", &cmdi_sample_args::dpm_order, "dpm_order", 1, 3, "", History::kX0, false,
+     true, nullptr,
+     {"eta (DPM-Solver++ is deterministic after x_T: eta must be 0)", "noise_tape (no noise is drawn after x_T)", nullptr,
+      "dump_xstart", "plms_order", "plms_old_eps_out", kResumeInit}},
+    {"CMDI_SAMPLER_UNIPC", "UniPC", &cmdi_sample_args::unipc_order, "unipc_order", 1, 3, "", History::kX0, false, true,
+     nullptr,
+     {"eta (UniPC is deterministic after x_T: eta must be 0)", "noise_tape (no noise is drawn after x_T)", nullptr,
+      "dump_xstart", "plms_order", "plms_old_eps_out", kResumeInit}},
+    {"CMDI_SAMPLER_DPM_SOLVER_SDE", "SDE-DPM-Solver++", &cmdi_sample_args::dpm_order, "dpm_order", 1, 2,
+     " (CMDI_SAMPLER_DPM_SOLVER_SDE)", History::kX0, false, true, nullptr,
+     {"eta (the SDE solver's noise is fixed by the schedule: eta must be 0)", nullptr, nullptr, "dump_xstart",
+      "plms_order", "plms_old_eps_out", kResumeInit}},
+    {"CMDI_SAMPLER_REPAINT", "RePaint", &cmdi_sample_args::repaint_jump_length, "repaint_jump_length", 1, 0, "",
+     History::kWalk, false, false, nullptr,
+     {"eta (RePaint denoises with p_sample: eta must be 0)", nullptr, nullptr, "dump_xstart", "plms_order",
+      "plms_old_eps_out", kResumeInit}},
+};
+constexpr int kNumSamplers = sizeof(kSamplers) / sizeof(kSamplers[0]);
+
+// The sampler's order, or 0 for a sampler without one.
+int order_of(const cmdi_sample_args* a) {
+  const SamplerInfo& sm = kSamplers[a->sampler];
+  return sm.order ? a->*sm.order : 0;
 }
 
-// Kernel launches of one evaluation of a sampling step: the denoiser pass, a guided one's backward pass, the step kernel.
-int launches_per_eval(const cmdi_engine* e, bool guided) {
-  return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) + (e->joint_on ? 1 : 0) : 0);
+// The step index a call starts from: DDIM inversion ascends from skip_timesteps, every other sampler descends from
+// T - 1 - skip_timesteps.
+int first_step(const cmdi_engine* e, const cmdi_sample_args* a) {
+  return kSamplers[a->sampler].ascends ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
+}
+
+// Kernel launches of one evaluation of a sampling step: the denoiser pass, a guided one's backward pass and joint seed,
+// the step kernel.
+int launches_per_eval(const cmdi_engine* e, bool guided, const Guidance& g) {
+  return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) + (g.joint ? 1 : 0) : 0);
 }
 
 // What every sampler's step kernel reads and writes: the schedule, the device step counter, the combine inputs (model
@@ -1616,16 +1675,15 @@ enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
 // The graph of `group` consecutive steps of this call's configuration with guidance `guided`; for PLMS, of one step of
 // kind `plms_kind` whose second evaluation has guidance `guided2` (both 0 for the other samplers).  The first step index
 // lives in device memory, so t0 stays 0.  PLMS draws no noise: its key leaves eta and the tape at zero.  The order is
-// plms_order, unipc_order or (DPM-Solver++, ODE and SDE) dpm_order; the sampler field tells the two DPM-Solver++ apart.
+// the sampler's (order_of); the sampler field tells apart the samplers that read the same order field.
 // GraphKey is ordered by memcmp and has padding bytes, so the whole struct is zeroed before it is filled.
 GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int plms_kind, bool guided2) {
-  const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
   GraphKey key;
   memset(&key, 0, sizeof(key));
   key.B = a->batch; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
   key.stop_at = a->stop_imputation_at; key.has_cond = a->cond_emb != nullptr; key.uncond = a->uncond != 0;
   key.guided = guided; key.group = group;
-  key.order = plms ? a->plms_order : a->sampler == CMDI_SAMPLER_UNIPC ? a->unipc_order : a->dpm_order;
+  key.order = order_of(a);
   key.variant = a->unipc_variant; key.corrector = a->unipc_corrector;
   key.jump_length = a->repaint_jump_length; key.jump_n_sample = a->repaint_jump_n_sample;
   key.win_K = a->window_count; key.win_N = a->global_frames;
@@ -1633,51 +1691,58 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.contact = a->foot_contact != 0;
   key.joint_abs3d = (key.joint || key.contact) && a->joint_abs3d != 0;
   key.passes = 1 + (a->cfg ? 1 : 0) + (a->keyframe_scale ? 1 : 0);
-  if (!plms) {
+  if (a->sampler != CMDI_SAMPLER_PLMS) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
   key.plms_phase = plms_kind; key.guided2 = guided2;
   return key;
 }
 
-// use_graph 1: calls of one or two steps are launched directly unless a step graph of this configuration already exists
-// (capturing and instantiating one costs more than it saves there); use_graph 2 (the *_progressive generators: one
-// native call per step, many calls): always through the step graph.  A noise tape (a test aid) is addressed through a
-// kernel argument: per-step calls with a moving tape pointer would capture a new graph every step, so they are
-// launched directly.
-bool step_uses_graph(int use_graph, bool no_graph, int nsteps, const float* tape, bool key_exists) {
-  return use_graph && !no_graph && (nsteps >= 3 || (use_graph >= 2 && !tape) || key_exists);
-}
-
-// The executable graph of `key`: the cached one, or what `enqueue(stream)` issues, captured on a private stream (so a
-// caller's legacy / default stream is never put into capture mode), instantiated and cached.
+// Runs the steps of `key`: key.group of them through its step graph, or one by direct launches, and counts `launches`
+// kernel launches per step run into *ran.  The graph is the cached one, or what `enqueue(stream, steps)` issues,
+// captured on a private stream (so a caller's legacy / default stream is never put into capture mode), instantiated and
+// cached.  use_graph 1: calls of one or two steps are launched directly unless a one-step graph of this configuration
+// already exists (capturing and instantiating one costs more than it saves there); use_graph 2 (the *_progressive
+// generators: one native call per step, many calls): always through the step graph.  A noise tape (a test aid) is
+// addressed through a kernel argument: per-step calls with a moving tape pointer would capture a new graph every step,
+// so they are launched directly.
 template <class Enqueue>
-int capture_step_graph(cmdi_engine* e, const GraphKey& key, Enqueue enqueue, cudaGraphExec_t* out_exec) {
-  auto it = e->graphs.find(key);
-  if (it != e->graphs.end()) {
-    *out_exec = it->second;
+int dispatch_steps(cmdi_engine* e, const cmdi_sample_args* a, const GraphKey& key, int nsteps, Enqueue enqueue,
+                   int64_t launches, cudaStream_t s, int* ran) {
+  GraphKey one = key;
+  one.group = 1;
+  const bool exists = e->graphs.count(one) != 0;
+  *ran = 1;
+  if (!a->use_graph || e->no_graph || !(nsteps >= 3 || (a->use_graph >= 2 && !a->noise_tape) || exists)) {
+    CKI(enqueue(s, 1));
+    e->launches += launches;
     return 0;
   }
-  cudaStream_t cs = nullptr;
-  CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t ex = nullptr;
-  int erc = 0;
-  cudaError_t ce = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-  if (ce == cudaSuccess) {
-    erc = enqueue(cs);
-    ce = cudaStreamEndCapture(cs, &graph);  // also when enqueueing failed: the stream must leave capture mode
-    if (!erc && ce == cudaSuccess) ce = cudaGraphInstantiate(&ex, graph, 0);
+  auto it = e->graphs.find(key);
+  if (it == e->graphs.end()) {
+    cudaStream_t cs = nullptr;
+    CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t ex = nullptr;
+    int erc = 0;
+    cudaError_t ce = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
+    if (ce == cudaSuccess) {
+      erc = enqueue(cs, key.group);
+      ce = cudaStreamEndCapture(cs, &graph);  // also when enqueueing failed: the stream must leave capture mode
+      if (!erc && ce == cudaSuccess) ce = cudaGraphInstantiate(&ex, graph, 0);
+    }
+    if (graph) cudaGraphDestroy(graph);
+    cudaStreamDestroy(cs);
+    if (erc) return 1;  // enqueue has set the error
+    if (ce != cudaSuccess) {
+      set_last_error("capturing or instantiating a step graph failed: %s", cudaGetErrorString(ce));
+      return 1;
+    }
+    it = e->graphs.emplace(key, ex).first;
   }
-  if (graph) cudaGraphDestroy(graph);
-  cudaStreamDestroy(cs);
-  if (erc) return 1;  // enqueue has set the error
-  if (ce != cudaSuccess) {
-    set_last_error("capturing or instantiating a step graph failed: %s", cudaGetErrorString(ce));
-    return 1;
-  }
-  e->graphs[key] = ex;
-  *out_exec = ex;
+  CK(cudaGraphLaunch(it->second, s));
+  *ran = key.group;
+  e->launches += (int64_t)key.group * launches;
   return 0;
 }
 
@@ -1706,7 +1771,7 @@ int check_windows(const cmdi_engine* e, const cmdi_sample_args* a) {
     set_last_error("window_count %d must be >= 0", K);
     return 1;
   }
-  if (a->sampler == CMDI_SAMPLER_DDIM_REVERSE || a->sampler == CMDI_SAMPLER_REPAINT) {
+  if (!kSamplers[a->sampler].windows) {
     set_last_error("window_count: sampler %d (DDIM inversion / RePaint) does not run on overlapping windows", a->sampler);
     return 1;
   }
@@ -1738,92 +1803,68 @@ int check_windows(const cmdi_engine* e, const cmdi_sample_args* a) {
   return 0;
 }
 
-}  // namespace
-
-namespace {
-int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
-  if (!e || !a || !out) {
-    set_last_error("null argument");
-    return 1;
-  }
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
-  CK(cudaSetDevice(e->device));
+// Every refusal of cmdi_sample, in the order the call meets them.  It allocates, copies and writes nothing, so a refused
+// call leaves the engine, its running history included, as it found it.
+int check_sample_args(const cmdi_engine* e, const cmdi_sample_args* a) {
   const int B = a->batch;
   CKI(check_ready(e, B, true));
-  if (a->sampler != CMDI_SAMPLER_DDPM && a->sampler != CMDI_SAMPLER_DDIM && a->sampler != CMDI_SAMPLER_PLMS &&
-      a->sampler != CMDI_SAMPLER_DDIM_REVERSE && a->sampler != CMDI_SAMPLER_DPM_SOLVER && a->sampler != CMDI_SAMPLER_UNIPC &&
-      a->sampler != CMDI_SAMPLER_DPM_SOLVER_SDE && a->sampler != CMDI_SAMPLER_REPAINT) {
+  if (a->sampler < 0 || a->sampler >= kNumSamplers) {
     set_last_error("unknown sampler %d", a->sampler);
     return 1;
   }
-  const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
-  const bool dpm = a->sampler == CMDI_SAMPLER_DPM_SOLVER;
-  const bool unipc = a->sampler == CMDI_SAMPLER_UNIPC;
-  // SDE-DPM-Solver++: DPM-Solver++'s x0 history, with DDPM's per-step draws
-  const bool sde = a->sampler == CMDI_SAMPLER_DPM_SOLVER_SDE;
-  // RePaint: p_sample steps and undo ops along a walk that revisits steps; its running walk is its history
-  const bool repaint = a->sampler == CMDI_SAMPLER_REPAINT;
-  const bool multistep = plms || dpm || unipc || sde || repaint;  // samplers with a device-resident history
-  // DDIM inversion (ddim_reverse_sample, eta = 0): ascends from t0 = skip_timesteps, starts from the given state, draws
-  // nothing and has no q_sample, dump or PLMS history
-  const bool rev = a->sampler == CMDI_SAMPLER_DDIM_REVERSE;
-  if (!dpm && !sde && a->dpm_order) {
+  const SamplerInfo& sm = kSamplers[a->sampler];
+  // the order fields of the other samplers must be 0
+  if (sm.order != &cmdi_sample_args::dpm_order && a->dpm_order) {
     set_last_error("dpm_order is a CMDI_SAMPLER_DPM_SOLVER / CMDI_SAMPLER_DPM_SOLVER_SDE field: it must be 0 for sampler %d",
                    a->sampler);
     return 1;
   }
-  if (!unipc && (a->unipc_order || a->unipc_variant || a->unipc_corrector)) {
+  if (sm.order != &cmdi_sample_args::unipc_order && (a->unipc_order || a->unipc_variant || a->unipc_corrector)) {
     set_last_error("%s is a CMDI_SAMPLER_UNIPC field: it must be 0 for sampler %d",
                    a->unipc_order ? "unipc_order" : a->unipc_variant ? "unipc_variant" : "unipc_corrector", a->sampler);
     return 1;
   }
-  if (!repaint && (a->repaint_jump_length || a->repaint_jump_n_sample)) {
+  if (sm.order != &cmdi_sample_args::repaint_jump_length && (a->repaint_jump_length || a->repaint_jump_n_sample)) {
     set_last_error("%s is a CMDI_SAMPLER_REPAINT field: it must be 0 for sampler %d",
                    a->repaint_jump_length ? "repaint_jump_length" : "repaint_jump_n_sample", a->sampler);
     return 1;
   }
-  if (const char* bad = field_to_unset(a)) {
-    set_last_error("%s: %s must be unset",
-                   dpm ? "CMDI_SAMPLER_DPM_SOLVER" : unipc ? "CMDI_SAMPLER_UNIPC" : sde ? "CMDI_SAMPLER_DPM_SOLVER_SDE"
-                   : repaint ? "CMDI_SAMPLER_REPAINT" : "CMDI_SAMPLER_DDIM_REVERSE", bad);
+  const bool set[7] = {a->eta != 0.f, a->noise_tape != nullptr, a->init_image != nullptr, a->dump_xstart != nullptr,
+                       a->plms_order != 0, a->plms_old_eps_out != nullptr, a->resume && a->init_image};
+  for (int f = 0; f < 7; ++f) {
+    if (sm.unset[f] && set[f]) {
+      set_last_error("%s: %s must be unset", sm.name, sm.unset[f]);
+      return 1;
+    }
+  }
+  const int order = order_of(a);
+  if (sm.order && sm.order_hi == 0 && order < sm.order_lo) {
+    set_last_error("%s %d must be >= %d", sm.order_name, order, sm.order_lo);
     return 1;
   }
-  if (repaint && (a->repaint_jump_length < 1 || a->repaint_jump_n_sample < 1)) {
-    set_last_error("%s %d must be >= 1", a->repaint_jump_length < 1 ? "repaint_jump_length" : "repaint_jump_n_sample",
-                   a->repaint_jump_length < 1 ? a->repaint_jump_length : a->repaint_jump_n_sample);
+  if (sm.order && sm.order_hi != 0 && (order < sm.order_lo || order > sm.order_hi)) {
+    set_last_error("%s %d outside [%d, %d]%s", sm.order_name, order, sm.order_lo, sm.order_hi, sm.bounds_note);
     return 1;
   }
-  if (dpm && (a->dpm_order < 1 || a->dpm_order > 3)) {
-    set_last_error("dpm_order %d outside [1, 3]", a->dpm_order);
+  if (sm.order == &cmdi_sample_args::repaint_jump_length && a->repaint_jump_n_sample < 1) {
+    set_last_error("repaint_jump_n_sample %d must be >= 1", a->repaint_jump_n_sample);
     return 1;
   }
-  if (sde && (a->dpm_order < 1 || a->dpm_order > 2)) {
-    set_last_error("dpm_order %d outside [1, 2] (CMDI_SAMPLER_DPM_SOLVER_SDE)", a->dpm_order);
-    return 1;
-  }
-  if (unipc && (a->unipc_order < 1 || a->unipc_order > 3)) {
-    set_last_error("unipc_order %d outside [1, 3]", a->unipc_order);
-    return 1;
-  }
-  if (unipc && a->unipc_variant != CMDI_UNIPC_BH1 && a->unipc_variant != CMDI_UNIPC_BH2) {
+  if (sm.order == &cmdi_sample_args::unipc_order && a->unipc_variant != CMDI_UNIPC_BH1 && a->unipc_variant != CMDI_UNIPC_BH2) {
     set_last_error("unipc_variant %d is neither CMDI_UNIPC_BH1 (1) nor CMDI_UNIPC_BH2 (2)", a->unipc_variant);
     return 1;
   }
-  if (unipc && a->unipc_corrector != 0 && a->unipc_corrector != 1) {
+  if (sm.order == &cmdi_sample_args::unipc_order && a->unipc_corrector != 0 && a->unipc_corrector != 1) {
     set_last_error("unipc_corrector %d is neither 0 nor 1", a->unipc_corrector);
     return 1;
   }
-  if (rev && !a->x_T) {
-    set_last_error("CMDI_SAMPLER_DDIM_REVERSE needs x_T, the state to invert");
-    return 1;
-  }
-  if (plms && (a->plms_order < 2 || a->plms_order > 4)) {
-    set_last_error("plms_order %d outside [2, 4]", a->plms_order);
+  if (sm.ascends && !a->x_T) {
+    set_last_error("%s needs x_T, the state to invert", sm.name);
     return 1;
   }
   CKI(check_windows(e, a));
-  if (plms && (a->noise_tape || a->dump_xstart)) {
-    set_last_error("PLMS draws no per-step noise and has no dump_steps: noise_tape and dump_xstart must be NULL");
+  if (sm.no_tape_or_dump && (a->noise_tape || a->dump_xstart)) {
+    set_last_error("%s", sm.no_tape_or_dump);
     return 1;
   }
   if (a->cfg && (!a->cond_emb || !a->text_scale)) {
@@ -1831,7 +1872,6 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     return 1;
   }
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
-  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   if ((a->imputate || a->recon_guidance) && (!a->inpainted_motion || !a->inpainting_mask)) {
     set_last_error("imputate / reconstruction_guidance need inpainted_motion and inpainting_mask (editing_util.py:330, :343)");
     return 1;
@@ -1840,25 +1880,16 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     set_last_error(kUnetGuidancePrecision);
     return 1;
   }
-  if (a->recon_guidance) {
-    if (!a->recon_coef) {
-      set_last_error("reconstruction_guidance needs recon_coef");
-      return 1;
-    }
-    CKI(ensure_stash(e, s));
-    if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
-    CK(cudaMemcpyAsync(e->guide_coef, a->recon_coef, (size_t)e->T * 4, cudaMemcpyHostToDevice, s));
+  if (a->recon_guidance && !a->recon_coef) {
+    set_last_error("reconstruction_guidance needs recon_coef");
+    return 1;
   }
-  e->joint_on = e->contact_on = e->joint_targets = false;
-  const bool contact = a->foot_contact != 0;
-  // the joint seed runs at guided evaluations: joint-position guidance, foot-contact guidance or both
-  const bool joint = a->joint_guidance != 0 || contact;
-  if (joint) {
+  if (a->joint_guidance || a->foot_contact) {
     if (a->joint_guidance && (!a->joint_coef || !a->joint_target || !a->joint_mask || !a->joint_mean || !a->joint_std)) {
       set_last_error("joint_guidance needs joint_coef, joint_target, joint_mask, joint_mean and joint_std");
       return 1;
     }
-    if (contact && (!a->foot_contact_coef || !a->joint_mean || !a->joint_std)) {
+    if (a->foot_contact && (!a->foot_contact_coef || !a->joint_mean || !a->joint_std)) {
       set_last_error("foot_contact needs foot_contact_coef, joint_mean and joint_std");
       return 1;
     }
@@ -1875,9 +1906,75 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
       set_last_error(kUnetGuidancePrecision);
       return 1;
     }
+  }
+  if (a->skip_timesteps < 0 || a->skip_timesteps >= e->T) {
+    set_last_error("skip_timesteps %d outside [0, %d)", a->skip_timesteps, e->T);
+    return 1;
+  }
+  const int t0 = first_step(e, a);
+  if (sm.hist != History::kNone && a->resume) {
+    // a RePaint walk resumes at the position its next op starts from: p for a denoise op at p, p - 1 for an undo op
+    // into p
+    const bool at = sm.hist != History::kWalk ? t0 == e->hist_t_start - e->hist_steps
+                                              : e->walk_next < e->walk.size() &&
+                                                    t0 == e->walk[e->walk_next].p - (e->walk[e->walk_next].undo ? 1 : 0);
+    if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
+        e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
+        e->hist_jump_n_sample != a->repaint_jump_n_sample || e->hist_win != window_key(a) || !at) {
+      set_last_error("%s resume at step %d does not continue the running history", sm.label, t0);
+      return 1;
+    }
+  }
+  if (sm.hist == History::kWalk && !a->resume) {
+    // the walk's ops are numbered in device memory and its engine-generator streams start at 2^30 (the kernel's
+    // kWalkStream): 2^28 ops are far more than any schedule needs
+    const long long j = a->repaint_jump_length, r = a->repaint_jump_n_sample;
+    const long long ops = t0 + 1 + 2 * (r - 1) * j * (j <= t0 ? t0 / j : 0);
+    if (ops > (1LL << 28)) {
+      set_last_error("repaint_jump_length %d and repaint_jump_n_sample %d give a walk of %lld ops (at most 2^28)",
+                     a->repaint_jump_length, a->repaint_jump_n_sample, ops);
+      return 1;
+    }
+  }
+  if (a->rng_mode == CMDI_RNG_TORCH) {
+    if (a->aten_threads == 0 || a->aten_increment == 0 || (a->aten_increment & 3) || (a->aten_offset & 3)) {
+      set_last_error("rng_mode=CMDI_RNG_TORCH needs aten_threads > 0 and aten_offset / aten_increment multiples of 4");
+      return 1;
+    }
+  } else if (a->rng_mode != CMDI_RNG_ENGINE) {
+    set_last_error("unknown rng_mode %d", a->rng_mode);
+    return 1;
+  }
+  CKI(check_cond(e, a));
+  if (a->noise_tape && a->host_buffers) {
+    set_last_error("noise_tape must be a device pointer (it is a test aid; stage it once outside the call)");
+    return 1;
+  }
+  return 0;
+}
+
+// A call that check_sample_args has accepted: stages its inputs, starts or continues the running history, runs its
+// steps and writes its outputs.
+int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStream_t s) {
+  const SamplerInfo& sm = kSamplers[a->sampler];
+  const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
+  const bool walk = sm.hist == History::kWalk;  // RePaint: p_sample steps and undo ops along a walk that revisits steps
+  const int B = a->batch;
+  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
+  const bool host = a->host_buffers != 0;
+  const bool contact = a->foot_contact != 0;
+  // the joint seed runs at guided evaluations: joint-position guidance, foot-contact guidance or both
+  Guidance g;
+  g.joint = a->joint_guidance || contact; g.contact = contact; g.targets = a->joint_guidance != 0; g.abs3d = a->joint_abs3d != 0;
+  if (a->recon_guidance) {
+    CKI(ensure_stash(e, s));
+    if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
+    CK(cudaMemcpyAsync(e->guide_coef, a->recon_coef, (size_t)e->T * 4, cudaMemcpyHostToDevice, s));
+  }
+  if (g.joint) {
     CKI(ensure_stash(e, s));
     CKI(stage_joint(e, B, a->joint_guidance ? a->joint_target : nullptr, a->joint_guidance ? a->joint_mask : nullptr,
-                    a->joint_mean, a->joint_std, a->joint_abs3d, s));
+                    a->joint_mean, a->joint_std, s));
     // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere.  With foot-contact guidance the
     // joint seed applies (c_j, c_c) itself and the guidance seed's second coefficient is 1.
     e->h_seed_coef.assign((size_t)2 * e->T, 0.f);
@@ -1898,15 +1995,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
       if (a->foot_contact_mask) CK(cudaMemcpyAsync(e->contact_valid, a->foot_contact_mask, (size_t)B * e->L, cudaMemcpyDefault, s));
       else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
     }
-    e->joint_on = true;
-    e->contact_on = contact;
-    e->joint_targets = a->joint_guidance != 0;
   }
-  if (a->skip_timesteps < 0 || a->skip_timesteps >= e->T) {
-    set_last_error("skip_timesteps %d outside [0, %d)", a->skip_timesteps, e->T);
-    return 1;
-  }
-  const bool host = a->host_buffers != 0;
   const size_t n = (size_t)B * e->D * e->L;
   // overlapping windows: x_T, the noise and the outputs are global (Bg, D, 1, N), everything else is per window
   const bool win = a->window_count > 0;
@@ -1925,72 +2014,47 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
       e->h_win_f0 = f0;
     }
   }
-  const int t0 = rev ? a->skip_timesteps : e->T - 1 - a->skip_timesteps;
-  const int remaining = rev ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
+  const int t0 = first_step(e, a);
+  const int remaining = sm.ascends ? e->T - t0 : t0 + 1;  // steps left in this loop's direction
   int nsteps = (a->num_steps > 0 && a->num_steps < remaining) ? a->num_steps : remaining;
-  // PLMS / DPM-Solver++ / UniPC / SDE-DPM-Solver++ / RePaint: a call without `resume` starts a new history at t0; a
-  // `resume` call continues the running one
+  // a call with a history and without `resume` starts a new history at t0; a `resume` call continues the running one
   int hist_t0 = t0;
-  if (multistep) {
-    const int order = plms ? a->plms_order : unipc ? a->unipc_order : repaint ? a->repaint_jump_length : a->dpm_order;
-    if (a->resume) {
-      // a RePaint walk resumes at the position its next op starts from: p for a denoise op at p, p - 1 for an undo op
-      // into p
-      const bool at = !repaint ? t0 == e->hist_t_start - e->hist_steps
-                               : e->walk_next < e->walk.size() &&
-                                     t0 == e->walk[e->walk_next].p - (e->walk[e->walk_next].undo ? 1 : 0);
-      if (!e->hist_live || e->hist_sampler != a->sampler || e->hist_order != order || e->hist_B != B ||
-          e->hist_variant != a->unipc_variant || e->hist_corrector != a->unipc_corrector ||
-          e->hist_jump_n_sample != a->repaint_jump_n_sample || e->hist_win != window_key(a) || !at) {
-        set_last_error("%s resume at step %d does not continue the running history",
-                       plms ? "PLMS" : unipc ? "UniPC" : sde ? "SDE-DPM-Solver++" : repaint ? "RePaint" : "DPM-Solver++", t0);
-        return 1;
-      }
-      hist_t0 = e->hist_t_start;
-    } else {
-      const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
-      if (repaint) {
-        // the walk's ops are numbered in device memory and its engine-generator streams start at 2^30 (the
-        // kernel's kWalkStream): 2^28 ops are far more than any schedule needs
-        const long long j = a->repaint_jump_length, r = a->repaint_jump_n_sample;
-        const long long ops = t0 + 1 + 2 * (r - 1) * j * (j <= t0 ? t0 / j : 0);
-        if (ops > (1LL << 28)) {
-          set_last_error("repaint_jump_length %d and repaint_jump_n_sample %d give a walk of %lld ops (at most 2^28)",
-                         a->repaint_jump_length, a->repaint_jump_n_sample, ops);
-          return 1;
-        }
+  const size_t slot = (size_t)e->maxB * e->L * e->D_pad;
+  if (sm.hist != History::kNone && a->resume) {
+    hist_t0 = e->hist_t_start;
+  } else if (sm.hist != History::kNone) {
+    const int order = order_of(a);
+    if (!walk && !e->hist) CKI(dev_alloc(e, &e->hist, 3 * slot));
+    if ((sm.hist == History::kEps || a->unipc_corrector) && !e->hist_keep) CKI(dev_alloc(e, &e->hist_keep, slot));
+    // one history runs at a time: DPM-Solver++, its SDE form and RePaint's undo ops share the [T][4] table
+    switch (a->sampler) {
+      case CMDI_SAMPLER_DPM_SOLVER: dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef); break;
+      case CMDI_SAMPLER_DPM_SOLVER_SDE: dpm_solver_sde_coefs(e->h_acp, t0, order, &e->h_dpm_coef); break;
+      case CMDI_SAMPLER_REPAINT:
         e->walk = repaint_walk(t0, a->repaint_jump_length, a->repaint_jump_n_sample);
         e->walk_next = 0;
-        // undo into p: x <- a_p x + b_p z, a_p = fp32(sqrt(1 - beta_p)), b_p = fp32(sqrt(beta_p)); one history runs at a
-        // time, so the table takes DPM-Solver++'s buffer
+        // undo into p: x <- a_p x + b_p z, a_p = fp32(sqrt(1 - beta_p)), b_p = fp32(sqrt(beta_p))
         e->h_dpm_coef.assign((size_t)4 * e->T, 0.f);
         for (int p = 0; p < e->T; ++p) {
           e->h_dpm_coef[(size_t)4 * p] = (float)std::sqrt(1.0 - e->h_betas[p]);
           e->h_dpm_coef[(size_t)4 * p + 1] = (float)std::sqrt(e->h_betas[p]);
         }
-        CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
-      } else if (!e->hist) {
-        CKI(dev_alloc(e, &e->hist, 3 * slot));
-      }
-      if ((plms || (unipc && a->unipc_corrector)) && !e->hist_keep) CKI(dev_alloc(e, &e->hist_keep, slot));
-      if (dpm || sde) {  // one history runs at a time: the SDE table takes the same buffer
-        if (dpm) dpm_solver_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
-        else dpm_solver_sde_coefs(e->h_acp, t0, order, &e->h_dpm_coef);
-        CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
-      }
-      if (unipc) {
+        break;
+      case CMDI_SAMPLER_UNIPC:
         if (!e->unipc_coef) CK(cudaMalloc(&e->unipc_coef, (size_t)12 * e->T * 4));
         unipc_coefs(e->h_acp, t0, order, a->unipc_variant, a->unipc_corrector != 0, &e->h_unipc_coef);
         CK(cudaMemcpyAsync(e->unipc_coef, e->h_unipc_coef.data(), e->h_unipc_coef.size() * 4, cudaMemcpyHostToDevice, s));
-      }
-      e->hist_live = true;
-      e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
-      e->hist_variant = a->unipc_variant; e->hist_corrector = a->unipc_corrector;
-      e->hist_jump_n_sample = a->repaint_jump_n_sample;
-      e->hist_win = window_key(a);
+        break;
     }
+    if (sm.order == &cmdi_sample_args::dpm_order || walk)
+      CK(cudaMemcpyAsync(e->dpm_coef, e->h_dpm_coef.data(), e->h_dpm_coef.size() * 4, cudaMemcpyHostToDevice, s));
+    e->hist_live = true;
+    e->hist_sampler = a->sampler; e->hist_order = order; e->hist_B = B; e->hist_t_start = t0; e->hist_steps = 0;
+    e->hist_variant = a->unipc_variant; e->hist_corrector = a->unipc_corrector;
+    e->hist_jump_n_sample = a->repaint_jump_n_sample;
+    e->hist_win = window_key(a);
   }
-  if (repaint) {  // num_steps counts denoise ops
+  if (walk) {  // num_steps counts denoise ops
     int left = 0;
     for (size_t i = e->walk_next; i < e->walk.size(); ++i) left += e->walk[i].undo ? 0 : 1;
     nsteps = (a->num_steps > 0 && a->num_steps < left) ? a->num_steps : left;
@@ -2005,15 +2069,6 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   RngState rng{};
   rng.seed = a->seed; rng.sample_offset = a->sample_offset; rng.mode = a->rng_mode;
   rng.aten_offset = a->aten_offset; rng.aten_increment = a->aten_increment; rng.aten_threads = a->aten_threads;
-  if (a->rng_mode == CMDI_RNG_TORCH) {
-    if (a->aten_threads == 0 || a->aten_increment == 0 || (a->aten_increment & 3) || (a->aten_offset & 3)) {
-      set_last_error("rng_mode=CMDI_RNG_TORCH needs aten_threads > 0 and aten_offset / aten_increment multiples of 4");
-      return 1;
-    }
-  } else if (a->rng_mode != CMDI_RNG_ENGINE) {
-    set_last_error("unknown rng_mode %d", a->rng_mode);
-    return 1;
-  }
   if (!xT) {
     if (a->rng_mode == CMDI_RNG_TORCH) {
       CK(launch_fill_normal_aten(e->ref_a, ng, a->seed, a->aten_offset, a->aten_threads, s));
@@ -2032,7 +2087,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   CK(launch_set_rng(e->rng, rng, s));
   e->launches += 1;
   // ---- init_image / skip_timesteps: img = q_sample(init_image, t0, img) (:1252-1260) ----
-  if (!rev && !a->resume && (a->init_image || a->skip_timesteps)) {
+  if (!sm.ascends && !a->resume && (a->init_image || a->skip_timesteps)) {
     const float* init = (const float*)stage_in(a->init_image, e->ref_b, n * 4, host, s, &rc);
     if (rc) return 1;
     if (!init) {
@@ -2046,7 +2101,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   CK(launch_ref_to_frames(xT, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
   e->launches += 1;
   // ---- keyframes ----
-  if (joint && !a->imputate && !a->recon_guidance) {  // no feature keyframes: M = 0
+  if (g.joint && !a->imputate && !a->recon_guidance) {  // no feature keyframes: M = 0
     CK(cudaMemsetAsync(e->x_obs, 0, (size_t)B * e->L * e->D_pad * 4, s));
     CK(cudaMemsetAsync(e->obs_mask, 0, (size_t)B * e->L * e->D_pad, s));
   }
@@ -2059,33 +2114,25 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     CK(launch_mask_to_frames(msk, ym, B, e->D, e->L, e->D_pad, e->obs_mask, s));
     e->launches += 2;
   }
-  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, host, s));
   // ---- conditioning ----
-  CKI(prepare_cond(e, B, a->cond_emb, host, s));
-  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
-  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, s));
-  CK(launch_set_int(e->step_ctr, t0, s));
+  CKI(stage_cond(e, a, ps, host, t0, s));
   // [2]: the history's first step (the call's for the single-step samplers), [3]: the call's first step, from which the
   // per-step draws of SDE-DPM-Solver++ are numbered (they differ on a resume)
   CK(launch_set_int(e->step_ctr + 2, hist_t0, s, t0));
-  e->launches += 2;
-  if (repaint) {
+  e->launches += 1;
+  if (walk) {
     // [4]: the walk index of the call's first op, from which its draws are numbered, [5]: that of the next op
     CK(launch_set_int(e->step_ctr + 4, (int)e->walk_next, s, (int)e->walk_next));
     e->launches += 1;
   }
 
   const float* tape = a->noise_tape;
-  if (tape && host) {
-    set_last_error("noise_tape must be a device pointer (it is a test aid; stage it once outside the call)");
-    return 1;
-  }
   const bool has_cond = a->cond_emb != nullptr;
   // one evaluation: the denoiser pass and, for a guided one, its backward pass
   auto enqueue_eval = [&](cudaStream_t st, bool guided) -> int {
     CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
-    if (guided && joint) CKI(run_joint_seed(e, B, ps, st));
-    if (guided) CKI(run_backward(e, B, ps, st));
+    if (guided && g.joint) CKI(run_joint_seed(e, B, ps, g, st));
+    if (guided) CKI(run_backward(e, B, ps, g, st));
     return 0;
   };
   // RePaint's two ops; the walk position and the draw number live in step_ctr
@@ -2097,21 +2144,19 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     sp.advance = 1; sp.sampler = a->sampler; sp.eta = a->eta;
     // first step index: step_ctr[2] (DDPM / DDIM) or step_ctr[3] (SDE-DPM-Solver++); graphs do not depend on it
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
-    if (repaint) {
-      rq.phase = 0;
-      CK(launch_repaint_step(sp, rq, st));
-    } else if (dpm || sde) {
-      DpmParams q{};
-      q.order = a->dpm_order; q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.coef = e->dpm_coef;
-      CK(dpm ? launch_dpm_solver_step(sp, q, st) : launch_dpm_solver_sde_step(sp, q, st));
-    } else if (unipc) {
-      UnipcParams q{};
-      q.order = a->unipc_order; q.corrector = a->unipc_corrector;
-      q.x0_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad;
-      q.xc = a->unipc_corrector ? e->hist_keep : nullptr; q.coef = e->unipc_coef;
-      CK(launch_unipc_step(sp, q, st));
-    } else {
-      CK(rev ? launch_ddim_reverse_step(sp, st) : launch_diffusion_step(sp, st));
+    DpmParams dq{};
+    dq.order = a->dpm_order; dq.x0_hist = e->hist; dq.hist_stride = slot; dq.coef = e->dpm_coef;
+    UnipcParams uq{};
+    uq.order = a->unipc_order; uq.corrector = a->unipc_corrector; uq.x0_hist = e->hist; uq.hist_stride = slot;
+    uq.xc = a->unipc_corrector ? e->hist_keep : nullptr; uq.coef = e->unipc_coef;
+    rq.phase = 0;
+    switch (a->sampler) {
+      case CMDI_SAMPLER_REPAINT: CK(launch_repaint_step(sp, rq, st)); break;
+      case CMDI_SAMPLER_DPM_SOLVER: CK(launch_dpm_solver_step(sp, dq, st)); break;
+      case CMDI_SAMPLER_DPM_SOLVER_SDE: CK(launch_dpm_solver_sde_step(sp, dq, st)); break;
+      case CMDI_SAMPLER_UNIPC: CK(launch_unipc_step(sp, uq, st)); break;
+      case CMDI_SAMPLER_DDIM_REVERSE: CK(launch_ddim_reverse_step(sp, st)); break;
+      default: CK(launch_diffusion_step(sp, st));
     }
     return 0;
   };
@@ -2119,7 +2164,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
     PlmsParams q{};
     q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
-    q.eps_hist = e->hist; q.hist_stride = (size_t)e->maxB * e->L * e->D_pad; q.x_keep = e->hist_keep;
+    q.eps_hist = e->hist; q.hist_stride = slot; q.x_keep = e->hist_keep;
     const bool guided[2] = {g1, g2};
     for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
       CKI(enqueue_eval(st, guided[ev]));
@@ -2137,11 +2182,15 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
   // is one step.
   const int group = !plms && e->steps_per_graph > 1 ? e->steps_per_graph : 1;
 
-  // a frame-major state [B*L, D_pad] -> the reference layout of the call's outputs: per sample, or on overlapping windows
-  // the global (Bg, D, 1, N) gathered from the first window covering each frame
-  auto to_ref = [&](const float* frames, float* dst) -> int {
-    if (win) CK(launch_window_gather(frames, Bg, a->window_count, e->D, N, e->L, e->D_pad, e->win_f0, dst, s));
-    else CK(launch_frames_to_ref(frames, B, e->D, e->L, e->D_pad, dst, s));
+  // a frame-major state [B*L, D_pad] -> `dst` in the reference layout: the call's global layout (per sample, or on
+  // overlapping windows gathered from the first window covering each frame), or with `per_window` the window layout.  A
+  // host `dst` receives a copy through ref_b, complete at the synchronise that ends the call.
+  auto write_ref = [&](const float* frames, float* dst, bool per_window) -> int {
+    float* to = host ? e->ref_b : dst;
+    if (win && !per_window) CK(launch_window_gather(frames, Bg, a->window_count, e->D, N, e->L, e->D_pad, e->win_f0, to, s));
+    else CK(launch_frames_to_ref(frames, B, e->D, e->L, e->D_pad, to, s));
+    if (host) CK(cudaMemcpyAsync(dst, e->ref_b, (per_window ? n : ng) * 4, cudaMemcpyDeviceToHost, s));
+    e->launches += 1;
     return 0;
   };
   int dump_i = 0;
@@ -2151,11 +2200,11 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
     return (a->recon_guidance && t >= a->stop_recguidance_at) || (a->joint_guidance && t >= a->stop_jointguidance_at) ||
            (contact && t >= a->stop_footcontact_at);
   };
-  auto guided_at = [&](int k) { return guided_t(rev ? t0 + k : t0 - k); };
+  auto guided_at = [&](int k) { return guided_t(sm.ascends ? t0 + k : t0 - k); };
   // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
   // launch each; a denoise op is one evaluation and the step kernel, guided by its position, through the step graphs.
   // A graph holds one denoise op.
-  for (int k = 0; repaint && k < nsteps; ++e->walk_next) {
+  for (int k = 0; walk && k < nsteps; ++e->walk_next) {
     const WalkOp op = e->walk[e->walk_next];
     if (op.undo) {
       StepParams sp = step_params(e, a, false);
@@ -2166,102 +2215,61 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* str
       continue;
     }
     const bool guided = guided_t(op.p);
-    const GraphKey key = step_graph_key(a, guided, 1, 0, false);
-    if (step_uses_graph(a->use_graph, e->no_graph, nsteps, tape, e->graphs.count(key) != 0)) {
-      cudaGraphExec_t exec = nullptr;
-      CKI(capture_step_graph(e, key, [&](cudaStream_t cs) { return enqueue_step(cs, guided); }, &exec));
-      CK(cudaGraphLaunch(exec, s));
-    } else {
-      CKI(enqueue_step(s, guided));
-    }
-    e->launches += launches_per_eval(e, guided);
+    int ran = 0;
+    CKI(dispatch_steps(e, a, step_graph_key(a, guided, 1, 0, false), nsteps,
+                       [&](cudaStream_t st, int) { return enqueue_step(st, guided); }, launches_per_eval(e, guided, g), s, &ran));
     ++k;
   }
-  for (int k = 0; !repaint && k < nsteps;) {
+  for (int k = 0; !walk && k < nsteps;) {
     const bool guided = guided_at(k);
     // PLMS: the kind of this step and the guidance of a first step's second evaluation, at t - 1
     const int kind = !plms || e->hist_steps + k > 0 ? kPlmsSteady : (t0 - k > 0 ? kPlmsFirst : kPlmsFirstAtZero);
     const bool guided2 = kind == kPlmsFirst && guided_at(k + 1);
     auto enqueue = [&](cudaStream_t st, int steps) -> int {
       if (plms) return enqueue_plms(st, kind, guided, guided2);
-      for (int g = 0; g < steps; ++g) CKI(enqueue_step(st, guided));
+      for (int i = 0; i < steps; ++i) CKI(enqueue_step(st, guided));
       return 0;
     };
-    int run = 1;
     GraphKey key = step_graph_key(a, guided, 1, kind, guided2);
-    if (step_uses_graph(a->use_graph, e->no_graph, nsteps, tape, e->graphs.count(key) != 0)) {
-      const bool dump_in_group = a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] < k + group;
-      if (group > 1 && k + group <= nsteps && !dump_in_group && guided_at(k + group - 1) == guided) key.group = run = group;
-      cudaGraphExec_t exec = nullptr;
-      CKI(capture_step_graph(e, key, [&](cudaStream_t cs) { return enqueue(cs, run); }, &exec));
-      CK(cudaGraphLaunch(exec, s));
-    } else {
-      CKI(enqueue(s, 1));
-    }
-    e->launches += (long long)run * launches_per_eval(e, guided);
-    if (kind == kPlmsFirst) e->launches += launches_per_eval(e, guided2);
-    k += run;
+    const bool dump_in_group = a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] < k + group;
+    if (group > 1 && k + group <= nsteps && !dump_in_group && guided_at(k + group - 1) == guided) key.group = group;
+    const int64_t per_step = launches_per_eval(e, guided, g) + (kind == kPlmsFirst ? launches_per_eval(e, guided2, g) : 0);
+    int ran = 0;
+    CKI(dispatch_steps(e, a, key, nsteps, enqueue, per_step, s, &ran));
+    k += ran;
     if (a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] == k - 1) {
-      if (host) {
-        CKI(to_ref(e->pred_x0, e->ref_b));
-        CK(cudaMemcpyAsync(a->dump_xstart + (size_t)dump_i * ng, e->ref_b, ng * 4, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-      } else {
-        CKI(to_ref(e->pred_x0, a->dump_xstart + (size_t)dump_i * ng));
-      }
-      e->launches += 1;
+      CKI(write_ref(e->pred_x0, a->dump_xstart + (size_t)dump_i * ng, false));
       ++dump_i;
     }
   }
   // ---- results back in the reference layout ----
-  if (host) {
-    CKI(to_ref(e->x_state, e->ref_a));
-    CK(cudaMemcpyAsync(out, e->ref_a, ng * 4, cudaMemcpyDeviceToHost, s));
-    if (a->pred_xstart_out) {
-      CKI(to_ref(e->pred_x0, e->ref_b));
-      CK(cudaMemcpyAsync(a->pred_xstart_out, e->ref_b, ng * 4, cudaMemcpyDeviceToHost, s));
-    }
-    CK(cudaStreamSynchronize(s));
-  } else {
-    CKI(to_ref(e->x_state, out));
-    if (a->pred_xstart_out) CKI(to_ref(e->pred_x0, a->pred_xstart_out));
-  }
-  e->launches += a->pred_xstart_out ? 2 : 1;
-  if (a->window_out) {  // the windows' own states, in the window layout
-    CK(launch_frames_to_ref(e->x_state, B, e->D, e->L, e->D_pad, host ? e->ref_a : a->window_out, s));
-    if (host) {
-      CK(cudaMemcpyAsync(a->window_out, e->ref_a, n * 4, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-    }
-    e->launches += 1;
-  }
-  if (multistep) e->hist_steps += nsteps;
-  if (plms) {
-    if (a->plms_old_eps_out) {
-      // the reference's old_eps list after this call's last step: eps of the last min(steps, order - 1) iterations,
-      // oldest first
-      const int n_hist = std::min(e->hist_steps, a->plms_order - 1);
-      for (int j = 0; j < n_hist; ++j) {
-        const int it = e->hist_steps - n_hist + j;
-        const float* src = e->hist + (size_t)(it % 3) * e->maxB * e->L * e->D_pad;
-        float* dst = a->plms_old_eps_out + (size_t)j * n;
-        CK(launch_frames_to_ref(src, B, e->D, e->L, e->D_pad, host ? e->ref_b : dst, s));
-        if (host) CK(cudaMemcpyAsync(dst, e->ref_b, n * 4, cudaMemcpyDeviceToHost, s));
-      }
-      if (host) CK(cudaStreamSynchronize(s));
-      e->launches += n_hist;
+  CKI(write_ref(e->x_state, out, false));
+  if (a->pred_xstart_out) CKI(write_ref(e->pred_x0, a->pred_xstart_out, false));
+  if (a->window_out) CKI(write_ref(e->x_state, a->window_out, true));  // the windows' own states
+  if (sm.hist != History::kNone) e->hist_steps += nsteps;
+  if (plms && a->plms_old_eps_out) {
+    // the reference's old_eps list after this call's last step: eps of the last min(steps, order - 1) iterations,
+    // oldest first
+    const int n_hist = std::min(e->hist_steps, a->plms_order - 1);
+    for (int j = 0; j < n_hist; ++j) {
+      const int it = e->hist_steps - n_hist + j;
+      CKI(write_ref(e->hist + (size_t)(it % 3) * slot, a->plms_old_eps_out + (size_t)j * n, true));
     }
   }
+  if (host) CK(cudaStreamSynchronize(s));
   return 0;
 }
 
 }  // namespace
 
-// The sampling loop (sample_call); the joint seed of a joint- or foot-contact-guided call is never left on for a later call.
 extern "C" int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* a, float* out, void* stream_) {
-  const int rc = sample_call(e, a, out, stream_);
-  if (e) e->joint_on = e->contact_on = e->joint_targets = false;
-  return rc;
+  if (!e || !a || !out) {
+    set_last_error("null argument");
+    return 1;
+  }
+  CK(cudaSetDevice(e->device));
+  CKI(check_sample_args(e, a));
+  return sample_call(e, a, out, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int B, const float* model_out_c,
@@ -2300,103 +2308,59 @@ extern "C" int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int
   return 0;
 }
 
-// One (CFG: batch-doubled) evaluation of the guided pass and its input-VJP, as a guided sampling step runs them: the
-// seed dL/dx0_hat of sum((inpainted_motion - x0_hat)^2 * M) (M = inpainting_mask), then the backward pass.  grad receives
-// e->guide_grad in the reference layout: (cfg ? 2 : 1) x (B, njoints, 1, nframes), the cond pass's gradient w.r.t. x first.
-// Device pointers only.
-extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
-                                   const uint8_t* inpainting_mask, float* grad, void* stream_) {
-  if (!e || !a || !a->x || !inpainted_motion || !inpainting_mask || !grad || a->host_buffers) {
-    set_last_error("cmdi_test_input_vjp: null argument or host buffers");
-    return 1;
-  }
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
-  CK(cudaSetDevice(e->device));
-  const int B = a->batch;
-  CKI(check_ready(e, B, false));
-  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
-    set_last_error("cfg needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
-    return 1;
-  }
-  if (a->timestep < 0 || a->timestep >= 5000) {
-    set_last_error("timestep %d outside the positional table", a->timestep);
-    return 1;
-  }
-  if (e->unet && !e->f16) {
-    set_last_error(kUnetGuidancePrecision);
-    return 1;
-  }
-  CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
-  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
-  CKI(ensure_temb(e, s));
-  CKI(ensure_stash(e, s));
-  const size_t n = (size_t)B * e->D * e->L;
-  CK(launch_ref_to_frames(a->x, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
-  CK(launch_ref_to_frames(inpainted_motion, B, e->D, e->L, e->D_pad, e->x_obs, nullptr, nullptr, s));
-  CK(launch_mask_to_frames(inpainting_mask, nullptr, B, e->D, e->L, e->D_pad, e->obs_mask, s));
-  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
-  CKI(prepare_cond(e, B, a->cond_emb, false, s));
-  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
-  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
-  CK(launch_set_int(e->step_ctr, a->timestep, s));
-  CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
-  e->joint_on = e->contact_on = false;
-  CKI(run_backward(e, B, ps, s));
-  const size_t fr = (size_t)B * e->L * e->D_pad;
-  for (int pass = 0; pass < ps.n; ++pass)
-    CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
-  e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 6;
-  return 0;
-}
-
 namespace {
 
-// cmdi_test_joint_input_vjp and cmdi_test_foot_contact_input_vjp: one guided evaluation whose seed is c_r G + c_j G_j
-// (contact 0) or c_r G + (c_j G_j + c_c G_c) (contact 1, joint_target / joint_mask may be null), as a guided sampling
-// step at a step index with those coefficients forms it.
-int joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion, const uint8_t* inpainting_mask,
-                    float c_r, const float* joint_target, const uint8_t* joint_mask, const float* joint_mean,
-                    const float* joint_std, int joint_abs3d, float c_j, int contact, const uint8_t* contact_valid, float c_c,
-                    float* grad, void* stream_, const char* fn) {
-  if (!e || !a || !a->x || !grad || a->host_buffers || !joint_mean || !joint_std ||
-      (!contact && (!joint_target || !joint_mask)) || (!joint_target) != (!joint_mask) ||
-      (!inpainted_motion) != (!inpainting_mask)) {
+// The joint term of a guided evaluation's seed: joint-position guidance (contact 0) or foot-contact guidance (contact 1;
+// target / mask may then be null), with the coefficients (c_r, c_j, c_c) of one step index.
+struct JointVjp {
+  float c_r, c_j, c_c;
+  const float *target, *mean, *stdv;
+  const uint8_t *mask, *valid;
+  int abs3d, contact;
+};
+
+// One (CFG: batch-doubled) evaluation of the guided pass and its input-VJP, as a guided sampling step runs them: the seed
+// dL/dx0_hat of sum((inpainted_motion - x0_hat)^2 * M) (M = inpainting_mask), or with `j` c_r G + c_j G_j (contact 0) or
+// c_r G + (c_j G_j + c_c G_c) (contact 1), G = 0 without inpainted_motion; then the backward pass.  grad receives
+// e->guide_grad in the reference layout: one (B, njoints, 1, nframes) block per pass, the cond pass's gradient w.r.t. x
+// first.  Device pointers only.
+int input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion, const uint8_t* inpainting_mask,
+              const JointVjp* j, float* grad, void* stream_, const char* fn) {
+  if (!e || !a || !a->x || !grad || a->host_buffers || (!inpainted_motion) != (!inpainting_mask) ||
+      (j ? !j->mean || !j->stdv || (!j->contact && !j->target) || (!j->target) != (!j->mask) : !inpainted_motion)) {
     set_last_error("%s: null argument or host buffers", fn);
     return 1;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
   CK(cudaSetDevice(e->device));
   const int B = a->batch;
-  CKI(check_ready(e, B, false));
-  if (a->cfg && (!a->cond_emb || !a->text_scale)) {
-    set_last_error("cfg needs cond_emb and text_scale (cfg_sampler.py:26, :35)");
-    return 1;
-  }
-  if (a->timestep < 0 || a->timestep >= kMaxT) {
-    set_last_error("timestep %d outside the positional table", a->timestep);
-    return 1;
-  }
+  CKI(check_forward_args(e, a, "cfg"));
   if (e->unet && !e->f16) {
     set_last_error(kUnetGuidancePrecision);
     return 1;
   }
-  if (e->D != 263) {
+  if (j && e->D != 263) {
     set_last_error("%s needs HumanML3D's 263 features (22 joints), the engine has njoints = %d",
-                   contact ? "foot-contact guidance" : "joint-position guidance", e->D);
+                   j->contact ? "foot-contact guidance" : "joint-position guidance", e->D);
     return 1;
   }
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  CKI(check_cond(e, a));
   const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
+  Guidance g;
   CKI(ensure_temb(e, s));
   CKI(ensure_stash(e, s));
-  CKI(stage_joint(e, B, joint_target, joint_mask, joint_mean, joint_std, joint_abs3d, s));
-  const float coef[2] = {c_r, contact ? 1.f : c_j};
-  CK(cudaMemcpy(e->seed_coef + 2 * a->timestep, coef, sizeof(coef), cudaMemcpyHostToDevice));
-  if (contact) {
-    const float cc[2] = {c_j, c_c};
-    CK(cudaMemcpy(e->contact_coef + 2 * a->timestep, cc, sizeof(cc), cudaMemcpyHostToDevice));
-    if (contact_valid) CK(cudaMemcpyAsync(e->contact_valid, contact_valid, (size_t)B * e->L, cudaMemcpyDeviceToDevice, s));
-    else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
+  if (j) {
+    g.joint = true; g.contact = j->contact != 0; g.targets = j->target != nullptr; g.abs3d = j->abs3d != 0;
+    CKI(stage_joint(e, B, j->target, j->mask, j->mean, j->stdv, s));
+    const float coef[2] = {j->c_r, j->contact ? 1.f : j->c_j};
+    CK(cudaMemcpy(e->seed_coef + 2 * a->timestep, coef, sizeof(coef), cudaMemcpyHostToDevice));
+    if (j->contact) {
+      const float cc[2] = {j->c_j, j->c_c};
+      CK(cudaMemcpy(e->contact_coef + 2 * a->timestep, cc, sizeof(cc), cudaMemcpyHostToDevice));
+      if (j->valid) CK(cudaMemcpyAsync(e->contact_valid, j->valid, (size_t)B * e->L, cudaMemcpyDeviceToDevice, s));
+      else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
+    }
   }
   const size_t n = (size_t)B * e->D * e->L, fr = (size_t)B * e->L * e->D_pad;
   CK(launch_ref_to_frames(a->x, B, e->D, e->L, e->D_pad, e->x_state, e->x_state_p.hi, e->x_state_p.lo, s));
@@ -2407,26 +2371,22 @@ int joint_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inp
     CK(cudaMemsetAsync(e->x_obs, 0, fr * 4, s));
     CK(cudaMemsetAsync(e->obs_mask, 0, fr, s));
   }
-  CKI(stage_keyframe_input(e, B, a->obs_x0, a->obs_mask, false, s));
-  CKI(prepare_cond(e, B, a->cond_emb, false, s));
-  if (a->cfg) CK(cudaMemcpyAsync(e->text_scale, a->text_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
-  if (ps.kf) CK(cudaMemcpyAsync(e->kf_scale, a->keyframe_scale, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
-  CK(launch_set_int(e->step_ctr, a->timestep, s));
+  CKI(stage_cond(e, a, ps, false, a->timestep, s));
   CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, a->cond_emb != nullptr, nullptr, s, nullptr, 1, &e->stash));
-  e->joint_on = true;
-  e->contact_on = contact != 0;
-  e->joint_targets = joint_target != nullptr;
-  int rc = run_joint_seed(e, B, ps, s);
-  rc = rc || run_backward(e, B, ps, s);
-  e->joint_on = e->contact_on = e->joint_targets = false;
-  if (rc) return 1;
+  if (j) CKI(run_joint_seed(e, B, ps, g, s));
+  CKI(run_backward(e, B, ps, g, s));
   for (int pass = 0; pass < ps.n; ++pass)
     CK(launch_frames_to_ref(e->guide_grad + pass * fr, B, e->D, e->L, e->D_pad, grad + pass * n, s));
-  e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 7;
+  e->launches += launches_per_pass(e, true) + launches_per_backward(e) + 5 + (j ? 1 : 0);
   return 0;
 }
 
 }  // namespace
+
+extern "C" int cmdi_test_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                   const uint8_t* inpainting_mask, float* grad, void* stream_) {
+  return input_vjp(e, a, inpainted_motion, inpainting_mask, nullptr, grad, stream_, "cmdi_test_input_vjp");
+}
 
 // cmdi_test_input_vjp with the joint term: the seed c_r G + c_j G_j, as a joint-guided sampling step at a step index
 // whose coefficients are (c_r, c_j) forms it.
@@ -2434,8 +2394,8 @@ extern "C" int cmdi_test_joint_input_vjp(cmdi_engine* e, const cmdi_forward_args
                                          const uint8_t* inpainting_mask, float c_r, const float* joint_target,
                                          const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
                                          int joint_abs3d, float c_j, float* grad, void* stream_) {
-  return joint_input_vjp(e, a, inpainted_motion, inpainting_mask, c_r, joint_target, joint_mask, joint_mean, joint_std,
-                         joint_abs3d, c_j, 0, nullptr, 0.f, grad, stream_, "cmdi_test_joint_input_vjp");
+  const JointVjp j{c_r, c_j, 0.f, joint_target, joint_mean, joint_std, joint_mask, nullptr, joint_abs3d, 0};
+  return input_vjp(e, a, inpainted_motion, inpainting_mask, &j, grad, stream_, "cmdi_test_joint_input_vjp");
 }
 
 // cmdi_test_joint_input_vjp with the foot-contact term: the seed c_r G + (c_j G_j + c_c G_c), as a foot-contact-guided
@@ -2445,8 +2405,8 @@ extern "C" int cmdi_test_foot_contact_input_vjp(cmdi_engine* e, const cmdi_forwa
                                                 const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
                                                 int joint_abs3d, float c_j, const uint8_t* valid, float c_c, float* grad,
                                                 void* stream_) {
-  return joint_input_vjp(e, a, inpainted_motion, inpainting_mask, c_r, joint_target, joint_mask, joint_mean, joint_std,
-                         joint_abs3d, c_j, 1, valid, c_c, grad, stream_, "cmdi_test_foot_contact_input_vjp");
+  const JointVjp j{c_r, c_j, c_c, joint_target, joint_mean, joint_std, joint_mask, valid, joint_abs3d, 1};
+  return input_vjp(e, a, inpainted_motion, inpainting_mask, &j, grad, stream_, "cmdi_test_foot_contact_input_vjp");
 }
 
 extern "C" int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,

@@ -240,27 +240,34 @@ class Engine:
         if want_old_eps and sampler == capi.SAMPLER_PLMS:
             n_old = min(plms_steps, int(plms_order) - 1)  # the length of the reference's list after that many steps
             old_eps = torch.empty((max(n_old, 1),) + shape, dtype=torch.float32, device=dev, pin_memory=host_buffers)
-        unipc = sampler == capi.SAMPLER_UNIPC
+        a = capi.SampleArgs(
+            batch=batch, sampler=sampler, eta=float(eta), skip_timesteps=int(skip_timesteps), num_steps=int(num_steps),
+            resume=int(resume), init_image=_ptr(init_image), x_T=_ptr(x_T), noise_tape=_ptr(noise_tape),
+            seed=int(seed) & (2 ** 64 - 1), sample_offset=int(sample_offset), rng_mode=int(rng_mode),
+            aten_offset=int(aten_offset), aten_increment=int(aten_increment), aten_threads=int(aten_threads),
+            cond_emb=_ptr(cond_emb), uncond=int(uncond), cfg=int(cfg), text_scale=_ptr(text_scale), y_mask=_ptr(y_mask),
+            imputate=int(imputate), stop_imputation_at=int(stop_imputation_at), inpainted_motion=_ptr(inpainted_motion),
+            inpainting_mask=_ptr(inpainting_mask), recon_guidance=int(recon_guidance),
+            stop_recguidance_at=int(stop_recguidance_at), recon_coef=coef_arr, pred_xstart_out=_ptr(pred),
+            dump_xstart=_ptr(dump), dump_steps=dump_arr, n_dump=n_dump, host_buffers=int(host_buffers),
+            use_graph=int(use_graph), obs_x0=_ptr(obs_x0), obs_mask=_ptr(obs_mask), plms_old_eps_out=_ptr(old_eps),
+            window_count=K, window_frames0=f0_arr if K else None, global_frames=int(global_frames), window_out=_ptr(windows),
+            joint_guidance=int(joint_guidance), stop_jointguidance_at=int(stop_jointguidance_at), joint_coef=jcoef_arr,
+            joint_target=_ptr(joint_target), joint_mask=_ptr(joint_mask), joint_mean=_ptr(joint_mean),
+            joint_std=_ptr(joint_std), joint_abs3d=int(joint_abs3d), keyframe_scale=_ptr(keyframe_scale),
+            foot_contact=int(foot_contact), stop_footcontact_at=int(stop_footcontact_at), foot_contact_coef=fcoef_arr)
+        # the sampler-specific fields go only to their sampler (the engine refuses them elsewhere)
         dpm = sampler in (capi.SAMPLER_DPM_SOLVER, capi.SAMPLER_DPM_SOLVER_SDE)
-        repaint = sampler == capi.SAMPLER_REPAINT
-        a = capi.SampleArgs(batch, sampler, float(eta), int(skip_timesteps), int(num_steps), int(resume), _ptr(init_image), _ptr(x_T), _ptr(noise_tape),
-                            int(seed) & (2 ** 64 - 1), int(sample_offset), int(rng_mode), int(aten_offset), int(aten_increment),
-                            int(aten_threads), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale),
-                            _ptr(y_mask), int(imputate), int(stop_imputation_at), _ptr(inpainted_motion),
-                            _ptr(inpainting_mask), int(recon_guidance), int(stop_recguidance_at), coef_arr, _ptr(pred), _ptr(dump),
-                            dump_arr, n_dump, int(host_buffers),
-                            int(use_graph), _ptr(obs_x0), _ptr(obs_mask),
-                            0 if sampler in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_UNIPC) or dpm or repaint
-                            else int(plms_order),
-                            _ptr(old_eps), int(dpm_order) if dpm else 0,
-                            int(unipc_order) if unipc else 0, int(unipc_variant) if unipc else 0,
-                            int(unipc_corrector) if unipc else 0,
-                            int(repaint_jump_length) if repaint else 0, int(repaint_jump_n_sample) if repaint else 0,
-                            K, f0_arr if K else None, int(global_frames), _ptr(windows),
-                            int(joint_guidance), int(stop_jointguidance_at), jcoef_arr, _ptr(joint_target),
-                            _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), _ptr(keyframe_scale),
-                            int(foot_contact), int(stop_footcontact_at), fcoef_arr,
-                            _ptr(foot_contact_mask) if foot_contact else None)
+        if not dpm and sampler not in (capi.SAMPLER_DDIM_REVERSE, capi.SAMPLER_UNIPC, capi.SAMPLER_REPAINT):
+            a.plms_order = int(plms_order)
+        if dpm:
+            a.dpm_order = int(dpm_order)
+        if sampler == capi.SAMPLER_UNIPC:
+            a.unipc_order, a.unipc_variant, a.unipc_corrector = int(unipc_order), int(unipc_variant), int(unipc_corrector)
+        if sampler == capi.SAMPLER_REPAINT:
+            a.repaint_jump_length, a.repaint_jump_n_sample = int(repaint_jump_length), int(repaint_jump_n_sample)
+        if foot_contact:
+            a.foot_contact_mask = _ptr(foot_contact_mask)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")

@@ -278,6 +278,7 @@ CMDI_API int cmdi_load_weights(cmdi_engine* e, const cmdi_tensor_desc* tensors, 
 /* betas: the (respaced) float64 betas of the sampler, length T; timestep_map[t] = original timestep of step t */
 CMDI_API int cmdi_set_schedule(cmdi_engine* e, const double* betas, int T, const int64_t* timestep_map);
 CMDI_API int cmdi_model_forward(cmdi_engine* e, const cmdi_forward_args* args, float* out, void* stream);
+/* the sampling loop of cmdi_sample_args (above); a call that fails leaves the running history as it was */
 CMDI_API int cmdi_sample(cmdi_engine* e, const cmdi_sample_args* args, float* out, void* stream);
 /* number of kernels of this library launched (directly or through graph replay) by the engine so far */
 CMDI_API int64_t cmdi_launch_count(const cmdi_engine* e);
