@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint8, c_uint64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint8, c_uint32, c_uint64, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CONDMDI_B200_LIB") or os.path.join(HERE, "libcondmdi_b200.so")  # override: A/B builds
@@ -15,6 +15,7 @@ PRECISION_BF16X3 = 3
 PRECISION_BF16 = 1
 PRECISION_FP16 = 2  # "autocast", MDM_UNET only: the arithmetic of torch.autocast("cuda", float16) (use_fp16 checkpoints)
 RNG_ENGINE, RNG_TORCH = 0, 1
+MAX_OBSTACLES = 16  # CMDI_MAX_OBSTACLES: obstacles per sample of obstacle-avoidance guidance
 SAMPLER_DDPM = 0
 SAMPLER_DDIM = 1
 SAMPLER_PLMS = 2
@@ -34,6 +35,7 @@ EXPORTS = [
     "cmdi_test_normal_aten", "cmdi_recover_from_ric", "cmdi_test_input_vjp", "cmdi_joints_to_features", "cmdi_convert_motion",
     "cmdi_test_chain_layer", "cmdi_test_attention_hi", "cmdi_test_attention_bwd_at", "cmdi_test_unet_ops",
     "cmdi_test_joint_input_vjp", "cmdi_joint_guidance_seed", "cmdi_test_foot_contact_input_vjp", "cmdi_foot_contact_seed",
+    "cmdi_test_obstacle_input_vjp", "cmdi_obstacle_seed",
 ]
 
 
@@ -73,7 +75,9 @@ class SampleArgs(Structure):
                 ("joint_target", c_void_p), ("joint_mask", c_void_p), ("joint_mean", c_void_p), ("joint_std", c_void_p),
                 ("joint_abs3d", c_int32), ("keyframe_scale", c_void_p),
                 ("foot_contact", c_int32), ("stop_footcontact_at", c_int32), ("foot_contact_coef", POINTER(c_float)),
-                ("foot_contact_mask", c_void_p)]
+                ("foot_contact_mask", c_void_p),
+                ("obstacle_guidance", c_int32), ("stop_obstacleguidance_at", c_int32), ("obstacle_coef", POINTER(c_float)),
+                ("obstacles", c_void_p), ("n_obstacles", c_int32), ("obstacle_joints", c_uint32), ("obstacle_mask", c_void_p)]
 
 
 class UnetOpInfo(Structure):
@@ -160,6 +164,12 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
                                                      c_void_p]
     lib.cmdi_foot_contact_seed.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_int, c_float, c_float, c_void_p, c_void_p]
+    lib.cmdi_test_obstacle_input_vjp.argtypes = [c_void_p, POINTER(ForwardArgs), c_void_p, c_void_p, c_float, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int, c_float,
+                                                 c_void_p, c_int, c_uint32, c_float, c_void_p, c_void_p]
+    lib.cmdi_obstacle_seed.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_int, c_float, c_int, c_float, c_void_p, c_int, c_uint32, c_float,
+                                       c_void_p, c_void_p]
     _lib = lib
     return lib
 

@@ -137,13 +137,16 @@ __device__ __forceinline__ int foot_index(int j) {
   return j == 7 ? 0 : j == 10 ? 1 : j == 8 ? 2 : j == 11 ? 3 : -1;
 }
 
-// FC: foot-contact guidance (JointSeedParams::contact).  The instance without it is the joint seed alone.
-template <bool FC>
-__global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p) {
+// The joint seed's body.  FC: foot-contact guidance (JointSeedParams::contact); OB: obstacle-avoidance guidance
+// (JointSeedParams::obstacle).  The instance without either is the joint seed alone.
+template <bool FC, bool OB>
+__device__ __forceinline__ void joint_seed(const JointSeedParams& p) {
   __shared__ float sa[256], sb[256], sc[256], wsum[8];
   // FC: world positions of the four foot joints per frame ([3 k + axis][f]) and kappa(f, k) m(f) m(f + 1) ([k][f])
   __shared__ float fpos[FC ? 12 * 256 : 1];
   __shared__ uint8_t fw[FC ? 4 * 256 : 1];
+  // OB: this sample's obstacles (c_x, c_z, r)
+  __shared__ float obs[OB ? 3 * kMaxObstacles : 1];
   const int b = blockIdx.x, f = threadIdx.x, L = p.L;
   const bool live = f < L;
   const long long base = (long long)b * p.sb + (long long)f * p.sf;
@@ -182,17 +185,27 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
   float sn, cs;
   sincosf(ang, &sn, &cs);
   const float C2 = __fsub_rn(1.f, __fmul_rn(2.f, __fmul_rn(sn, sn))), S2 = __fmul_rn(2.f, __fmul_rn(sn, cs));
-  // ---- FC: the foot joints' positions and contact weights, exchanged with the neighbouring frames ----
-  float cj = 1.f, cc = 0.f;
-  if constexpr (FC) {
+  // ---- the coefficients of the terms (FC / OB: the joint seed applies them itself) ----
+  float cj = 1.f, cc = 0.f, co = 0.f;
+  if constexpr (FC || OB) {
+    constexpr int stride = OB ? 3 : 2;
     if (p.step_ptr) {
       const int t = *p.step_ptr;
-      cj = p.coef[2 * t];
-      cc = p.coef[2 * t + 1];
+      cj = p.coef[stride * t];
+      if constexpr (FC) cc = p.coef[stride * t + 1];
+      if constexpr (OB) co = p.coef[stride * t + 2];
     } else {
       cj = p.c_j;
       cc = p.c_c;
+      co = p.c_o;
     }
+  }
+  if constexpr (OB) {
+    if (f < 3 * p.n_obstacles) obs[f] = p.obstacles[(size_t)b * 3 * p.n_obstacles + f];
+    __syncthreads();
+  }
+  // ---- FC: the foot joints' positions and contact weights, exchanged with the neighbouring frames ----
+  if constexpr (FC) {
     const bool pair = live && f + 1 < L && (!p.valid || (p.valid[(size_t)b * L + f] && p.valid[(size_t)b * L + f + 1]));
     for (int k = 0; k < 4; ++k) {
       const int j = k == 0 ? 7 : k == 1 ? 10 : k == 2 ? 8 : 11;
@@ -219,27 +232,50 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
     const float out = fw[k * 256 + f] ? __fmul_rn(2.f, __fsub_rn(q[f + 1], q[f])) : 0.f;
     return __fsub_rn(in, out);
   };
-  // FC: c_j (joint term) + c_c (contact term); otherwise the joint term unscaled
-  auto comb = [&](float gj, float gc) -> float {
-    return FC ? __fadd_rn(__fmul_rn(cj, gj), __fmul_rn(cc, gc)) : gj;
+  // dL_o/dP^x, dL_o/dP^z of a joint of S at world (px, pz) on this frame, L_o's 1 / L and m_o(f) included: the sum over
+  // the obstacles it is inside (distance <= r) of -(P - c) / distance, 0 at distance 0 (torch's subgradients)
+  const float o_scale = OB && live && (!p.obstacle_valid || p.obstacle_valid[(size_t)b * L + f]) ? __frcp_rn((float)L) : 0.f;
+  auto obstacle_grad = [&](float px, float pz, float& gx, float& gz) {
+    float sx = 0.f, sz = 0.f;
+    for (int k = 0; k < p.n_obstacles; ++k) {
+      const float dx = __fsub_rn(px, obs[3 * k]), dz = __fsub_rn(pz, obs[3 * k + 1]);
+      const float d = __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dz, dz)));
+      if (d <= obs[3 * k + 2] && d > 0.f) {
+        sx = __fadd_rn(sx, __fdiv_rn(dx, d));
+        sz = __fadd_rn(sz, __fdiv_rn(dz, d));
+      }
+    }
+    gx = -__fmul_rn(sx, o_scale);
+    gz = -__fmul_rn(sz, o_scale);
+  };
+  auto in_s = [&](int j) { return OB && ((p.obstacle_joints >> j) & 1u); };
+  // FC / OB: c_j (joint term) + c_c (contact term) + c_o (obstacle term); otherwise the joint term unscaled
+  auto comb = [&](float gj, float gc, float go) -> float {
+    if constexpr (!FC && !OB) return gj;
+    float r = __fmul_rn(cj, gj);
+    if constexpr (FC) r = __fadd_rn(r, __fmul_rn(cc, gc));
+    if constexpr (OB) r = __fadd_rn(r, __fmul_rn(co, go));
+    return r;
   };
   // ---- joints: residuals, the gradients of the local coordinates, and the sums over joints ----
   float g_ang = 0.f, g_rx = 0.f, g_rz = 0.f, g_ry = 0.f;
   float* o = p.out + base;
   if (live) {
     const size_t jb = ((size_t)b * L + f) * 66;
-    // FC without joint targets: the joint term is zero (its mask reads as all-false)
-    const bool jt = !FC || p.mask;
+    // FC / OB without joint targets: the joint term is zero (its mask reads as all-false)
+    const bool jt = !(FC || OB) || p.mask;
     const float* tg = jt ? p.target + jb : nullptr;
     const uint8_t* mk = jt ? p.mask + jb : nullptr;
     auto on = [&](int i) { return jt && mk[i]; };
     g_rx = on(0) ? __fmul_rn(2.f, __fsub_rn(rx, tg[0])) : 0.f;
     g_ry = on(1) ? __fmul_rn(2.f, __fsub_rn(d3, tg[1])) : 0.f;
     g_rz = on(2) ? __fmul_rn(2.f, __fsub_rn(rz, tg[2])) : 0.f;
-    if constexpr (FC) {
-      g_rx = comb(g_rx, 0.f);
-      g_ry = comb(g_ry, 0.f);
-      g_rz = comb(g_rz, 0.f);
+    if constexpr (FC || OB) {
+      float ox = 0.f, oz = 0.f;
+      if (in_s(0)) obstacle_grad(rx, rz, ox, oz);
+      g_rx = comb(g_rx, 0.f, ox);
+      g_ry = comb(g_ry, 0.f, 0.f);
+      g_rz = comb(g_rz, 0.f, oz);
     }
     for (int j = 1; j < 22; ++j) {
       const int c0 = 4 + 3 * (j - 1);
@@ -249,11 +285,13 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
       float gx = on(3 * j) ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(xo, rx), tg[3 * j])) : 0.f;
       float gy = on(3 * j + 1) ? __fmul_rn(2.f, __fsub_rn(ly, tg[3 * j + 1])) : 0.f;
       float gz = on(3 * j + 2) ? __fmul_rn(2.f, __fsub_rn(__fadd_rn(zo, rz), tg[3 * j + 2])) : 0.f;
-      if constexpr (FC) {
-        const int k = foot_index(j);
-        gx = comb(gx, k >= 0 ? contact_grad(k, 0) : 0.f);
-        gy = comb(gy, k >= 0 ? contact_grad(k, 1) : 0.f);
-        gz = comb(gz, k >= 0 ? contact_grad(k, 2) : 0.f);
+      if constexpr (FC || OB) {
+        const int k = FC ? foot_index(j) : -1;
+        float ox = 0.f, oz = 0.f;
+        if (in_s(j)) obstacle_grad(__fadd_rn(xo, rx), __fadd_rn(zo, rz), ox, oz);
+        gx = comb(gx, k >= 0 ? contact_grad(k, 0) : 0.f, ox);
+        gy = comb(gy, k >= 0 ? contact_grad(k, 1) : 0.f, 0.f);
+        gz = comb(gz, k >= 0 ? contact_grad(k, 2) : 0.f, oz);
       }
       o[(long long)c0 * p.sc] = __fmul_rn(__fadd_rn(__fmul_rn(gx, C2), __fmul_rn(gz, S2)), p.stdv[c0]);
       o[(long long)(c0 + 1) * p.sc] = __fmul_rn(gy, p.stdv[c0 + 1]);
@@ -306,6 +344,17 @@ __global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p
     const int ff = i / nz, c = kJointChannels + i % nz;
     ob[(long long)ff * p.sf + (long long)c * p.sc] = 0.f;
   }
+}
+
+template <bool FC>
+__global__ void __launch_bounds__(256) joint_seed_kernel(const JointSeedParams p) {
+  joint_seed<FC, false>(p);
+}
+
+// The joint seed with obstacle-avoidance guidance (and foot-contact guidance when FC).
+template <bool FC>
+__global__ void __launch_bounds__(256) obstacle_seed_kernel(const JointSeedParams p) {
+  joint_seed<FC, true>(p);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -412,9 +461,18 @@ cudaError_t launch_guidance_seed(const GuidanceSeedParams& p, cudaStream_t strea
 cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream) {
   if (p.L < 1 || p.L > 256 || p.D < kJointChannels || p.out_cols < kJointChannels) return cudaErrorInvalidValue;
   if (p.contact && (p.D < kContactChannel + 4 || (p.step_ptr && !p.coef))) return cudaErrorInvalidValue;
+  if (p.obstacle && (p.n_obstacles < 0 || p.n_obstacles > kMaxObstacles || (p.n_obstacles > 0 && !p.obstacles) ||
+                     (p.obstacle_joints >> 22) != 0 || (p.step_ptr && !p.coef)))
+    return cudaErrorInvalidValue;
   if (p.B == 0) return cudaSuccess;
-  if (p.contact) joint_seed_kernel<true><<<p.B, 256, 0, stream>>>(p);
-  else joint_seed_kernel<false><<<p.B, 256, 0, stream>>>(p);
+  if (p.obstacle) {
+    if (p.contact) obstacle_seed_kernel<true><<<p.B, 256, 0, stream>>>(p);
+    else obstacle_seed_kernel<false><<<p.B, 256, 0, stream>>>(p);
+  } else if (p.contact) {
+    joint_seed_kernel<true><<<p.B, 256, 0, stream>>>(p);
+  } else {
+    joint_seed_kernel<false><<<p.B, 256, 0, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 

@@ -46,6 +46,7 @@ namespace {
 constexpr int kDModel = 512;
 constexpr int kBnWide = 256;    // QKV, FFN1
 constexpr int kBnNarrow = 128;  // N = 512 / 264 outputs: more tiles per wave
+static_assert(CMDI_MAX_OBSTACLES == kMaxObstacles, "the C ABI's obstacle limit is the seed kernel's");
 constexpr int kMaxT = 5000;     // entries of the per-step coefficient tables (step indices and original timesteps)
 constexpr const char* kUnetGuidancePrecision =
     "reconstruction guidance (the denoiser's input-VJP) is implemented for the transformer denoiser and, at "
@@ -105,6 +106,8 @@ struct GraphKey {
                                    // arguments); its targets and coefficients live in device memory
   int passes;                      // denoiser passes per evaluation (Passes::n): keyframe CFG adds one
   int contact;                     // foot-contact guidance (the joint seed's FC instance); joint: joint targets
+  int obstacle, n_obstacles;       // obstacle-avoidance guidance (the obstacle seed instance) and its obstacles per sample
+  uint32_t obstacle_joints;        // its joint set S (a launch argument of the seed)
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
 };
 
@@ -121,12 +124,14 @@ struct Passes {
   bool combine() const { return n > 1; }
 };
 
-// The joint seed of a call's guided evaluations (joint-position guidance, foot-contact guidance or both): whether it
-// runs, whether it adds the foot-contact term, whether it reads joint_target / joint_mask, and the root representation.
-// Its targets, statistics and coefficients live in the engine's buffers (the step graphs read them there).
+// The joint seed of a call's guided evaluations (joint-position, foot-contact and obstacle-avoidance guidance, in any
+// combination): whether it runs, whether it adds the foot-contact term, whether it adds the obstacle term (with K
+// obstacles per sample and the joint set S), whether it reads joint_target / joint_mask, and the root representation.
+// Its targets, obstacles, statistics and coefficients live in the engine's buffers (the step graphs read them there).
 struct Guidance {
-  bool joint = false, contact = false, targets = false;
-  int abs3d = 0;
+  bool joint = false, contact = false, targets = false, obstacle = false;
+  int abs3d = 0, n_obstacles = 0;
+  uint32_t obstacle_joints = 0;
 };
 
 // One op of a RePaint walk: denoise at p (the position moves p -> p - 1) or undo into p (p - 1 -> p).
@@ -207,8 +212,11 @@ struct cmdi_engine {
   std::vector<float> h_seed_coef;
   // foot-contact guidance (cmdi_sample_args.foot_contact): the joint seed's FC instance applies (c_j, c_c) itself
   uint8_t* contact_valid = nullptr;  // (maxB, L) frame validity
-  float* contact_coef = nullptr;     // [kMaxT][2] (c_j, c_c) per step index
+  float* contact_coef = nullptr;     // [kMaxT][2] (c_j, c_c) per step index; [kMaxT][3] (c_j, c_c, c_o) with obstacles
   std::vector<float> h_contact_coef;
+  // obstacle-avoidance guidance (cmdi_sample_args.obstacle_guidance): the joint seed's obstacle instance applies c_o
+  float* obstacle_buf = nullptr;     // (maxB, kMaxObstacles, 3) (c_x, c_z, r), K per sample as the call gives them
+  uint8_t* obstacle_valid = nullptr; // (maxB, L) frame validity
   // forward path with LayerNorm folded into the consuming linear layers and the linear layers of a layer chained into one
   // persistent launch (gemm_chain.cu).  CMDI_CHAIN=0 selects the round-1 path (one launch per layer + LayerNorm kernels),
   // which guided steps (they stash LayerNorm inputs for the backward pass) always use.
@@ -695,6 +703,11 @@ int run_joint_seed(cmdi_engine* e, int B, const Passes& ps, const Guidance& g, c
     if (!g.targets) { jp.target = nullptr; jp.mask = nullptr; }
     jp.contact = 1; jp.valid = e->contact_valid; jp.coef = e->contact_coef; jp.step_ptr = e->step_ctr;
   }
+  if (g.obstacle) {
+    if (!g.targets) { jp.target = nullptr; jp.mask = nullptr; }
+    jp.obstacle = 1; jp.obstacles = e->obstacle_buf; jp.n_obstacles = g.n_obstacles; jp.obstacle_joints = g.obstacle_joints;
+    jp.obstacle_valid = e->obstacle_valid; jp.coef = e->contact_coef; jp.step_ptr = e->step_ctr;
+  }
   CK(launch_joint_seed(jp, s));
   return 0;
 }
@@ -709,7 +722,9 @@ int ensure_joint(cmdi_engine* e) {
   CKI(dev_alloc(e, &e->seed_coef, (size_t)2 * kMaxT));
   CKI(dev_alloc(e, &e->unit_coef, (size_t)kMaxT));
   CKI(dev_alloc(e, &e->contact_valid, (size_t)e->maxB * e->L));
-  CKI(dev_alloc(e, &e->contact_coef, (size_t)2 * kMaxT));
+  CKI(dev_alloc(e, &e->contact_coef, (size_t)3 * kMaxT));
+  CKI(dev_alloc(e, &e->obstacle_buf, (size_t)e->maxB * kMaxObstacles * 3));
+  CKI(dev_alloc(e, &e->obstacle_valid, (size_t)e->maxB * e->L));
   const std::vector<float> ones(kMaxT, 1.f);
   CK(cudaMemcpy(e->unit_coef, ones.data(), ones.size() * 4, cudaMemcpyHostToDevice));
   return 0;
@@ -1659,7 +1674,8 @@ StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool gui
   sp.model_out = e->model_out; sp.cfg = ps.combine(); sp.text_scale = ps.scale; sp.keyframe_scale = ps.kf_scale;
   sp.x_t = e->x_state; sp.impute = a->imputate != 0; sp.stop_imputation_at = a->stop_imputation_at;
   sp.x_obs = e->x_obs; sp.obs_mask = e->obs_mask;
-  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance || a->foot_contact ? e->unit_coef : e->guide_coef;
+  sp.guided = guided; sp.guide_grad = e->guide_grad; sp.guide_coef = a->joint_guidance || a->foot_contact || a->obstacle_guidance ? e->unit_coef
+                                                                                                      : e->guide_coef;
   sp.x_next = e->x_state; sp.x_next_hi = e->x_state_p.hi; sp.x_next_lo = e->nsplit == 3 ? e->x_state_p.lo : nullptr;
   sp.pred_xstart = e->pred_x0;
   sp.win_K = a->window_count; sp.win_N = a->global_frames; sp.win_f0 = e->win_f0;
@@ -1689,7 +1705,10 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.win_K = a->window_count; key.win_N = a->global_frames;
   key.joint = a->joint_guidance != 0;
   key.contact = a->foot_contact != 0;
-  key.joint_abs3d = (key.joint || key.contact) && a->joint_abs3d != 0;
+  key.obstacle = a->obstacle_guidance != 0;
+  key.n_obstacles = key.obstacle ? a->n_obstacles : 0;
+  key.obstacle_joints = key.obstacle ? a->obstacle_joints : 0u;
+  key.joint_abs3d = (key.joint || key.contact || key.obstacle) && a->joint_abs3d != 0;
   key.passes = 1 + (a->cfg ? 1 : 0) + (a->keyframe_scale ? 1 : 0);
   if (a->sampler != CMDI_SAMPLER_PLMS) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
@@ -1884,7 +1903,7 @@ int check_sample_args(const cmdi_engine* e, const cmdi_sample_args* a) {
     set_last_error("reconstruction_guidance needs recon_coef");
     return 1;
   }
-  if (a->joint_guidance || a->foot_contact) {
+  if (a->joint_guidance || a->foot_contact || a->obstacle_guidance) {
     if (a->joint_guidance && (!a->joint_coef || !a->joint_target || !a->joint_mask || !a->joint_mean || !a->joint_std)) {
       set_last_error("joint_guidance needs joint_coef, joint_target, joint_mask, joint_mean and joint_std");
       return 1;
@@ -1893,7 +1912,21 @@ int check_sample_args(const cmdi_engine* e, const cmdi_sample_args* a) {
       set_last_error("foot_contact needs foot_contact_coef, joint_mean and joint_std");
       return 1;
     }
-    const char* what = a->joint_guidance ? "joint-position guidance" : "foot-contact guidance";
+    if (a->obstacle_guidance && (!a->obstacle_coef || !a->joint_mean || !a->joint_std)) {
+      set_last_error("obstacle_guidance needs obstacle_coef, joint_mean and joint_std");
+      return 1;
+    }
+    if (a->obstacle_guidance && (a->n_obstacles < 0 || a->n_obstacles > kMaxObstacles || (a->n_obstacles > 0 && !a->obstacles))) {
+      set_last_error("obstacle_guidance needs 0 <= n_obstacles <= %d obstacles per sample (got %d) and obstacles when "
+                     "n_obstacles > 0", kMaxObstacles, a->n_obstacles);
+      return 1;
+    }
+    if (a->obstacle_guidance && (a->obstacle_joints == 0 || (a->obstacle_joints >> 22) != 0)) {
+      set_last_error("obstacle_joints 0x%x must name at least one of the 22 joints (bits 0 .. 21)", a->obstacle_joints);
+      return 1;
+    }
+    const char* what = a->joint_guidance ? "joint-position guidance"
+                       : a->foot_contact ? "foot-contact guidance" : "obstacle-avoidance guidance";
     if (e->D != 263) {
       set_last_error("%s needs HumanML3D's 263 features (22 joints), the engine has njoints = %d", what, e->D);
       return 1;
@@ -1962,10 +1995,12 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
   const int B = a->batch;
   const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
   const bool host = a->host_buffers != 0;
-  const bool contact = a->foot_contact != 0;
-  // the joint seed runs at guided evaluations: joint-position guidance, foot-contact guidance or both
+  const bool contact = a->foot_contact != 0, obstacle = a->obstacle_guidance != 0;
+  // the joint seed runs at guided evaluations: joint-position, foot-contact or obstacle guidance, in any combination
   Guidance g;
-  g.joint = a->joint_guidance || contact; g.contact = contact; g.targets = a->joint_guidance != 0; g.abs3d = a->joint_abs3d != 0;
+  g.joint = a->joint_guidance || contact || obstacle; g.contact = contact; g.targets = a->joint_guidance != 0;
+  g.abs3d = a->joint_abs3d != 0;
+  g.obstacle = obstacle; g.n_obstacles = obstacle ? a->n_obstacles : 0; g.obstacle_joints = obstacle ? a->obstacle_joints : 0u;
   if (a->recon_guidance) {
     CKI(ensure_stash(e, s));
     if (!e->guide_coef) CK(cudaMalloc(&e->guide_coef, (size_t)5000 * 4));
@@ -1975,25 +2010,34 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
     CKI(ensure_stash(e, s));
     CKI(stage_joint(e, B, a->joint_guidance ? a->joint_target : nullptr, a->joint_guidance ? a->joint_mask : nullptr,
                     a->joint_mean, a->joint_std, s));
-    // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere.  With foot-contact guidance the
-    // joint seed applies (c_j, c_c) itself and the guidance seed's second coefficient is 1.
+    // (c_r, c_j) per step index: each term's coefficient where it applies, 0 elsewhere.  With foot-contact or obstacle
+    // guidance the joint seed applies (c_j, c_c) or (c_j, c_c, c_o) itself and the guidance seed's second coefficient is 1.
+    const int stride = obstacle ? 3 : 2;
     e->h_seed_coef.assign((size_t)2 * e->T, 0.f);
-    e->h_contact_coef.assign((size_t)2 * e->T, 0.f);
+    e->h_contact_coef.assign((size_t)stride * e->T, 0.f);
     for (int t = 0; t < e->T; ++t) {
       const float cj = a->joint_guidance && t >= a->stop_jointguidance_at ? a->joint_coef[t] : 0.f;
       if (a->recon_guidance && t >= a->stop_recguidance_at) e->h_seed_coef[2 * t] = a->recon_coef[t];
       if (a->joint_guidance && t >= a->stop_jointguidance_at) e->h_seed_coef[2 * t + 1] = a->joint_coef[t];
-      if (contact) {
+      if (contact || obstacle) {
         e->h_seed_coef[2 * t + 1] = 1.f;
-        e->h_contact_coef[2 * t] = cj;
-        if (t >= a->stop_footcontact_at) e->h_contact_coef[2 * t + 1] = a->foot_contact_coef[t];
+        e->h_contact_coef[stride * t] = cj;
+        if (contact && t >= a->stop_footcontact_at) e->h_contact_coef[stride * t + 1] = a->foot_contact_coef[t];
+        if (obstacle && t >= a->stop_obstacleguidance_at) e->h_contact_coef[stride * t + 2] = a->obstacle_coef[t];
       }
     }
     CK(cudaMemcpyAsync(e->seed_coef, e->h_seed_coef.data(), e->h_seed_coef.size() * 4, cudaMemcpyHostToDevice, s));
-    if (contact) {
+    if (contact || obstacle)
       CK(cudaMemcpyAsync(e->contact_coef, e->h_contact_coef.data(), e->h_contact_coef.size() * 4, cudaMemcpyHostToDevice, s));
+    if (contact) {
       if (a->foot_contact_mask) CK(cudaMemcpyAsync(e->contact_valid, a->foot_contact_mask, (size_t)B * e->L, cudaMemcpyDefault, s));
       else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
+    }
+    if (obstacle) {
+      if (a->n_obstacles > 0)
+        CK(cudaMemcpyAsync(e->obstacle_buf, a->obstacles, (size_t)B * a->n_obstacles * 3 * 4, cudaMemcpyDefault, s));
+      if (a->obstacle_mask) CK(cudaMemcpyAsync(e->obstacle_valid, a->obstacle_mask, (size_t)B * e->L, cudaMemcpyDefault, s));
+      else CK(cudaMemsetAsync(e->obstacle_valid, 1, (size_t)B * e->L, s));
     }
   }
   const size_t n = (size_t)B * e->D * e->L;
@@ -2195,10 +2239,10 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
   };
   int dump_i = 0;
   // utils/editing_util.py:325-333: guidance is active while t >= stop_recguidance_at (t is uniform over the batch); a step
-  // is guided when reconstruction, joint or foot-contact guidance is active at it
+  // is guided when reconstruction, joint, foot-contact or obstacle guidance is active at it
   auto guided_t = [&](int t) {
     return (a->recon_guidance && t >= a->stop_recguidance_at) || (a->joint_guidance && t >= a->stop_jointguidance_at) ||
-           (contact && t >= a->stop_footcontact_at);
+           (contact && t >= a->stop_footcontact_at) || (obstacle && t >= a->stop_obstacleguidance_at);
   };
   auto guided_at = [&](int k) { return guided_t(sm.ascends ? t0 + k : t0 - k); };
   // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
@@ -2310,13 +2354,19 @@ extern "C" int cmdi_test_step(cmdi_engine* e, int sampler, float eta, int t, int
 
 namespace {
 
-// The joint term of a guided evaluation's seed: joint-position guidance (contact 0) or foot-contact guidance (contact 1;
-// target / mask may then be null), with the coefficients (c_r, c_j, c_c) of one step index.
+// The joint term of a guided evaluation's seed: joint-position guidance (contact 0), foot-contact guidance (contact 1;
+// target / mask may then be null) and obstacle guidance (obstacle 1; target / mask may then be null; valid is the frame
+// mask of both terms), with the coefficients (c_r, c_j, c_c, c_o) of one step index.
 struct JointVjp {
   float c_r, c_j, c_c;
   const float *target, *mean, *stdv;
   const uint8_t *mask, *valid;
   int abs3d, contact;
+  int obstacle = 0;
+  float c_o = 0.f;
+  const float* obstacles = nullptr;
+  int n_obstacles = 0;
+  uint32_t obstacle_joints = 0;
 };
 
 // One (CFG: batch-doubled) evaluation of the guided pass and its input-VJP, as a guided sampling step runs them: the seed
@@ -2327,7 +2377,8 @@ struct JointVjp {
 int input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion, const uint8_t* inpainting_mask,
               const JointVjp* j, float* grad, void* stream_, const char* fn) {
   if (!e || !a || !a->x || !grad || a->host_buffers || (!inpainted_motion) != (!inpainting_mask) ||
-      (j ? !j->mean || !j->stdv || (!j->contact && !j->target) || (!j->target) != (!j->mask) : !inpainted_motion)) {
+      (j ? !j->mean || !j->stdv || (!j->contact && !j->obstacle && !j->target) || (!j->target) != (!j->mask)
+         : !inpainted_motion)) {
     set_last_error("%s: null argument or host buffers", fn);
     return 1;
   }
@@ -2341,7 +2392,14 @@ int input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted
   }
   if (j && e->D != 263) {
     set_last_error("%s needs HumanML3D's 263 features (22 joints), the engine has njoints = %d",
-                   j->contact ? "foot-contact guidance" : "joint-position guidance", e->D);
+                   j->obstacle ? "obstacle-avoidance guidance" : j->contact ? "foot-contact guidance" : "joint-position guidance",
+                   e->D);
+    return 1;
+  }
+  if (j && j->obstacle && (j->n_obstacles < 0 || j->n_obstacles > kMaxObstacles || (j->n_obstacles > 0 && !j->obstacles) ||
+                           j->obstacle_joints == 0 || (j->obstacle_joints >> 22) != 0)) {
+    set_last_error("%s: needs 0 <= n_obstacles <= %d (got %d), obstacles when n_obstacles > 0 and obstacle_joints naming "
+                   "at least one of the 22 joints (got 0x%x)", fn, kMaxObstacles, j->n_obstacles, j->obstacle_joints);
     return 1;
   }
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
@@ -2352,12 +2410,22 @@ int input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted
   CKI(ensure_stash(e, s));
   if (j) {
     g.joint = true; g.contact = j->contact != 0; g.targets = j->target != nullptr; g.abs3d = j->abs3d != 0;
+    g.obstacle = j->obstacle != 0; g.n_obstacles = j->n_obstacles; g.obstacle_joints = j->obstacle_joints;
     CKI(stage_joint(e, B, j->target, j->mask, j->mean, j->stdv, s));
-    const float coef[2] = {j->c_r, j->contact ? 1.f : j->c_j};
+    const float coef[2] = {j->c_r, j->contact || j->obstacle ? 1.f : j->c_j};
     CK(cudaMemcpy(e->seed_coef + 2 * a->timestep, coef, sizeof(coef), cudaMemcpyHostToDevice));
-    if (j->contact) {
+    if (j->obstacle) {
+      const float cc[3] = {j->c_j, j->c_c, j->c_o};
+      CK(cudaMemcpy(e->contact_coef + 3 * a->timestep, cc, sizeof(cc), cudaMemcpyHostToDevice));
+      if (j->n_obstacles > 0)
+        CK(cudaMemcpyAsync(e->obstacle_buf, j->obstacles, (size_t)B * j->n_obstacles * 3 * 4, cudaMemcpyDeviceToDevice, s));
+      if (j->valid) CK(cudaMemcpyAsync(e->obstacle_valid, j->valid, (size_t)B * e->L, cudaMemcpyDeviceToDevice, s));
+      else CK(cudaMemsetAsync(e->obstacle_valid, 1, (size_t)B * e->L, s));
+    } else if (j->contact) {
       const float cc[2] = {j->c_j, j->c_c};
       CK(cudaMemcpy(e->contact_coef + 2 * a->timestep, cc, sizeof(cc), cudaMemcpyHostToDevice));
+    }
+    if (j->contact) {
       if (j->valid) CK(cudaMemcpyAsync(e->contact_valid, j->valid, (size_t)B * e->L, cudaMemcpyDeviceToDevice, s));
       else CK(cudaMemsetAsync(e->contact_valid, 1, (size_t)B * e->L, s));
     }
@@ -2409,6 +2477,21 @@ extern "C" int cmdi_test_foot_contact_input_vjp(cmdi_engine* e, const cmdi_forwa
   return input_vjp(e, a, inpainted_motion, inpainting_mask, &j, grad, stream_, "cmdi_test_foot_contact_input_vjp");
 }
 
+// cmdi_test_foot_contact_input_vjp with the obstacle term: the seed c_r G + (c_j G_j + c_c G_c + c_o G_o), as an
+// obstacle-guided sampling step at a step index whose coefficients are (c_r, c_j, c_c, c_o) forms it (c_c and G_c only
+// with foot_contact).
+extern "C" int cmdi_test_obstacle_input_vjp(cmdi_engine* e, const cmdi_forward_args* a, const float* inpainted_motion,
+                                            const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                            const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                            int joint_abs3d, float c_j, const uint8_t* valid, int foot_contact, float c_c,
+                                            const float* obstacles, int n_obstacles, uint32_t obstacle_joints, float c_o,
+                                            float* grad, void* stream_) {
+  JointVjp j{c_r, c_j, foot_contact ? c_c : 0.f, joint_target, joint_mean, joint_std, joint_mask, valid, joint_abs3d,
+             foot_contact != 0};
+  j.obstacle = 1; j.c_o = c_o; j.obstacles = obstacles; j.n_obstacles = n_obstacles; j.obstacle_joints = obstacle_joints;
+  return input_vjp(e, a, inpainted_motion, inpainting_mask, &j, grad, stream_, "cmdi_test_obstacle_input_vjp");
+}
+
 extern "C" int cmdi_joint_guidance_seed(const float* x0, int B, int D, int L, int ld, const float* target, const uint8_t* mask,
                                         const float* mean, const float* std, int abs_3d, float* grad, void* stream_) {
   if (!x0 || !target || !mask || !mean || !std || !grad || B < 0 || D < kJointChannels || L < 1 || L > 256 ||
@@ -2446,6 +2529,33 @@ extern "C" int cmdi_foot_contact_seed(const float* x0, int B, int D, int L, int 
   }
   jp.target = target; jp.mask = mask; jp.mean = mean; jp.stdv = std; jp.abs_3d = abs_3d != 0; jp.out = grad;
   jp.contact = 1; jp.valid = valid; jp.c_j = c_j; jp.c_c = c_c;
+  CK(launch_joint_seed(jp, reinterpret_cast<cudaStream_t>(stream_)));
+  return 0;
+}
+
+extern "C" int cmdi_obstacle_seed(const float* x0, int B, int D, int L, int ld, const uint8_t* valid, const float* target,
+                                  const uint8_t* mask, const float* mean, const float* std, int abs_3d, float c_j,
+                                  int foot_contact, float c_c, const float* obstacles, int n_obstacles,
+                                  uint32_t obstacle_joints, float c_o, float* grad, void* stream_) {
+  if (!x0 || !mean || !std || !grad || (!target) != (!mask) || B < 0 || D < (foot_contact ? kContactChannel + 4 : kJointChannels) ||
+      L < 1 || L > 256 || (ld != 0 && ld < D) || n_obstacles < 0 || n_obstacles > kMaxObstacles ||
+      (n_obstacles > 0 && !obstacles) || obstacle_joints == 0 || (obstacle_joints >> 22) != 0) {
+    set_last_error("cmdi_obstacle_seed: bad arguments (need non-null x0, mean, std and grad, target and mask both or "
+                   "neither, D >= 67 (263 with foot_contact), 1 <= L <= 256, ld 0 or >= D, 0 <= n_obstacles <= %d with "
+                   "obstacles when n_obstacles > 0, obstacle_joints naming at least one of the 22 joints)", kMaxObstacles);
+    return 1;
+  }
+  JointSeedParams jp{};
+  jp.B = B; jp.L = L; jp.D = D; jp.x0 = x0;
+  if (ld) {
+    jp.sb = (long long)L * ld; jp.sf = ld; jp.sc = 1; jp.out_cols = ld;
+  } else {
+    jp.sb = (long long)D * L; jp.sf = 1; jp.sc = L; jp.out_cols = D;
+  }
+  jp.target = target; jp.mask = mask; jp.mean = mean; jp.stdv = std; jp.abs_3d = abs_3d != 0; jp.out = grad;
+  jp.contact = foot_contact != 0; jp.valid = valid; jp.c_j = c_j; jp.c_c = foot_contact ? c_c : 0.f;
+  jp.obstacle = 1; jp.obstacles = obstacles; jp.n_obstacles = n_obstacles; jp.obstacle_joints = obstacle_joints;
+  jp.obstacle_valid = valid; jp.c_o = c_o;
   CK(launch_joint_seed(jp, reinterpret_cast<cudaStream_t>(stream_)));
   return 0;
 }

@@ -506,11 +506,23 @@ struct JointSeedParams {
   // term is off.  contact == 0: out = G_j, unscaled (the fields below are not read).
   int contact;
   const uint8_t* valid;       // (B, L) frame validity bytes (y['mask']), or null: every frame valid
-  const float* coef;          // [T][2] (c_j, c_c) per step index
+  const float* coef;          // [T][2] (c_j, c_c) per step index; [T][3] (c_j, c_c, c_o) with obstacle guidance
   const int* step_ptr;
   float c_j, c_c;
+  // obstacle-avoidance guidance (obstacle != 0): out = c_j G_j (+ c_c G_c) + c_o G_o, where G_o = d/dx0_hat of
+  //   L_o = (1 / L) sum_{f, j in S, k} m_o(f) max(r_k - |(P_j^x(f), P_j^z(f)) - (c_x, c_z)_k|, 0)
+  // with S the joints of obstacle_joints and m_o = obstacle_valid, and torch's subgradients: at distance 0 the joint gets
+  // 0 from that obstacle, at distance r_k it gets -(P - c) / r_k / L.  Radius-0 rows contribute exact zeros.  The
+  // coefficients come from coef[3 t .. 3 t + 2] (c_c read only with contact) or (c_j, c_c, c_o) when step_ptr is null.
+  int obstacle;
+  const float* obstacles;     // (B, n_obstacles, 3): (c_x, c_z, r) per obstacle
+  int n_obstacles;            // 0 .. kMaxObstacles
+  uint32_t obstacle_joints;   // bit j: joint j is in S (bits 0 .. 21)
+  const uint8_t* obstacle_valid;  // (B, L) frame validity bytes, or null: every frame valid
+  float c_o;
 };
 constexpr int kContactChannel = 259;  // HumanML3D's foot-contact labels: channels 259 .. 262 for joints 7, 10, 8, 11
+constexpr int kMaxObstacles = 16;     // obstacles per sample of obstacle guidance (staged in shared memory)
 cudaError_t launch_joint_seed(const JointSeedParams& p, cudaStream_t stream);
 cudaError_t launch_layernorm512_bwd(const float* dy, const float* v, const float* gamma, float eps, int rows, float* dv,
                                     __nv_bfloat16* dv_hi, __nv_bfloat16* dv_lo, cudaStream_t stream);

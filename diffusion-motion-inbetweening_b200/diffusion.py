@@ -24,7 +24,9 @@ Not accelerated (raise NotImplementedError, like the reference does for its own 
 cond_fn / 'gmd' classifier guidance, learned variances, EPSILON/PREVIOUS_X parametrisations,
 const_noise.  `reconstruction_guidance` runs a backward pass through the denoiser on the GPU (csrc/backward.cu), and
 `joint_guidance` (not in the reference) adds a loss on world-space joint positions to the same update (JointSpace), and
-`foot_contact_guidance` (not in the reference) one against foot sliding on the frames x0 marks as in contact.
+`foot_contact_guidance` (not in the reference) one against foot sliding on the frames x0 marks as in contact, and
+`obstacle_guidance` GMD's obstacle avoidance (sample/gmd/condition.py, CondKeyLocationsWithSdf's collision term) as a
+fourth loss on the same update.
 """
 from __future__ import annotations
 
@@ -132,7 +134,13 @@ class JointSpace:
       L_c = sum_{b, f, k} kappa(b, f, k) m(b, f) m(b, f + 1) |P_{J_k}(f + 1) - P_{J_k}(f)|^2,
       kappa(b, f, k) = [channel 259 + k of x0^T * std + mean > 0.5] (a constant), m = y['mask']
     with the coefficient w_c[t] * foot_contact_weight * sqrt(alpha_bar_t) / 2 (w_c = get_gradient_schedule(
-    y['foot_contact_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_footcontact_at']."""
+    y['foot_contact_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_footcontact_at'].
+
+    With y['obstacle_guidance'] set, every guided step also adds, with obstacles (c_x, c_z, r_k) = y['obstacles'] and S
+    the joints y['obstacle_joints'] (default (0,), the pelvis, as GMD),
+      L_o = sum_b (1 / L) sum_{f, j in S, k} m(b, f) max(r_k - |(P_j^x, P_j^z)(b, f) - (c_x, c_z)_k|, 0),  m = y['mask']
+    with the coefficient w_o[t] * obstacle_weight * sqrt(alpha_bar_t) / 2 (w_o = get_gradient_schedule(
+    y['obstacle_gradient_schedule'], y['diffusion_steps'])) while t >= y['stop_obstacleguidance_at']."""
     mean: torch.Tensor = field(repr=False)
     std: torch.Tensor = field(repr=False)
     abs_3d: bool = True
@@ -184,7 +192,7 @@ def _joint_guidance_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, 
 
 
 def _check_joint_space(space, D, window, what) -> None:
-    """The refusals joint-position and foot-contact guidance share, raised before any launch."""
+    """The refusals joint-position, foot-contact and obstacle guidance share, raised before any launch."""
     if space is None:
         raise NotImplementedError(f"{what} needs diffusion.joint_space (a JointSpace: the dataset statistics and abs_3d)")
     if not isinstance(space, JointSpace):
@@ -220,6 +228,79 @@ def _foot_contact_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, wi
     return dict(foot_contact=True, stop_footcontact_at=int(stop), foot_contact_coef=(w_c * sab / 2).float().numpy(),
                 foot_contact_mask=valid, joint_mean=space.mean.to(device), joint_std=space.std.to(device),
                 joint_abs3d=bool(space.abs_3d))
+
+
+MAX_OBSTACLES = capi.MAX_OBSTACLES
+
+
+def _obstacles_tensor(obstacles, B: int) -> torch.Tensor:
+    """y['obstacles'] as a (B, K, 3) fp32 CPU tensor of (c_x, c_z, r): a (B, K, 3) tensor, or GMD's obs_list
+    [((c_x, c_z), r), ...] shared by the batch.  Refuses K > MAX_OBSTACLES, r < 0 and non-finite values."""
+    if isinstance(obstacles, torch.Tensor):
+        if not obstacles.is_floating_point() or obstacles.dim() != 3 or obstacles.shape[0] != B or obstacles.shape[2] != 3:
+            raise ValueError(f"y['obstacles'] must be a float tensor of shape ({B}, K, 3) (c_x, c_z, r), got "
+                             f"{obstacles.dtype} {tuple(obstacles.shape)}")
+        obs = obstacles.detach().to(device="cpu", dtype=torch.float32)
+    elif isinstance(obstacles, (list, tuple)):
+        rows = []
+        for o in obstacles:
+            try:
+                (cx, cz), r = o
+                rows.append([float(cx), float(cz), float(r)])
+            except (TypeError, ValueError):
+                raise ValueError(f"y['obstacles'] as a list holds ((c_x, c_z), r) per obstacle (GMD's obs_list), got {o!r}")
+        obs = torch.tensor(rows, dtype=torch.float32).reshape(1, len(rows), 3).expand(B, -1, -1)
+    else:
+        raise ValueError(f"y['obstacles'] must be a ({B}, K, 3) tensor or a list of ((c_x, c_z), r), got {type(obstacles)}")
+    if obs.shape[1] > MAX_OBSTACLES:
+        raise ValueError(f"obstacle guidance takes at most {MAX_OBSTACLES} obstacles per sample, got {obs.shape[1]}")
+    if not bool(torch.isfinite(obs).all()):
+        raise ValueError("y['obstacles'] holds a non-finite value")
+    if bool((obs[..., 2] < 0).any()):
+        raise ValueError("y['obstacles'] holds a negative radius (r = 0 marks a padding row)")
+    return obs.contiguous()
+
+
+def _obstacle_joint_mask(joints) -> int:
+    """y['obstacle_joints'] (distinct joint indices in [0, 22)) as the engine's bit mask"""
+    if isinstance(joints, torch.Tensor):
+        joints = joints.tolist()
+    if not isinstance(joints, (list, tuple)) or not joints:
+        raise ValueError(f"y['obstacle_joints'] must be a non-empty sequence of joint indices in [0, 22), got {joints!r}")
+    mask = 0
+    for j in joints:
+        if isinstance(j, bool) or not isinstance(j, (int, np.integer)) or not 0 <= int(j) < 22 or (mask >> int(j)) & 1:
+            raise ValueError(f"y['obstacle_joints'] must hold distinct joint indices in [0, 22), got {joints!r}")
+        mask |= 1 << int(j)
+    return mask
+
+
+def _obstacle_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, window, device) -> dict:
+    """Engine arguments of y['obstacle_guidance'] (validated here, before any launch)."""
+    _check_joint_space(space, D, window, "obstacle guidance")
+    for k in ("obstacles", "obstacle_weight", "stop_obstacleguidance_at", "diffusion_steps"):
+        if k not in y:
+            raise ValueError(f"obstacle guidance needs y[{k!r}]")
+    weight, stop = y["obstacle_weight"], y["stop_obstacleguidance_at"]
+    if isinstance(weight, bool) or not isinstance(weight, (int, float, np.integer, np.floating)):
+        raise ValueError(f"y['obstacle_weight'] must be a number, got {weight!r}")
+    if isinstance(stop, bool) or not isinstance(stop, (int, np.integer)):
+        raise ValueError(f"y['stop_obstacleguidance_at'] must be an int, got {stop!r}")
+    obstacles = _obstacles_tensor(y["obstacles"], B)
+    joints = _obstacle_joint_mask(y.get("obstacle_joints", (0,)))
+    valid = y.get("mask")
+    if valid is not None:
+        if not isinstance(valid, torch.Tensor) or valid.numel() != B * L:
+            raise ValueError(f"y['mask'] must hold one entry per frame ({B} x {L}), got {tuple(getattr(valid, 'shape', ()))}")
+        valid = valid.to(device).reshape(B, L).bool()
+    # w_o[t] * weight * sqrt(alpha_bar_t) / 2 in fp32, as reconstruction guidance forms its coefficient
+    ws = get_gradient_schedule(y.get("obstacle_gradient_schedule"), y["diffusion_steps"])
+    tt = torch.arange(num_timesteps)
+    w_o = torch.from_numpy(ws)[tt].float() * float(weight)
+    sab = torch.from_numpy(sqrt_alphas_cumprod)[tt].float()
+    return dict(obstacle_guidance=True, stop_obstacleguidance_at=int(stop), obstacle_coef=(w_o * sab / 2).float().numpy(),
+                obstacles=obstacles.to(device), obstacle_joints=joints, obstacle_mask=valid,
+                joint_mean=space.mean.to(device), joint_std=space.std.to(device), joint_abs3d=bool(space.abs_3d))
 
 
 def _crop_windows(x: torch.Tensor, f0: List[int], F: int) -> torch.Tensor:
@@ -363,6 +444,9 @@ class GaussianDiffusion:
         if y.get("foot_contact_guidance", False):
             joint.update(_foot_contact_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
                                             self.sqrt_alphas_cumprod, self.window, device))
+        if y.get("obstacle_guidance", False):
+            joint.update(_obstacle_args(self.joint_space, y, B, int(shape[1]), int(shape[-1]), self.num_timesteps,
+                                        self.sqrt_alphas_cumprod, self.window, device))
         rows = keyframe_cfg_max_batch(B * K, is_cfg) if kf_cfg else B * K  # keyframe CFG: its passes fit 2 * max_batch
         eng = inner.engine_for(device, max_batch=max(rows, self.max_batch or 0), precision=self.precision, nframes=F)
         eng.set_schedule(self.betas, self.timestep_map)

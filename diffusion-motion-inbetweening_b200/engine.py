@@ -132,7 +132,10 @@ class Engine:
                joint_target: Optional[torch.Tensor] = None, joint_mask: Optional[torch.Tensor] = None,
                joint_mean: Optional[torch.Tensor] = None, joint_std: Optional[torch.Tensor] = None, joint_abs3d: bool = False,
                keyframe_scale: Optional[torch.Tensor] = None, foot_contact: bool = False, stop_footcontact_at: int = 0,
-               foot_contact_coef: Optional[Sequence[float]] = None, foot_contact_mask: Optional[torch.Tensor] = None):
+               foot_contact_coef: Optional[Sequence[float]] = None, foot_contact_mask: Optional[torch.Tensor] = None,
+               obstacle_guidance: bool = False, stop_obstacleguidance_at: int = 0,
+               obstacle_coef: Optional[Sequence[float]] = None, obstacles: Optional[torch.Tensor] = None,
+               obstacle_joints: int = 1, obstacle_mask: Optional[torch.Tensor] = None):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -165,6 +168,10 @@ class Engine:
         foot_contact*: foot-contact guidance (cmdi_sample_args.foot_contact): foot_contact_coef one entry per sampler
         step, foot_contact_mask (batch, nframes) the valid frames or None; it reads joint_mean / joint_std / joint_abs3d,
         and joint_target / joint_mask only with joint_guidance.
+        obstacle_*: obstacle-avoidance guidance (cmdi_sample_args.obstacle_guidance): obstacle_coef one entry per sampler
+        step, obstacles (batch, K, 3) fp32 (c_x, c_z, r) with K <= capi.MAX_OBSTACLES, obstacle_joints the bit mask of
+        the joint set, obstacle_mask (batch, nframes) the valid frames or None; it reads joint_mean / joint_std /
+        joint_abs3d, and joint_target / joint_mask only with joint_guidance.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         K = 0 if window_frames0 is None else len(window_frames0)
@@ -232,6 +239,18 @@ class Engine:
             fcoef_arr = fcoef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
             foot_contact_mask = prep(foot_contact_mask, torch.uint8, (batch, self.nframes))
             joint_mean, joint_std = prep(joint_mean, shp=(self.njoints,)), prep(joint_std, shp=(self.njoints,))
+        ocoef_arr, n_obstacles = None, 0
+        if obstacle_guidance:
+            ocoef = np.ascontiguousarray(np.asarray(obstacle_coef, dtype=np.float32))
+            if ocoef.shape != (self.num_timesteps,):
+                raise ValueError(f"obstacle_coef must have one entry per sampler step ({self.num_timesteps})")
+            ocoef_arr = ocoef.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+            if obstacles is None or obstacles.dim() != 3 or obstacles.shape[0] != batch or obstacles.shape[2] != 3:
+                raise ValueError(f"obstacles must be ({batch}, K, 3), got {tuple(getattr(obstacles, 'shape', ()))}")
+            n_obstacles = int(obstacles.shape[1])
+            obstacles = prep(obstacles) if n_obstacles else None
+            obstacle_mask = prep(obstacle_mask, torch.uint8, (batch, self.nframes))
+            joint_mean, joint_std = prep(joint_mean, shp=(self.njoints,)), prep(joint_std, shp=(self.njoints,))
         n_iter = self.num_timesteps - int(skip_timesteps)
         if num_steps:
             n_iter = min(n_iter, int(num_steps))
@@ -268,6 +287,10 @@ class Engine:
             a.repaint_jump_length, a.repaint_jump_n_sample = int(repaint_jump_length), int(repaint_jump_n_sample)
         if foot_contact:
             a.foot_contact_mask = _ptr(foot_contact_mask)
+        if obstacle_guidance:
+            a.obstacle_guidance, a.stop_obstacleguidance_at, a.obstacle_coef = 1, int(stop_obstacleguidance_at), ocoef_arr
+            a.obstacles, a.n_obstacles, a.obstacle_joints = _ptr(obstacles), n_obstacles, int(obstacle_joints)
+            a.obstacle_mask = _ptr(obstacle_mask)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")
@@ -395,6 +418,42 @@ class Engine:
         """foot_contact_seed (cmdi_foot_contact_seed), the seed kernel alone"""
         return foot_contact_seed(*args, **kwargs)
 
+    def test_obstacle_input_vjp(self, x, timestep, joint_mean, joint_std, joint_abs3d, obstacles, c_o, obstacle_joints=1,
+                                valid=None, foot_contact=False, c_c=0.0, joint_target=None, joint_mask=None, c_j=0.0,
+                                inpainted_motion=None, inpainting_mask=None, c_r=0.0, cond_emb=None, uncond=False, cfg=False,
+                                text_scale=None, obs_x0=None, obs_mask=None, keyframe_scale=None) -> torch.Tensor:
+        """test_foot_contact_input_vjp with obstacle-avoidance guidance (cmdi_test_obstacle_input_vjp): the gradient of
+        c_r L_r + c_j L_j + c_c L_c + c_o L_o w.r.t. x through each pass, (passes, B, njoints, 1, nframes).  obstacles
+        (B, K, 3); obstacle_joints the bit mask of the joint set; valid (B, nframes): the valid frames of both the obstacle
+        and the foot-contact term (None: all); foot_contact False: no contact term; joint_target None: no joint term;
+        inpainted_motion None: no reconstruction term."""
+        dev = lambda t, dt=torch.float32: None if t is None else t.to(self.device, dt).contiguous()  # noqa: E731
+        x = dev(x)
+        B = x.shape[0]
+        cond_emb, text_scale, obs_x0, inpainted_motion = dev(cond_emb), dev(text_scale), dev(obs_x0), dev(inpainted_motion)
+        obs_mask, inpainting_mask = dev(obs_mask, torch.uint8), dev(inpainting_mask, torch.uint8)
+        joint_target, joint_mask, valid = dev(joint_target), dev(joint_mask, torch.uint8), dev(valid, torch.uint8)
+        joint_mean, joint_std, keyframe_scale, obstacles = dev(joint_mean), dev(joint_std), dev(keyframe_scale), dev(obstacles)
+        if valid is not None:
+            valid = valid.reshape(B, -1).contiguous()
+        K = int(obstacles.shape[1])
+        passes = 1 + int(bool(cfg)) + int(keyframe_scale is not None)
+        grad = torch.empty((passes,) + tuple(x.shape), dtype=torch.float32, device=self.device)
+        a = capi.ForwardArgs(B, _ptr(x), int(timestep), _ptr(cond_emb), int(uncond), int(cfg), _ptr(text_scale), 0,
+                             _ptr(obs_x0), _ptr(obs_mask), _ptr(keyframe_scale))
+        with torch.cuda.device(self.device):
+            capi.check(self.lib.cmdi_test_obstacle_input_vjp(
+                self._h, ctypes.byref(a), _ptr(inpainted_motion), _ptr(inpainting_mask), float(c_r), _ptr(joint_target),
+                _ptr(joint_mask), _ptr(joint_mean), _ptr(joint_std), int(joint_abs3d), float(c_j), _ptr(valid),
+                int(bool(foot_contact)), float(c_c), _ptr(obstacles) if K else None, K, int(obstacle_joints), float(c_o),
+                grad.data_ptr(), _stream_ptr(self.device)), "cmdi_test_obstacle_input_vjp")
+        return grad
+
+    @staticmethod
+    def obstacle_seed(*args, **kwargs) -> torch.Tensor:
+        """obstacle_seed (cmdi_obstacle_seed), the seed kernel alone"""
+        return obstacle_seed(*args, **kwargs)
+
     def test_unet_ops(self, hook, x, timestep, cond_emb=None, uncond=False, cfg=False, text_scale=None, obs_x0=None,
                       obs_mask=None, inpainted_motion=None, inpainting_mask=None) -> torch.Tensor:
         """MDM_UNET (cmdi_test_unet_ops): the forward Engine.forward runs, or with inpainted_motion / inpainting_mask the
@@ -479,4 +538,38 @@ def foot_contact_seed(x0: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, a
         capi.check(lib.cmdi_foot_contact_seed(_ptr(x0), B, D, L, int(ld), _ptr(valid), _ptr(target), _ptr(mask), _ptr(mean),
                                               _ptr(std), int(abs_3d), float(c_j), float(c_c), grad.data_ptr(), _stream_ptr(dev)),
                    "cmdi_foot_contact_seed")
+    return grad
+
+
+def obstacle_seed(x0: torch.Tensor, mean: torch.Tensor, std: torch.Tensor, abs_3d: bool, obstacles: torch.Tensor,
+                  obstacle_joints: int = 1, c_o: float = 1.0, valid: Optional[torch.Tensor] = None, foot_contact: bool = False,
+                  c_c: float = 0.0, target: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None,
+                  c_j: float = 0.0, ld: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """cmdi_obstacle_seed: c_j dL_j/dx0 + c_c dL_c/dx0 + c_o dL_o/dx0 on a CUDA device, L_o the obstacle loss
+    (cmdi_sample_args.obstacle_guidance) of obstacles (B, K, 3) (c_x, c_z, r) over the joints of the bit mask
+    obstacle_joints, with valid (B, L) the valid frames (None: all); L_c foot_contact_seed's loss when foot_contact (same
+    valid); L_j joint_guidance_seed's loss (target / mask None: no joint term).  Layouts as joint_guidance_seed."""
+    lib = capi.load()
+    dev = x0.device
+    if dev.type != "cuda":
+        raise RuntimeError("obstacle_seed runs on CUDA devices only (no CPU fallback)")
+    f = lambda t, dt=torch.float32: None if t is None else t.to(dev, dt).contiguous()  # noqa: E731
+    x0, mean, std, valid, target, mask = f(x0), f(mean), f(std), f(valid, torch.uint8), f(target), f(mask, torch.uint8)
+    obstacles = f(obstacles)
+    B, D = x0.shape[0], mean.shape[0]
+    L = x0.shape[1] if ld else x0.shape[-1]
+    want = (B, L, ld) if ld else (B, D, 1, L)
+    if (tuple(x0.shape) != want or std.shape != (D,) or (valid is not None and valid.numel() != B * L) or
+            obstacles.dim() != 3 or obstacles.shape[0] != B or obstacles.shape[2] != 3 or
+            (target is None) != (mask is None) or
+            (target is not None and (target.shape != (B, L, 22, 3) or mask.shape != (B, L, 22, 3)))):
+        raise ValueError("obstacle_seed: x0 must be (B, D, 1, L) (ld = 0) or (B, L, ld), mean / std (D,), obstacles "
+                         "(B, K, 3), valid B * L frames, and target / mask (B, L, 22, 3) both or neither")
+    K = int(obstacles.shape[1])
+    grad = torch.empty_like(x0) if out is None else out
+    with torch.cuda.device(dev):
+        capi.check(lib.cmdi_obstacle_seed(_ptr(x0), B, D, L, int(ld), _ptr(valid), _ptr(target), _ptr(mask), _ptr(mean),
+                                          _ptr(std), int(abs_3d), float(c_j), int(bool(foot_contact)), float(c_c),
+                                          _ptr(obstacles) if K else None, K, int(obstacle_joints), float(c_o),
+                                          grad.data_ptr(), _stream_ptr(dev)), "cmdi_obstacle_seed")
     return grad

@@ -270,7 +270,27 @@ typedef struct {
   int32_t stop_footcontact_at;
   const float* foot_contact_coef;  /* HOST array [T]: w_c[t] * foot_contact_weight * sqrt(alphas_cumprod[t]) / 2, fp32 */
   const uint8_t* foot_contact_mask; /* (B, L) bool bytes: the valid frames (y['mask']), or NULL */
+  /* Obstacle-avoidance guidance (all fields 0 / NULL: off): a fourth loss on the same update that keeps the joints of S
+     out of vertical cylinders, GMD's CondKeyLocationsWithSdf collision term.  With P as for joint guidance (joint_mean,
+     joint_std and joint_abs3d are read; joint_target / joint_mask only with joint_guidance on), obstacle k of sample b
+     o = (c_x, c_z, r) = obstacles[b][k] and S the joints of obstacle_joints,
+       L_o = sum over b of (1 / L) sum over f, j in S, k of m(b, f) max(r - |(P_j^x(b, f), P_j^z(b, f)) - (c_x, c_z)|, 0)
+       x0_tilde = x0_hat - ~M * (c_r(t) dL_r/dz + c_j(t) dL_j/dz + c_c(t) dL_c/dz + c_o(t) dL_o/dz)
+     with m = obstacle_mask (NULL: every frame valid) and c_o(t) = obstacle_coef[t] while t >= stop_obstacleguidance_at
+     (else 0).  The gradient is torch's subgradient: 0 at distance 0, -(P - c) / r at distance r.  Rows with r = 0 are
+     padding and contribute nothing; r < 0 and non-finite values are the caller's to refuse (the Python layer does).  A
+     step is guided when any of c_r, c_j, c_c, c_o applies.  The limits of joint guidance apply.  Pointers follow
+     host_buffers like the fields above. */
+  int32_t obstacle_guidance;
+  int32_t stop_obstacleguidance_at;
+  const float* obstacle_coef;   /* HOST array [T]: w_o[t] * obstacle_weight * sqrt(alphas_cumprod[t]) / 2, fp32 */
+  const float* obstacles;       /* (B, n_obstacles, 3) fp32 (c_x, c_z, r), or NULL when n_obstacles = 0 */
+  int32_t n_obstacles;          /* 0 .. CMDI_MAX_OBSTACLES */
+  uint32_t obstacle_joints;     /* bit j: joint j of the 22 is in S (nonzero, bits 0 .. 21; 1: the pelvis, as GMD) */
+  const uint8_t* obstacle_mask; /* (B, L) bool bytes: the valid frames (y['mask']), or NULL */
 } cmdi_sample_args;
+
+#define CMDI_MAX_OBSTACLES 16
 
 CMDI_API int cmdi_engine_create(const cmdi_model_cfg* cfg, int device, cmdi_engine** out);
 CMDI_API int cmdi_engine_destroy(cmdi_engine* e);
@@ -336,6 +356,25 @@ CMDI_API int cmdi_test_foot_contact_input_vjp(cmdi_engine* e, const cmdi_forward
 CMDI_API int cmdi_foot_contact_seed(const float* x0, int B, int D, int L, int ld, const uint8_t* valid, const float* target,
                                     const uint8_t* mask, const float* mean, const float* std, int abs_3d, float c_j, float c_c,
                                     float* grad, void* stream);
+/* cmdi_test_foot_contact_input_vjp with obstacle-avoidance guidance: grad receives the gradient of
+ * c_r L_r + c_j L_j + c_c L_c + c_o L_o through each pass (L_o as in cmdi_sample_args with obstacles (B, n_obstacles, 3)
+ * on the device and m = valid; L_c only with foot_contact, with the same m).  joint_target / joint_mask may both be NULL
+ * (no joint term); inpainted_motion / inpainting_mask may be NULL. */
+CMDI_API int cmdi_test_obstacle_input_vjp(cmdi_engine* e, const cmdi_forward_args* args, const float* inpainted_motion,
+                                          const uint8_t* inpainting_mask, float c_r, const float* joint_target,
+                                          const uint8_t* joint_mask, const float* joint_mean, const float* joint_std,
+                                          int joint_abs3d, float c_j, const uint8_t* valid, int foot_contact, float c_c,
+                                          const float* obstacles, int n_obstacles, uint32_t obstacle_joints, float c_o,
+                                          float* grad, void* stream);
+/* The obstacle guidance seed alone: grad = c_j dL_j/dx0 + c_c dL_c/dx0 + c_o dL_o/dx0 (L_j as cmdi_joint_guidance_seed,
+ * with target / mask both NULL: no joint term; L_c as cmdi_foot_contact_seed, only with foot_contact; L_o as in
+ * cmdi_sample_args, both with m = valid, (B, L) bytes or NULL).  Layouts as cmdi_joint_guidance_seed; channels >= 67 of
+ * grad are zero.  67 <= D (263 <= D with foot_contact), 1 <= L <= 256, 0 <= n_obstacles <= CMDI_MAX_OBSTACLES.  Device
+ * pointers. */
+CMDI_API int cmdi_obstacle_seed(const float* x0, int B, int D, int L, int ld, const uint8_t* valid, const float* target,
+                                const uint8_t* mask, const float* mean, const float* std, int abs_3d, float c_j,
+                                int foot_contact, float c_c, const float* obstacles, int n_obstacles,
+                                uint32_t obstacle_joints, float c_o, float* grad, void* stream);
 
 /* One MDM_UNET op of a pass, as cmdi_test_unet_ops hands it to its callback.  Views are device pointers into the engine's
  * own buffers, [rows, cols] with a row pitch; "level layout" is the halo layout of level l: nseq * (256 >> l) rows, the
