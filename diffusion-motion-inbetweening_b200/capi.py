@@ -77,7 +77,8 @@ class SampleArgs(Structure):
                 ("foot_contact", c_int32), ("stop_footcontact_at", c_int32), ("foot_contact_coef", POINTER(c_float)),
                 ("foot_contact_mask", c_void_p),
                 ("obstacle_guidance", c_int32), ("stop_obstacleguidance_at", c_int32), ("obstacle_coef", POINTER(c_float)),
-                ("obstacles", c_void_p), ("n_obstacles", c_int32), ("obstacle_joints", c_uint32), ("obstacle_mask", c_void_p)]
+                ("obstacles", c_void_p), ("n_obstacles", c_int32), ("obstacle_joints", c_uint32), ("obstacle_mask", c_void_p),
+                ("cfg_interval", c_int32), ("stop_cfg_at", c_int32), ("start_cfg_at", c_int32)]
 
 
 class UnetOpInfo(Structure):

@@ -104,7 +104,9 @@ struct GraphKey {
   int win_K, win_N;                // overlapping windows (the first frames live in device memory)
   int joint, joint_abs3d;          // joint-position guidance and its root representation (the joint seed's launch
                                    // arguments); its targets and coefficients live in device memory
-  int passes;                      // denoiser passes per evaluation (Passes::n): keyframe CFG adds one
+  int passes;                      // denoiser passes per evaluation (Passes::n): keyframe CFG adds one; 1 at a step
+                                   // outside the CFG interval (cmdi_sample_args.cfg_interval)
+  int passes2;                     // PLMS's first step: the passes of its second evaluation (at t - 1), else 0
   int contact;                     // foot-contact guidance (the joint seed's FC instance); joint: joint targets
   int obstacle, n_obstacles;       // obstacle-avoidance guidance (the obstacle seed instance) and its obstacles per sample
   uint32_t obstacle_joints;        // its joint set S (a launch argument of the seed)
@@ -115,7 +117,8 @@ struct GraphKey {
 // unconditional one; under keyframe CFG (cmdi_*_args.keyframe_scale) last the keyframe-free pass n (unconditional
 // embedding, x_t unblended, mask channels 0).  Keyframe CFG without CFG is the two-pass combine n + w_k (c - n), CFG's
 // arithmetic with w_k for the scale, so the step, seed and joint kernels see it as CFG; with CFG it is the three-pass
-// combine (n + w_k (u - n)) + s (c - u).
+// combine (n + w_k (u - n)) + s (c - u).  With a CFG interval (cmdi_sample_args.cfg_interval) the passes are chosen per
+// step: the call's passes inside the interval, the conditional pass alone (passes_of(e, false, false)) outside it.
 struct Passes {
   int n = 1;
   bool kf = false;                  // the last pass is keyframe-free
@@ -1660,15 +1663,16 @@ int first_step(const cmdi_engine* e, const cmdi_sample_args* a) {
 }
 
 // Kernel launches of one evaluation of a sampling step: the denoiser pass, a guided one's backward pass and joint seed,
-// the step kernel.
+// the step kernel.  The passes of an evaluation run as one batch, so the count does not depend on how many there are:
+// a step outside the CFG interval launches what a CFG step launches, over fewer rows.
 int launches_per_eval(const cmdi_engine* e, bool guided, const Guidance& g) {
   return launches_per_pass(e, guided) + 1 + (guided ? launches_per_backward(e) + (g.joint ? 1 : 0) : 0);
 }
 
 // What every sampler's step kernel reads and writes: the schedule, the device step counter, the combine inputs (model
-// output, CFG scale, keyframes, guidance gradient) and the state it advances in place.
-StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool guided) {
-  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
+// output, CFG scale, keyframes, guidance gradient) and the state it advances in place.  ps: the passes of the step's
+// evaluation, which decide the combine.
+StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, const Passes& ps, bool guided) {
   StepParams sp{};
   sp.tab = e->tab; sp.step_ptr = e->step_ctr; sp.B = a->batch; sp.L = e->L; sp.D = e->D; sp.D_pad = e->D_pad;
   sp.model_out = e->model_out; sp.cfg = ps.combine(); sp.text_scale = ps.scale; sp.keyframe_scale = ps.kf_scale;
@@ -1688,15 +1692,18 @@ StepParams step_params(const cmdi_engine* e, const cmdi_sample_args* a, bool gui
 // step is one evaluation and one Adams-Bashforth kernel.
 enum PlmsStep { kPlmsSteady = 0, kPlmsFirst = 1, kPlmsFirstAtZero = 2 };
 
-// The graph of `group` consecutive steps of this call's configuration with guidance `guided`; for PLMS, of one step of
-// kind `plms_kind` whose second evaluation has guidance `guided2` (both 0 for the other samplers).  The first step index
-// lives in device memory, so t0 stays 0.  PLMS draws no noise: its key leaves eta and the tape at zero.  The order is
-// the sampler's (order_of); the sampler field tells apart the samplers that read the same order field.
+// The graph of `group` consecutive steps of this call's configuration with guidance `guided` and `passes` denoiser
+// passes per evaluation; for PLMS, of one step of kind `plms_kind` whose second evaluation has guidance `guided2` and
+// `passes2` passes (0, 0 and 0 for the other samplers and the other step kinds).  A step outside the CFG interval has
+// one pass and no CFG: its graph is a plain step's.  The first step index lives in device memory, so t0 stays 0.  PLMS
+// draws no noise: its key leaves eta and the tape at zero.  The order is the sampler's (order_of); the sampler field
+// tells apart the samplers that read the same order field.
 // GraphKey is ordered by memcmp and has padding bytes, so the whole struct is zeroed before it is filled.
-GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int plms_kind, bool guided2) {
+GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int passes, int group, int plms_kind, bool guided2,
+                        int passes2) {
   GraphKey key;
   memset(&key, 0, sizeof(key));
-  key.B = a->batch; key.cfg = a->cfg != 0; key.sampler = a->sampler; key.impute = a->imputate != 0;
+  key.B = a->batch; key.cfg = a->cfg != 0 && passes > 1; key.sampler = a->sampler; key.impute = a->imputate != 0;
   key.stop_at = a->stop_imputation_at; key.has_cond = a->cond_emb != nullptr; key.uncond = a->uncond != 0;
   key.guided = guided; key.group = group;
   key.order = order_of(a);
@@ -1709,11 +1716,11 @@ GraphKey step_graph_key(const cmdi_sample_args* a, bool guided, int group, int p
   key.n_obstacles = key.obstacle ? a->n_obstacles : 0;
   key.obstacle_joints = key.obstacle ? a->obstacle_joints : 0u;
   key.joint_abs3d = (key.joint || key.contact || key.obstacle) && a->joint_abs3d != 0;
-  key.passes = 1 + (a->cfg ? 1 : 0) + (a->keyframe_scale ? 1 : 0);
+  key.passes = passes;
   if (a->sampler != CMDI_SAMPLER_PLMS) {
     key.eta = a->eta; key.tape = a->noise_tape; key.tape_mode = a->noise_tape != nullptr;
   }
-  key.plms_phase = plms_kind; key.guided2 = guided2;
+  key.plms_phase = plms_kind; key.guided2 = guided2; key.passes2 = passes2;
   return key;
 }
 
@@ -1891,6 +1898,24 @@ int check_sample_args(const cmdi_engine* e, const cmdi_sample_args* a) {
     return 1;
   }
   CKI(check_keyframe_cfg(e, B, a->cfg != 0, a->keyframe_scale, a->obs_x0, a->obs_mask));
+  if (a->cfg_interval != 0 && a->cfg_interval != 1) {
+    set_last_error("cfg_interval %d is neither 0 nor 1", a->cfg_interval);
+    return 1;
+  }
+  if (!a->cfg_interval && (a->stop_cfg_at || a->start_cfg_at)) {
+    set_last_error("%s is a cfg_interval field: it must be 0 when cfg_interval is 0",
+                   a->stop_cfg_at ? "stop_cfg_at" : "start_cfg_at");
+    return 1;
+  }
+  if (a->cfg_interval && !a->cfg && !a->keyframe_scale) {
+    set_last_error("cfg_interval limits classifier-free guidance to an interval of steps: it needs cfg or keyframe_scale");
+    return 1;
+  }
+  if (a->cfg_interval && a->stop_cfg_at > a->start_cfg_at) {
+    set_last_error("cfg_interval: stop_cfg_at %d > start_cfg_at %d (guidance runs at stop_cfg_at <= t <= start_cfg_at)",
+                   a->stop_cfg_at, a->start_cfg_at);
+    return 1;
+  }
   if ((a->imputate || a->recon_guidance) && (!a->inpainted_motion || !a->inpainting_mask)) {
     set_last_error("imputate / reconstruction_guidance need inpainted_motion and inpainting_mask (editing_util.py:330, :343)");
     return 1;
@@ -1993,7 +2018,8 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
   const bool plms = a->sampler == CMDI_SAMPLER_PLMS;
   const bool walk = sm.hist == History::kWalk;  // RePaint: p_sample steps and undo ops along a walk that revisits steps
   const int B = a->batch;
-  const Passes ps = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr);
+  // the passes of a step inside the CFG interval (every step without one) and outside it: the conditional pass alone
+  const Passes full = passes_of(e, a->cfg != 0, a->keyframe_scale != nullptr), one = passes_of(e, false, false);
   const bool host = a->host_buffers != 0;
   const bool contact = a->foot_contact != 0, obstacle = a->obstacle_guidance != 0;
   // the joint seed runs at guided evaluations: joint-position, foot-contact or obstacle guidance, in any combination
@@ -2104,7 +2130,8 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
     nsteps = (a->num_steps > 0 && a->num_steps < left) ? a->num_steps : left;
   }
   CKI(ensure_temb(e, s));
-  CKI(prepare_chain(e, ps.n * B));
+  CKI(prepare_chain(e, full.n * B));
+  if (a->cfg_interval) CKI(prepare_chain(e, B));
   int rc = 0;
 
   // ---- x_T (gaussian_diffusion.py:1245-1248) ----
@@ -2159,7 +2186,7 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
     e->launches += 2;
   }
   // ---- conditioning ----
-  CKI(stage_cond(e, a, ps, host, t0, s));
+  CKI(stage_cond(e, a, full, host, t0, s));
   // [2]: the history's first step (the call's for the single-step samplers), [3]: the call's first step, from which the
   // per-step draws of SDE-DPM-Solver++ are numbered (they differ on a resume)
   CK(launch_set_int(e->step_ctr + 2, hist_t0, s, t0));
@@ -2172,8 +2199,8 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
 
   const float* tape = a->noise_tape;
   const bool has_cond = a->cond_emb != nullptr;
-  // one evaluation: the denoiser pass and, for a guided one, its backward pass
-  auto enqueue_eval = [&](cudaStream_t st, bool guided) -> int {
+  // one evaluation of passes `ps`: the denoiser pass and, for a guided one, its backward pass
+  auto enqueue_eval = [&](cudaStream_t st, bool guided, const Passes& ps) -> int {
     CKI(run_denoiser(e, B, ps, a->uncond ? 0 : B, has_cond, e->d_tmap, st, nullptr, 1, guided ? &e->stash : nullptr));
     if (guided && g.joint) CKI(run_joint_seed(e, B, ps, g, st));
     if (guided) CKI(run_backward(e, B, ps, g, st));
@@ -2182,9 +2209,9 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
   // RePaint's two ops; the walk position and the draw number live in step_ctr
   RepaintParams rq{};
   rq.jump_length = a->repaint_jump_length; rq.jump_n_sample = a->repaint_jump_n_sample; rq.undo_coef = e->dpm_coef;
-  auto enqueue_step = [&](cudaStream_t st, bool guided) -> int {
-    CKI(enqueue_eval(st, guided));
-    StepParams sp = step_params(e, a, guided);
+  auto enqueue_step = [&](cudaStream_t st, bool guided, const Passes& ps) -> int {
+    CKI(enqueue_eval(st, guided, ps));
+    StepParams sp = step_params(e, a, ps, guided);
     sp.advance = 1; sp.sampler = a->sampler; sp.eta = a->eta;
     // first step index: step_ctr[2] (DDPM / DDIM) or step_ctr[3] (SDE-DPM-Solver++); graphs do not depend on it
     sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
@@ -2204,16 +2231,17 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
     }
     return 0;
   };
-  // one PLMS step of `kind` (PlmsStep): g1 / g2 = guidance of its first / second evaluation
-  auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2) -> int {
+  // one PLMS step of `kind` (PlmsStep): g1 / g2 = guidance and ps1 / ps2 = passes of its first / second evaluation
+  auto enqueue_plms = [&](cudaStream_t st, int kind, bool g1, bool g2, const Passes& ps1, const Passes& ps2) -> int {
     PlmsParams q{};
     q.order = a->plms_order; q.phase = kind == kPlmsSteady ? 0 : 1;
     q.eps_hist = e->hist; q.hist_stride = slot; q.x_keep = e->hist_keep;
     const bool guided[2] = {g1, g2};
+    const Passes* ps[2] = {&ps1, &ps2};
     for (int ev = 0; ev < (kind == kPlmsFirst ? 2 : 1); ++ev) {
-      CKI(enqueue_eval(st, guided[ev]));
+      CKI(enqueue_eval(st, guided[ev], *ps[ev]));
       if (ev == 1) q.phase = 2;
-      CK(launch_plms_step(step_params(e, a, guided[ev]), q, st));
+      CK(launch_plms_step(step_params(e, a, *ps[ev], guided[ev]), q, st));
     }
     return 0;
   };
@@ -2245,13 +2273,19 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
            (contact && t >= a->stop_footcontact_at) || (obstacle && t >= a->stop_obstacleguidance_at);
   };
   auto guided_at = [&](int k) { return guided_t(sm.ascends ? t0 + k : t0 - k); };
+  // the CFG interval (cmdi_sample_args.cfg_interval): CFG / keyframe CFG run while stop_cfg_at <= t <= start_cfg_at, the
+  // conditional pass alone elsewhere; tested where the guidance predicate is tested
+  auto passes_t = [&](int t) -> const Passes& {
+    return !a->cfg_interval || (t >= a->stop_cfg_at && t <= a->start_cfg_at) ? full : one;
+  };
+  auto passes_at = [&](int k) -> const Passes& { return passes_t(sm.ascends ? t0 + k : t0 - k); };
   // RePaint: the walk from its next op.  The undo ops that come before each of this call's nsteps denoise ops are one
-  // launch each; a denoise op is one evaluation and the step kernel, guided by its position, through the step graphs.
-  // A graph holds one denoise op.
+  // launch each; a denoise op is one evaluation and the step kernel, guided and given its passes by its position,
+  // through the step graphs.  A graph holds one denoise op.
   for (int k = 0; walk && k < nsteps; ++e->walk_next) {
     const WalkOp op = e->walk[e->walk_next];
     if (op.undo) {
-      StepParams sp = step_params(e, a, false);
+      StepParams sp = step_params(e, a, full, false);
       sp.noise_ref = tape; sp.tape_t0 = -1; sp.rng = e->rng;
       rq.phase = 1;
       CK(launch_repaint_step(sp, rq, s));
@@ -2259,24 +2293,31 @@ int sample_call(cmdi_engine* e, const cmdi_sample_args* a, float* out, cudaStrea
       continue;
     }
     const bool guided = guided_t(op.p);
+    const Passes& ps = passes_t(op.p);
     int ran = 0;
-    CKI(dispatch_steps(e, a, step_graph_key(a, guided, 1, 0, false), nsteps,
-                       [&](cudaStream_t st, int) { return enqueue_step(st, guided); }, launches_per_eval(e, guided, g), s, &ran));
+    CKI(dispatch_steps(e, a, step_graph_key(a, guided, ps.n, 1, 0, false, 0), nsteps,
+                       [&](cudaStream_t st, int) { return enqueue_step(st, guided, ps); }, launches_per_eval(e, guided, g), s,
+                       &ran));
     ++k;
   }
   for (int k = 0; !walk && k < nsteps;) {
     const bool guided = guided_at(k);
-    // PLMS: the kind of this step and the guidance of a first step's second evaluation, at t - 1
+    const Passes& ps = passes_at(k);
+    // PLMS: the kind of this step and the guidance and passes of a first step's second evaluation, at t - 1
     const int kind = !plms || e->hist_steps + k > 0 ? kPlmsSteady : (t0 - k > 0 ? kPlmsFirst : kPlmsFirstAtZero);
     const bool guided2 = kind == kPlmsFirst && guided_at(k + 1);
+    const Passes& ps2 = kind == kPlmsFirst ? passes_at(k + 1) : ps;
     auto enqueue = [&](cudaStream_t st, int steps) -> int {
-      if (plms) return enqueue_plms(st, kind, guided, guided2);
-      for (int i = 0; i < steps; ++i) CKI(enqueue_step(st, guided));
+      if (plms) return enqueue_plms(st, kind, guided, guided2, ps, ps2);
+      for (int i = 0; i < steps; ++i) CKI(enqueue_step(st, guided, ps));
       return 0;
     };
-    GraphKey key = step_graph_key(a, guided, 1, kind, guided2);
+    GraphKey key = step_graph_key(a, guided, ps.n, 1, kind, guided2, kind == kPlmsFirst ? ps2.n : 0);
     const bool dump_in_group = a->dump_xstart && dump_i < a->n_dump && a->dump_steps[dump_i] < k + group;
-    if (group > 1 && k + group <= nsteps && !dump_in_group && guided_at(k + group - 1) == guided) key.group = group;
+    // a group's steps share the guidance and the passes: it stops short of a guidance or CFG-interval boundary
+    bool uniform = group > 1 && k + group <= nsteps;
+    for (int i = 1; uniform && i < group; ++i) uniform = guided_at(k + i) == guided && &passes_at(k + i) == &ps;
+    if (uniform && !dump_in_group) key.group = group;
     const int64_t per_step = launches_per_eval(e, guided, g) + (kind == kPlmsFirst ? launches_per_eval(e, guided2, g) : 0);
     int ran = 0;
     CKI(dispatch_steps(e, a, key, nsteps, enqueue, per_step, s, &ran));

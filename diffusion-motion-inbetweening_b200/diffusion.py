@@ -303,6 +303,27 @@ def _obstacle_args(space, y, B, D, L, num_timesteps, sqrt_alphas_cumprod, window
                 joint_mean=space.mean.to(device), joint_std=space.std.to(device), joint_abs3d=bool(space.abs_3d))
 
 
+def _cfg_interval_args(y, guided: bool) -> dict:
+    """y['stop_cfg_at'] / y['start_cfg_at']: classifier-free guidance (CFG or keyframe CFG, `guided`) only at the steps
+    stop_cfg_at <= t <= start_cfg_at, the conditional pass alone at the others (cmdi_sample_args.cfg_interval).  Either
+    key may appear alone; with neither the loop is unchanged."""
+    keys = [k for k in ("stop_cfg_at", "start_cfg_at") if k in y.keys()]
+    if not keys:
+        return {}
+    for k in keys:
+        v = y[k]
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError(f"y[{k!r}] must be an int (a sampler step index), got {v!r}")
+    if not guided:
+        raise ValueError(f"y[{keys[0]!r}] limits classifier-free guidance to an interval of steps: the model must be a "
+                         "ClassifierFreeSampleModel or a KeyframeClassifierFreeSampleModel")
+    out = {k: int(y[k]) for k in keys}
+    if len(out) == 2 and out["stop_cfg_at"] > out["start_cfg_at"]:
+        raise ValueError(f"y['stop_cfg_at'] = {out['stop_cfg_at']} > y['start_cfg_at'] = {out['start_cfg_at']}: guidance "
+                         "runs while stop_cfg_at <= t <= start_cfg_at")
+    return out
+
+
 def _crop_windows(x: torch.Tensor, f0: List[int], F: int) -> torch.Tensor:
     """(B, ..., N) in the global layout -> (B * K, ..., F): row b * K + k holds frames [f0[k], f0[k] + F) of sample b."""
     idx = torch.tensor(f0, device=x.device)[:, None] + torch.arange(F, device=x.device)
@@ -422,6 +443,7 @@ class GaussianDiffusion:
         assert isinstance(shape, (tuple, list))
         inner, is_cfg = resolve_model(model)
         kf_cfg = is_keyframe_cfg(model)
+        cfg_interval = _cfg_interval_args(y, is_cfg or kf_cfg)
         if device is None:
             device = next(model.parameters()).device
         device = torch.device(device)
@@ -558,7 +580,7 @@ class GaussianDiffusion:
                       obs_x0=kf_obs, obs_mask=kf_mask, keyframe_scale=keyframe_scale,
                       y_mask=y_mask, imputate=imputate, stop_imputation_at=stop_at, inpainted_motion=obs,
                       inpainting_mask=mask, seed=seed, sample_offset=self.sample_offset, use_graph=self.use_graph,
-                      recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **joint, **rng_args)
+                      recon_guidance=recon, stop_recguidance_at=stop_rg, recon_coef=coef, **joint, **cfg_interval, **rng_args)
         if plms or dpm or sampler == capi.SAMPLER_DPM_SOLVER_SDE:
             common["plms_order" if plms else "dpm_order"] = int(order)
         if unipc:

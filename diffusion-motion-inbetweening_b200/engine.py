@@ -135,7 +135,8 @@ class Engine:
                foot_contact_coef: Optional[Sequence[float]] = None, foot_contact_mask: Optional[torch.Tensor] = None,
                obstacle_guidance: bool = False, stop_obstacleguidance_at: int = 0,
                obstacle_coef: Optional[Sequence[float]] = None, obstacles: Optional[torch.Tensor] = None,
-               obstacle_joints: int = 1, obstacle_mask: Optional[torch.Tensor] = None):
+               obstacle_joints: int = 1, obstacle_mask: Optional[torch.Tensor] = None,
+               stop_cfg_at: Optional[int] = None, start_cfg_at: Optional[int] = None):
         """The whole sampling loop in one native call. Tensors are in the reference layout (B, njoints, 1, nframes).
 
         host_buffers=False: every tensor must live on this engine's device; the result is a device tensor and the
@@ -172,6 +173,8 @@ class Engine:
         step, obstacles (batch, K, 3) fp32 (c_x, c_z, r) with K <= capi.MAX_OBSTACLES, obstacle_joints the bit mask of
         the joint set, obstacle_mask (batch, nframes) the valid frames or None; it reads joint_mean / joint_std /
         joint_abs3d, and joint_target / joint_mask only with joint_guidance.
+        stop_cfg_at / start_cfg_at: the CFG interval (cmdi_sample_args.cfg_interval): with cfg or keyframe_scale, either or
+        both limit guidance to the steps stop_cfg_at <= t <= start_cfg_at; the other steps run the conditional pass alone.
         """
         shape = (batch, self.njoints, 1, self.nframes)
         K = 0 if window_frames0 is None else len(window_frames0)
@@ -291,6 +294,12 @@ class Engine:
             a.obstacle_guidance, a.stop_obstacleguidance_at, a.obstacle_coef = 1, int(stop_obstacleguidance_at), ocoef_arr
             a.obstacles, a.n_obstacles, a.obstacle_joints = _ptr(obstacles), n_obstacles, int(obstacle_joints)
             a.obstacle_mask = _ptr(obstacle_mask)
+        if stop_cfg_at is not None or start_cfg_at is not None:
+            # a missing bound is one no step index reaches; the engine compares int32 step indices
+            lo, hi = -2 ** 31, 2 ** 31 - 1
+            a.cfg_interval = 1
+            a.stop_cfg_at = lo if stop_cfg_at is None else min(max(int(stop_cfg_at), lo), hi)
+            a.start_cfg_at = hi if start_cfg_at is None else min(max(int(start_cfg_at), lo), hi)
         with torch.cuda.device(self.device):
             capi.check(self.lib.cmdi_sample(self._h, ctypes.byref(a), out.data_ptr(), _stream_ptr(self.device)),
                        "cmdi_sample")

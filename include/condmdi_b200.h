@@ -288,6 +288,23 @@ typedef struct {
   int32_t n_obstacles;          /* 0 .. CMDI_MAX_OBSTACLES */
   uint32_t obstacle_joints;     /* bit j: joint j of the 22 is in S (nonzero, bits 0 .. 21; 1: the pelvis, as GMD) */
   const uint8_t* obstacle_mask; /* (B, L) bool bytes: the valid frames (y['mask']), or NULL */
+  /* CFG interval (all three 0: off; Kynkaenniemi et al. 2024, guidance in a limited interval): classifier-free guidance
+     (cfg) and keyframe CFG (keyframe_scale) run only at the steps t with stop_cfg_at <= t <= start_cfg_at, t the
+     sampler's step index (the spaced index under respacing, as for stop_recguidance_at).
+       - Inside the interval a step is exactly the step of the call without the interval.
+       - Outside it x0_hat is the conditional pass c alone, one pass of B rows, as the call with cfg = 0 and
+         keyframe_scale = NULL computes it: text and keyframe input are kept, uncond still makes it unconditional, and
+         text_scale / keyframe_scale are not read.  This is not u + 1 (c - u), which differs from c in fp32.
+       - Imputation, the guided steps' seeds and backward passes (the non-CFG seed form outside the interval) and the
+         window blend act on that x0_hat; the rule applies per step to every row, windows included.
+       - Where the interval is tested: PLMS's first step at t for its first evaluation and at t - 1 for its second (as
+         the guidance predicates); RePaint at each denoise op's position; DDIM inversion at each ascending step; UniPC's
+         corrector uses the x0 of the evaluation of its step, with that step's passes.
+     The call fails when cfg_interval is set without cfg and without keyframe_scale, when stop_cfg_at > start_cfg_at,
+     and when stop_cfg_at / start_cfg_at are set without cfg_interval. */
+  int32_t cfg_interval;         /* 1: on, 0: off */
+  int32_t stop_cfg_at;          /* guidance runs while t >= stop_cfg_at ... */
+  int32_t start_cfg_at;         /* ... and t <= start_cfg_at */
 } cmdi_sample_args;
 
 #define CMDI_MAX_OBSTACLES 16
